@@ -37,6 +37,8 @@ for _p in (ROOT, PKG):
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+HBM_PEAK_GBS, HBM_PEAK_SOURCE = 3350.0, "H100 SXM data sheet (HBM3 3.35 TB/s at up to 700 W), not measured"
+
 # name -> (schema, global rows, classes, trees, depth, maxBins, record dtype, reference site)
 WORKLOADS = {
     "kdd_full": ("kdd", 4898431, 5, 100, 16, 70, "f32", "BASELINE configs[1]"),
@@ -69,7 +71,11 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-sklearn", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed as DIR/<name>.npy (float64, <= 60 MiB in all)")
     a = ap.parse_args()
+    if a.impl == "reference" and a.dump_outputs and a.cpu_rows <= 0:
+        ap.error("--impl reference --dump-outputs needs --cpu-rows: without it the batch is sized by a timed probe")
     kind, rows, classes, trees, depth, bins, dtype, site = WORKLOADS[a.workload]
     a.kind, a.site = kind, site
     a.rows = a.rows or rows
@@ -135,7 +141,7 @@ class Workload:
                 "name": a.workload, "rows_per_gpu": rows_local, "global_rows": global_rows, "features": self.F, "classes": a.classes,
                 "num_trees": a.trees, "max_depth": a.depth, "max_bins": a.max_bins, "record_bytes": self.row_bytes,
                 "path": a.path, "parallelism": "rows sharded over %d GPU(s), per-level histogram exchange (NCCL)" % world,
-                "l2_policy": "inputs (%.0f MB records per GPU) larger than the 126 MB L2" % (rows_local * self.row_bytes / 1e6)}
+                "l2_policy": "inputs (%.0f MB records per GPU) larger than the 50 MB L2" % (rows_local * self.row_bytes / 1e6)}
 
 
 def forest_hash(ex):
@@ -147,6 +153,40 @@ def forest_hash(ex):
     internal = np.asarray(ex["is_leaf"]) == 0
     h.update(np.ascontiguousarray(np.asarray(ex["gain"], np.float64)[internal]).tobytes())
     return h.hexdigest()[:16]
+
+
+def forest_outputs(ex):
+    """the canonical forest export as float64 arrays (exact: every field fits 53 bits once the 64-bit left-set masks are split
+    into 32-bit halves; leaves carry no gain)."""
+    leaf = np.asarray(ex["is_leaf"]) != 0
+    cols = [np.asarray(ex[k], np.float64) for k in ("tree", "nid", "feat", "kind", "bin_thr", "is_leaf")]
+    cols.append(np.where(leaf, 0.0, np.asarray(ex["gain"], np.float64)))
+    mask = np.asarray(ex["mask"], np.uint64)
+    halves = np.stack([mask & np.uint64(0xFFFFFFFF), mask >> np.uint64(32)], axis=2).reshape(len(mask), -1)
+    return {"forest_nodes": np.stack(cols, axis=1), "forest_counts": np.asarray(ex["counts"], np.float64),
+            "forest_masks": halves.astype(np.float64)}
+
+
+def dump_outputs(path, arrays, budget=60 << 20):
+    """write each array as <path>/<name>.npy in float64.  The budget is shared out smallest array first; an array larger than
+    its share keeps a fixed, seeded sample of its rows (the same rows for the same shape on every run), whose indices go to
+    <name>_rows.npy."""
+    os.makedirs(path, exist_ok=True)
+    arrays = {k: np.atleast_1d(np.asarray(v, np.float64)) for k, v in arrays.items()}
+    left = len(arrays)
+    budget -= 2 * 128 * left                                     # .npy headers of the array and of its row indices
+    for name in sorted(arrays, key=lambda k: arrays[k].nbytes):
+        a, share = arrays[name], budget // left
+        row_bytes = a.nbytes // max(len(a), 1)
+        if a.nbytes > share:
+            keep = max(share // (row_bytes + 8), 1)
+            rows = np.sort(np.random.default_rng(2019).choice(len(a), keep, replace=False))
+            a = a[rows]
+            np.save(os.path.join(path, name + "_rows.npy"), rows.astype(np.float64))
+            budget -= rows.nbytes
+        np.save(os.path.join(path, name + ".npy"), a)
+        budget -= a.nbytes
+        left -= 1
 
 
 # ------------------------------------------------------------------------------------------------ CPU arm
@@ -244,7 +284,9 @@ def run_reference_stream(a, wl, threads):
         cpu_stream_pass(wl, plan, fo, meta, rec_np)
     t = []
     for _ in range(a.steps):
-        t0 = time.perf_counter(); cpu_stream_pass(wl, plan, fo, meta, rec_np); t.append(time.perf_counter() - t0)
+        t0 = time.perf_counter(); pred = cpu_stream_pass(wl, plan, fo, meta, rec_np); t.append(time.perf_counter() - t0)
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, {"prediction": pred})
     ms = 1e3 * sum(t) / len(t)
     v = a.cpu_rows / (ms / 1e3)
     line = {"impl": "reference", "metric": "flow-records/sec encode+predict (stream)", "value": v, "unit": "records/s", "n_gpus": a.gpus,
@@ -285,7 +327,9 @@ def run_reference(a):
         cpu_pass(wl, rec_np, dicts, a)
     t, f1, ph = [], 0.0, {}
     for _ in range(a.steps):
-        t0 = time.perf_counter(); f1, _, _ = cpu_pass(wl, rec_np, dicts, a, ph); t.append(time.perf_counter() - t0)
+        t0 = time.perf_counter(); f1, pred, ex = cpu_pass(wl, rec_np, dicts, a, ph); t.append(time.perf_counter() - t0)
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, dict(prediction=pred, macro_f1=f1, **forest_outputs(ex)))
     ms = 1e3 * sum(t) / len(t)
     v = a.cpu_rows / (ms / 1e3)
     cfg = wl.describe(world, a.rows, a.rows * world if a.scaling == "weak" else a.rows)
@@ -383,7 +427,7 @@ def step_resident(wl, rec, dicts, a, grp, keep=None):
     cm = bdist.all_reduce_sum_(fr.confusion_matrix(pred, yte.to(torch.float64), C), grp)   # R10
     f1 = fr.metrics_from_confusion(cm.cpu().numpy())["macroF1"]
     if keep is not None:
-        keep.update(model=model, pred=pred)
+        keep.update(model=model, pred=pred, raw=raw, prob=prob, cm=cm, f1=f1)
     return f1, nte, model.train_stats, model.n_nodes
 
 
@@ -441,14 +485,6 @@ def timed(fn, steps, warmup, grp):
     if grp is not None:
         dist.all_reduce(ms, op=dist.ReduceOp.MAX)
     return float(ms.item()) / steps, out
-
-
-def load_counters():
-    """per-kernel counters measured once with `ncu --set full` (profiles/): DRAM bytes per launch, LSU / issue utilisation."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))
-    except Exception:
-        return {}
 
 
 def main():
@@ -517,14 +553,13 @@ def main():
         if world > 1:
             dist.destroy_process_group()
         return
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, dict(prediction=keep["pred"].cpu().numpy(), raw_prediction=keep["raw"].cpu().numpy(),
+                                          probability=keep["prob"].cpu().numpy(), confusion=keep["cm"].cpu().numpy(),
+                                          macro_f1=keep["f1"], **forest_outputs(keep["model"].export())))
 
     # ---- roofline of the dominant kernel (CUDA events on the launching stream, inside the timed steps) -----
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak, peak_src = (peaks["hbm_gbs"], "measured (MEASURED_PEAKS.json)") if "hbm_gbs" in peaks else (6650.0, "fallback (B200_PROFILING.md)")
+    peak, peak_src = HBM_PEAK_GBS, HBM_PEAK_SOURCE
     kern = {k: {"launches_per_step": v[0] // a.steps, "ms_per_step": v[1] / a.steps, "share_of_step": v[1] / a.steps / ms_step}
             for k, v in prof.items() if not k.startswith("_")}
     ntr_rows = stats.get("rows", rows_local - nte)                                  # local train rows
@@ -550,21 +585,16 @@ def main():
     dom = max(kern, key=lambda k: kern[k]["ms_per_step"])
     d = kern[dom]
     avg_ms = d["ms_per_step"] / max(d["launches_per_step"], 1)
-    ctr = (load_counters().get(a.workload) or {}).get(dom) or {}       # counters exist for the workloads that were captured with ncu
-    traffic = ctr.get("dram_bytes_per_launch")
-    bound = {"route_hist_level": "lsu (shared-memory pipe: tile fills + tile reads + atomics), not hbm",
-             "hist_level": "lsu / record gather", "encode_bins": "issue + shared-memory (binary search), not hbm",
-             "predict": "l1 latency (divergent tree walk)", "encode": "hbm"}.get(dom, "hbm")
-    if dom == "route_hist_level" and ctr.get("lsu_pct") is not None and ctr["lsu_pct"] < 60:
-        bound = "gather latency (wide nodes: long-scoreboard stall, one record gather in flight per warp), not hbm"    # ncu: profiles/r02_route_hist_*_ncu.txt
+    bound = "expected, not profiled: " + {"route_hist_level": "lsu (shared-memory pipe: tile fills + tile reads + atomics), not hbm",
+                                          "hist_level": "lsu / record gather", "encode_bins": "issue + shared-memory (binary search), not hbm",
+                                          "predict": "l1 latency (divergent tree walk)", "encode": "hbm"}.get(dom, "hbm")
     roofline = {"kernel": dom, "bound": bound, "achieved": d.get("achieved_gbs"), "peak": peak, "unit": "GB/s",
-                "frac": d.get("frac_of_hbm_peak"), "traffic": traffic, "peak_source": peak_src,
-                "dram_frac": (traffic / (avg_ms * 1e-3) / 1e9 / peak) if traffic else None,
-                "lsu_pct": ctr.get("lsu_pct"), "issue_pct": ctr.get("issue_pct"), "counters_source": ctr.get("source"),
+                "frac": d.get("frac_of_hbm_peak"), "peak_source": peak_src,
+                "traffic": None, "dram_frac": None, "lsu_pct": None, "issue_pct": None,   # hardware counters are not captured here
                 "launches_per_step": d["launches_per_step"], "avg_launch_ms": avg_ms, "share_of_step": d["share_of_step"],
                 "note": "achieved = SURVEY 8(d) algorithmic bytes (per level and TRAINING row: F + 1 + 5*T) / CUDA-event kernel time "
-                        "inside the timed steps; after row de-duplication the kernel works on (unique record, tree) entries and is "
-                        "bound by the SM's load/store pipe, so dram_frac (measured DRAM bytes per launch, ncu) is the HBM view"}
+                        "inside the timed steps; after row de-duplication the kernel works on (unique record, tree) entries, so this "
+                        "is not its DRAM traffic"}
 
     # ---- CPU baseline + bit parity at the benched size -------------------------------------------------
     cpu = None
@@ -684,12 +714,9 @@ def run_stream(a, wl, dev, grp, world, rank, local):
         if world > 1:
             dist.destroy_process_group()
         return
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    peak, peak_src = (peaks["hbm_gbs"], "measured (MEASURED_PEAKS.json)") if "hbm_gbs" in peaks else (6650.0, "fallback (B200_PROFILING.md)")
+    if a.dump_outputs:
+        dump_outputs(a.dump_outputs, {"prediction": pred.cpu().numpy()})
+    peak, peak_src = HBM_PEAK_GBS, HBM_PEAK_SOURCE
     kern = {k: {"launches_per_step": v[0] // a.steps, "ms_per_step": v[1] / a.steps, "share_of_step": v[1] / a.steps / ms_step}
             for k, v in prof.items() if not k.startswith("_")}
     alg = {"encode_bins": rows * (wl.row_bytes + wl.F + 1), "predict": rows * (wl.F + 8)}
@@ -709,9 +736,9 @@ def run_stream(a, wl, dev, grp, world, rank, local):
                        "name": "stream", "rows_per_gpu": rows, "global_rows": rows * world, "rows_streamed_total": rows * world * a.steps,
                        "features": 41, "classes": a.classes, "num_trees": a.trees, "max_depth": a.depth, "max_bins": a.max_bins,
                        "parallelism": "row-sharded stream over %d GPU(s), no collective" % world,
-                       "l2_policy": "inputs (%.0f MB per step) larger than the 126 MB L2" % (rows * wl.row_bytes / 1e6)},
+                       "l2_policy": "inputs (%.0f MB per step) larger than the 50 MB L2" % (rows * wl.row_bytes / 1e6)},
             "clocks": sampler.summary() if sampler else None, "e2e": e2e, "gpu_launches": launches,
-            "roofline": {"kernel": "step (encode_bins + dedup + predict + gather)", "bound": "hbm for the encode; the tree walk is latency-bound",
+            "roofline": {"kernel": "step (encode_bins + dedup + predict + gather)", "bound": "expected, not profiled: hbm for the encode; the tree walk is latency-bound",
                          "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": None, "peak_source": peak_src,
                          "dominant_kernel": dom, "note": "achieved = (record bytes in + 8 B prediction out) x rows / step time, per GPU"},
             "kernels": kern, "cpu_baseline": None}

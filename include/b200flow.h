@@ -1,5 +1,5 @@
 /*
- * b200flow.h — C ABI of libb200flow.so: the B200 (sm_100a) hot path of the
+ * b200flow.h — C ABI of libb200flow.so: the H100 (sm_90a) hot path of the
  * flow-classification pipeline that biagiom/spark-network-traffic-classifier
  * drives through pyspark.ml.
  *
@@ -277,7 +277,7 @@ int b200flow_partition_level(const uint8_t* tp, int32_t tp_stride,
 /* R7 (inside fit: kdd99.py:79, cicids17.py:83) fused with the row routing: partition_level(L) + hist_level(L+1) in ONE pass — every entry's TreePoint
  * record is gathered once, routed by its parent's split and accumulated into its CHILD's histogram
  * (hist_next[child_slot][j][bin][class], child feature subsets in subset_next, caller zeroes hist_next and
- * cursors).  The kernel is persistent (148 x k CTAs); each warp gathers the records of its entries with
+ * cursors).  The kernel is persistent (132 x k CTAs); each warp gathers the records of its entries with
  * asynchronous copies into a private shared-memory tile and there is no CTA barrier except when the parent slot
  * changes.
  * b200flow_route_hist_config() picks the launch shape for a level shape (host-only, no device needed): it returns

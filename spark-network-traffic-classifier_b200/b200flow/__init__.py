@@ -1,4 +1,4 @@
-"""b200flow — Python host layer over libb200flow.so (hand-written sm_100a kernels, include/b200flow.h).
+"""b200flow — Python host layer over libb200flow.so (hand-written sm_90a kernels, include/b200flow.h).
 
 Only the hot path of biagiom/spark-network-traffic-classifier lives here: fused encode
 (StringIndexer + OneHotEncoder + StandardScaler + VectorAssembler) and the RandomForest /

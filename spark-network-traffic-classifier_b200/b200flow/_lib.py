@@ -28,7 +28,7 @@ class B200FlowError(RuntimeError):
 
 
 class UnsupportedParamError(B200FlowError, ValueError):
-    """a parameter value MLlib accepts but the B200 path does not implement (entropy impurity, maxBins > 256, ...): a
+    """a parameter value MLlib accepts but the CUDA path does not implement (entropy impurity, maxBins > 256, ...): a
     ValueError, so the pyspark shim reports it as IllegalArgumentException; CUDA/runtime failures stay B200FlowError."""
 
 

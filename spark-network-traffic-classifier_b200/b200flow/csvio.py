@@ -1,6 +1,6 @@
 """CSV files -> AoS flow records on the device (SURVEY.md 8f-3).
 
-`spark.read.csv(path_or_glob, inferSchema=True, header=...)` (kdd99.py:25, cicids17.py:19-20) made B200-native: the host only
+`spark.read.csv(path_or_glob, inferSchema=True, header=...)` (kdd99.py:25, cicids17.py:19-20) made GPU-native: the host only
 reads the files' BYTES into pinned memory and copies them to the GPU; the line index, Spark's per-column type inference, the
 string dictionaries and the text -> int32 / float64 / dictionary-code conversion are CUDA kernels (csrc/csv.cu), with Java's
 correctly rounded parseDouble semantics (csrc/csv_number.h).  The host touches text again only for the header line and to

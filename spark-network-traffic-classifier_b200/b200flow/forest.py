@@ -46,13 +46,12 @@ def profile_totals():
 
 
 ENTRY_BOUND_BYTES = 8 << 30        # the two entry buffers are sized by the bound T * U (no host read of the exact count) up to this many bytes
-HIST_BUDGET_BYTES = int(_os.environ.get("B200FLOW_HIST_BUDGET_GB", "24")) << 30   # cap of one level's histogram buffer (MLlib: maxMemoryInMB); beyond it the level is processed in node groups by the unfused kernels
+HIST_BUDGET_BYTES = int(_os.environ.get("B200FLOW_HIST_BUDGET_GB", "10")) << 30   # cap of one level's histogram buffer (MLlib: maxMemoryInMB; 10 GB of an 80 GB H100); beyond it the level is processed in node groups by the unfused kernels
 # Multi-GPU: level histograms of at least this many bytes are REDUCE-SCATTERED by node (each rank then scores only its own
 # nodes and the 64-byte split records are all-gathered) instead of all-reduced: half the NVLink bytes, 1/world of the scoring.
 # Smaller levels are latency-bound and keep the single all-reduce.
 RS_MIN_BYTES = int(_os.environ.get("B200FLOW_RS_MIN_BYTES", str(8 << 20)))
 RS_CHUNKS = int(_os.environ.get("B200FLOW_RS_CHUNKS", "1"))   # slot ranges per level whose reduce-scatter overlaps the scoring of the previous range
-# (measured on 2 x B200, KDD99-full weak scaling: 1 chunk 32.8 ms/step, 4 chunks 37.8 — the extra collectives cost more than the overlap hides)
 
 
 @dataclass
@@ -72,7 +71,7 @@ class ForestParams:
 
 def tp_stride(F):
     """TreePoint record stride: F bins + label, padded to whole 64-byte HBM bursts so that one random
-    record gather costs exactly ceil((F+1)/64) bursts (profiles/: both level kernels are gather-bound)."""
+    record gather costs exactly ceil((F+1)/64) bursts (both level kernels gather records at random)."""
     return (F + 1 + 63) // 64 * 64
 
 
@@ -372,7 +371,7 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
     _lib.require_cuda()
     p = params
     if p.impurity != "gini":
-        raise UnsupportedParamError("impurity=%r: only 'gini' is implemented on the B200 path" % p.impurity)
+        raise UnsupportedParamError("impurity=%r: only 'gini' is implemented on the CUDA path" % p.impurity)
     if not (0 <= p.max_depth <= 30):
         raise ValueError("maxDepth must be in [0, 30], got %d" % p.max_depth)
     dev = src.device

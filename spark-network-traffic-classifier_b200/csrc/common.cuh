@@ -1,4 +1,4 @@
-// common.cuh — shared device helpers for libb200flow (sm_100a only).
+// common.cuh — shared device helpers for libb200flow (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -16,7 +16,7 @@ int check_launch(const char* what);
         if (!(cond)) { b200flow::set_error(__VA_ARGS__); return B200FLOW_ERR_ARG; } \
     } while (0)
 
-constexpr int kNumSMs = 148;   // B200: 2 dies x 74 SMs; grids are sized in multiples of this
+constexpr int kNumSMs = 132;   // H100 SXM; grids are sized in multiples of this
 
 // ------------------------------------------------------------------ Philox4x32-10
 // Counter-based RNG (DESIGN.md §RNG): key = (lo32(seed) ^ purpose, hi32(seed)).
@@ -148,7 +148,7 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
 // read-once / write-once 64-bit accesses marked evict-first in the L2: the bagged-entry stream (1 GB per level) passes through
-// once per level and must not push the re-used TreePoint records (61 MB, gathered at random) out of the 126 MB L2
+// once per level and must not push the re-used TreePoint records (61 MB on KDD99-full, gathered at random) out of the 50 MB L2
 __device__ __forceinline__ uint2 ld_evict_first_u2(const void* p) {
     uint2 r;
     asm volatile("ld.global.cs.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));      // .cs = cache-streaming: evict-first

@@ -507,7 +507,7 @@ __global__ void __launch_bounds__(256) partition_level_kernel(
 }
 
 // ------------------------------------------------------------------ fused row routing + next-level histogram
-// Persistent CTAs (a multiple of 148), each owning a contiguous range of chunks (<= CH entries of one SPLIT parent).
+// Persistent CTAs (a multiple of 132), each owning a contiguous range of chunks (<= CH entries of one SPLIT parent).
 // Software pipeline per WARP, all copies asynchronous (LDGSTS, no register staging):
 //     entries(t+2)  -->  record gather(t+1)  -->  route + histogram(t)
 //   * the gather brings each entry's 64-byte-aligned TreePoint record (one HBM burst) into a shared-memory tile,
@@ -520,9 +520,9 @@ __global__ void __launch_bounds__(256) partition_level_kernel(
 //     reservation per warp step and side); the two child histograms stay in shared memory while consecutive chunks
 //     belong to the same parent and are flushed with sparse global REDs when the parent changes.
 // Launch shapes (route_cfg below): NW warps per CTA x KS entries per lane and step; a chunk is NW * KS * 32 entries.
-// Narrow nodes (KDD 5-class: 2 x 9.8 KB of child histograms) run 4 CTAs x 8 warps x 64 entries per SM; wide nodes
+// Narrow nodes (KDD 5-class: 2 x 9.8 KB of child histograms) run 3 CTAs x 8 warps x 64 entries per SM; wide nodes
 // (KDD 23-class: 2 x 45 KB, CICIDS 15-class: 2 x 42 KB) trade tile bytes for histogram bytes — 2 CTAs x 16 warps x 32
-// entries, or 1 CTA x 32 warps — so that the SM still holds 32 warps.  Nodes whose two child histograms exceed shared
+// entries, or 1 CTA x 32 warps.  Nodes whose two child histograms exceed shared
 // memory altogether (DecisionTree: every feature of every node) are processed in FEATURE PASSES: pass p accumulates
 // subset positions [j0, j0 + m_pass) and only pass 0 routes.
 #ifndef B2F_EVICT_FIRST
@@ -569,7 +569,7 @@ struct RouteArgs {
 //     route + histogram of step t from the tile
 // CTA-wide barriers happen only when the parent slot changes (flush + re-zero of the two child histograms).
 template <int M, int NW, int KS, int MERGE>   // MERGE: 0 plain shared atomics (runtime m), 1 top-group merge, 2 rotated features
-__global__ void __launch_bounds__(NW * 32, NW == 8 ? 4 : (NW == 16 ? 2 : 1)) route_hist_level_kernel(const RouteArgs a) {
+__global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) route_hist_level_kernel(const RouteArgs a) {
     extern __shared__ __align__(16) uint32_t sm_u32[];
     constexpr int kThreads = NW * 32, kSub = KS * 32;
     const int m = M > 0 ? M : a.m;
@@ -608,8 +608,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 4 : (NW == 16 ? 2 : 1)) rou
     };
     // The tile is entry-major ([kSub entries][nq quads]) and its kSub * nq 16-byte chunks are copied in linear order, lane
     // after lane: neighbouring lanes fetch neighbouring quads of the SAME record (same 32-byte sector) into neighbouring
-    // shared addresses, which the L1 fills with fewer wavefronts than one scattered 16-byte fill per lane (ncu source page:
-    // 23 instead of 31 wavefronts per LDGSTS).
+    // shared addresses, which the L1 can fill with fewer wavefronts than one scattered 16-byte fill per lane.
     const uint32_t inv_nq = (1u << 20) / (uint32_t)nq + 1u;     // c / nq == (c * inv_nq) >> 20 for c * nq < 2^20
     auto issue_gather = [&](const int4& d, const b2f_entry* x) {
         const int cn = count_of(d);
@@ -701,9 +700,8 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 4 : (NW == 16 ? 2 : 1)) rou
                     if (M > 0 && MERGE == 1) {
                         // top-group merge: per feature, the lanes that share the first active lane's (bin, label, child) counter are
                         // summed with ONE redux over the whole active mask (the others contribute 0: no divergence) and issue one
-                        // shared atomic; the other lanes add alone.  Measured and dropped: whole-key match.any merge (46 ms per fit
-                        // vs 20.6), per-feature match.any merge (80 ms: a redux per distinct mask serialises), further top-group
-                        // rounds (27 / 36 ms).
+                        // shared atomic; the other lanes add alone.  A per-feature match.any merge would issue one redux per
+                        // distinct mask, which serialises.
                         const uint32_t tag = (lab << 8) | ((uint32_t)side << 16);
 #pragma unroll
                         for (int j = 0; j < M; ++j) {
@@ -762,18 +760,18 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 4 : (NW == 16 ? 2 : 1)) rou
 
 // ---- launch shape of the fused kernel
 struct RouteCfg { int nw, ks, m_pass, per_sm; size_t smem; };
-constexpr size_t kSmemPerSM = 227 * 1024;                  // 232,448 B usable per SM on sm_100
+constexpr size_t kSmemPerSM = 227 * 1024;                  // 232,448 B usable per block on sm_90
 constexpr size_t kSmemCtaOverhead = 1024 + 128;            // driver reservation per CTA + the kernel's static shared memory
 
 static size_t route_hist_smem(int F, int mp, int n_bins, int C, int nw, int ks) {
     return (size_t)nw * ks * 32 * route_pitch(F) * kGran + 2 * (size_t)mp * n_bins * C * 4 + 2 * (size_t)mp * 4 + 64;
 }
-static int route_max_ctas(int nw) { return nw == 8 ? 4 : (nw == 16 ? 2 : 1); }   // __launch_bounds__
+static int route_max_ctas(int nw) { return nw == 8 ? 3 : (nw == 16 ? 2 : 1); }   // __launch_bounds__ (8 warps: 3 CTAs, 85 registers)
 
 // Picks (warps per CTA, entries per lane, features per pass): the fewest passes first (every extra pass gathers the
-// records again), then the most entries in flight per SM (resident warps x entries per lane; measured with the rotated
-// update, CICIDS 6-class: 8x2 with 24 warps 0.87 ms per level vs 8x1 with 32 warps 1.05), then the most resident warps,
-// then the smallest chunk.
+// records again), then the most entries in flight per SM (resident warps x entries per lane) up to 48, then the smallest
+// chunk, then the most resident warps.  On an H100 (KDD99-full, level kernel per fit) 8x2 with 3 CTAs per SM took 26.6 ms,
+// 16x2 with 64 entries in flight 30.5, 8x1 28.3, 16x1 28.4, and 8x2 with 4 CTAs per SM (64 registers: spills) 35.0.
 static bool route_cfg(int F, int m, int n_bins, int C, RouteCfg* out) {
     static const int cand[5][2] = {{8, 2}, {8, 1}, {16, 2}, {16, 1}, {32, 1}};
     int force_nw = 0, force_ks = 0;                         // tuning / test knob, read per call: B200FLOW_ROUTE_SHAPE=<warps>x<entries per lane>
@@ -794,7 +792,7 @@ static bool route_cfg(int F, int m, int n_bins, int C, RouteCfg* out) {
         int per_sm = (int)(kSmemPerSM / (smem + kSmemCtaOverhead));
         if (per_sm > route_max_ctas(nw)) per_sm = route_max_ctas(nw);
         const int warps = per_sm * nw > 32 ? 32 : per_sm * nw;
-        const long key = ((long)(warps * ks) << 20) + ((long)warps << 10) + (1023 - nw * ks);
+        const long key = ((long)(warps * ks < 48 ? warps * ks : 48) << 20) + ((long)(1023 - nw * ks) << 10) + warps;
         if (key > best_key) { best_key = key; best = i; }
     }
     if (best < 0) return false;
@@ -806,7 +804,7 @@ static bool route_cfg(int F, int m, int n_bins, int C, RouteCfg* out) {
 }
 
 // histogram update of the fused kernel: 2 = rotated features (default), 1 = top-group merge, 0 = generic runtime loop.
-// Tuning knob B200FLOW_ROUTE_VARIANT, read per call: "merge" / "generic" (KDD-full, route per fit: rotated 14.8 ms, merge 17.3 ms).
+// Tuning knob B200FLOW_ROUTE_VARIANT, read per call: "merge" / "generic".
 static int route_hist_variant() {
     const char* e = getenv("B200FLOW_ROUTE_VARIANT");
     if (e && !strcmp(e, "merge")) return 1;
@@ -1011,7 +1009,7 @@ extern "C" int b200flow_route_hist_level(const uint8_t* tp, int32_t tp_stride, i
     a.seg_begin = seg_begin; a.seg_end = seg_end; a.split = split; a.child_slot = child_slot; a.cursors = cursors;
     a.subset_next = subset_next; a.m_total = m; a.n_bins = n_bins; a.C = C; a.hist_next = hist_next;
     static int waves = -1;                                    // CTAs per resident slot: > 1 lets the block scheduler even out the tail
-    if (waves < 0) { const char* e = getenv("B200FLOW_ROUTE_WAVES"); waves = e ? atoi(e) : 2; if (waves < 1) waves = 1; }   // measured per fit: 17.7 (1), 17.4 (2-6), 17.6 ms (8)
+    if (waves < 0) { const char* e = getenv("B200FLOW_ROUTE_WAVES"); waves = e ? atoi(e) : 2; if (waves < 1) waves = 1; }
     int merge = route_hist_variant();
     if (merge == 1 && C > 128) merge = 2;                      // the merge key packs the label into 8 bits
     for (int j0 = 0, pass = 0; j0 < m; j0 += cfg.m_pass, ++pass) {

@@ -16,8 +16,7 @@ namespace b200flow {
 // votes accumulate in fp64, in tree order, in smem ([class*blockDim + t]).
 //
 // What bounds the walk is the L1: below the first few levels every lane of a warp is at a different node, so each level costs
-// 32 separate sector requests per warp and row (ncu: issue 36 %, LSU 29 %, long-scoreboard stalls — the t-stage serialises
-// them).  The top `top_levels` levels of the CURRENT tree (2^K - 1 nodes, heap-indexed by MLlib's node id) are therefore
+// 32 separate sector requests per warp and row (long-scoreboard stalls: the t-stage serialises them).  The top `top_levels` levels of the CURRENT tree (2^K - 1 nodes, heap-indexed by MLlib's node id) are therefore
 // staged in shared memory, double-buffered with cp.async one tree ahead: a scattered LDS.128 costs a handful of bank
 // wavefronts instead of 32 tag lookups, and only the levels below K go to the L1/L2.
 

@@ -325,7 +325,7 @@ __global__ void __launch_bounds__(256) dedup_min_kernel(int64_t n, const int32_t
     const int sl = i < n ? slot_of[i] : -1 - lane;
     const uint32_t g = __match_any_sync(0xffffffffu, sl);
     // a plain read first: once a small row index sits in the slot, later (larger) candidates skip the atomic altogether, so the
-    // hot slots (smurf, neptune) take a few hundred atomics instead of one per warp (ncu: 0.24 ms at 1 % issue before)
+    // hot slots (smurf, neptune) take a few hundred atomics instead of one per warp
     if (i < n && (int)(__ffs(g) - 1) == lane && (int)i < *(volatile const int32_t*)&minrow[sl]) atomicMin(&minrow[sl], (int)i);
 }
 __global__ void __launch_bounds__(256) dedup_flag_kernel(int64_t n, const int32_t* __restrict__ slot_of, const int32_t* __restrict__ minrow,
@@ -354,7 +354,7 @@ constexpr int kGroupTab = 256;          // per-CTA direct-mapped (unique id -> p
 __global__ void __launch_bounds__(256) group_count_kernel(const int32_t* __restrict__ uid, int64_t n, int32_t* gsize) {
     // persistent CTAs; the warp leaders of a duplicate group add into a small shared-memory cache keyed by the unique id, and
     // only evictions and the final flush touch global memory: a hot group (a third of KDD99 is one smurf record) costs one global
-    // atomic per CTA instead of one per warp (ncu: 0.28 ms of pure same-address atomics before)
+    // atomic per CTA instead of one per warp
     __shared__ int tab_key[kGroupTab];
     __shared__ int tab_cnt[kGroupTab];
     for (int k = threadIdx.x; k < kGroupTab; k += blockDim.x) { tab_key[k] = -1; tab_cnt[k] = 0; }
@@ -415,7 +415,7 @@ __global__ void __launch_bounds__(256) bag_weights_kernel(uint64_t seed, int T, 
     // Fast path for the hot duplicate groups: with the rows grouped (perm given, uid sorted along the positions) a CTA whose first
     // and last position carry the same unique id lies entirely inside ONE group — the smurf and neptune floods span thousands of
     // CTAs.  Its 1024 weights per tree are summed in registers, by shuffles and through shared memory, and ONE global RED per tree
-    // leaves the CTA (31 x fewer same-address REDs than one per 32-position run; ncu: bag_weights was bound by exactly those).
+    // leaves the CTA (31 x fewer same-address REDs than one per 32-position run).
     {
         const int64_t p_first = (int64_t)blockIdx.x * kBagBlockRows, p_last = min(n, p_first + kBagBlockRows) - 1;
         if (perm && uid && cdf && p_last - p_first + 1 == kBagBlockRows && uid[p_first] == uid[p_last]) {

@@ -88,7 +88,7 @@ class _TreeClassifierBase(Estimator, _TreeParams):
         imp = str(self.getOrDefault("impurity")).lower()
         if imp not in ("gini", "entropy"):
             raise IllegalArgumentException("impurity must be gini or entropy, got %r" % imp)
-        if imp == "entropy":       # log is not bit-reproducible between libm and CUDA: not offered on the B200 path (DESIGN.md)
+        if imp == "entropy":       # log is not bit-reproducible between libm and CUDA: not offered on the CUDA path (DESIGN.md)
             raise IllegalArgumentException("impurity='entropy' is not supported by the b200flow tree trainer; use 'gini' "
                                            "(the reference scripts take the default, kdd99.py:64 / cicids17.py:68)")
         seed = self.getOrDefault("seed")

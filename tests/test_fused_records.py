@@ -1,4 +1,4 @@
-"""Round-2 paths: the fused level kernel on the reference scripts' own forest shapes (KDD 23-class, CICIDS 14/15-class,
+"""The fused level kernel on the reference scripts' own forest shapes (KDD 23-class, CICIDS 14/15-class,
 DecisionTree feature passes — kdd99.py:61,64, cicids17.py:65,68) and the fused encode -> bins path (raw records -> TreePoint
 bins without the dense matrix; SURVEY.md 8d).  Every GPU result is compared with the CPU oracle through the C ABI."""
 import numpy as np
@@ -21,7 +21,7 @@ def test_route_hist_config_covers_the_reference_scripts_shapes():
         assert cfg is not None, shape
         chunk, m_pass = cfg
         assert m_pass == shape[1] and chunk in (256, 512, 1024)
-    # the measured optima (DESIGN.md 3): 8x2 for the narrow nodes, 16x1 / 32x1 for the wide ones
+    # the launch shapes measured fastest on the H100 (DESIGN.md 3): 8x2 for the narrow nodes, 16x1 / 32x1 for the wide ones
     assert [_lib.route_hist_config(*s)[0] for s in [(41, 7, 70, 5), (78, 9, 78, 6), (41, 7, 70, 23), (78, 9, 78, 15)]] == [512, 512, 512, 1024]
     # DecisionTree: every feature in every node -> feature passes, the first of which routes
     chunk, m_pass = _lib.route_hist_config(41, 41, 70, 23)

@@ -1,5 +1,5 @@
 #!/bin/bash
-# round-2 measurement suite on ONE B200: tests, one bench line per BASELINE config, ncu launch list + full captures
+# measurement suite on ONE H100: tests, one bench line per BASELINE config, ncu launch list + full captures
 O=gpurun_out/final; mkdir -p $O
 nvidia-smi --query-gpu=name,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active --format=csv > $O/smi.txt 2>&1
 timeout 900 python -m pytest tests -m gpu -q > $O/gpu_pytest.log 2>&1; echo "pytest rc=$?" >> $O/gpu_pytest.log; tail -3 $O/gpu_pytest.log
@@ -18,7 +18,7 @@ timeout 200 python tools/timeline.py --workload kdd_full > $O/timeline_kdd_full.
 timeout 200 python tools/timeline.py --workload kdd_script > $O/timeline_kdd_script.txt 2>&1
 # launch list of the bench command (serialised, cold-cache: compare shares)
 timeout 600 ncu --metrics gpu__time_duration.sum --clock-control none -c 1200 --csv --log-file $O/launches_kdd_full.csv python bench.py --steps 2 --warmup 1 --no-cpu-baseline --no-e2e > $O/launches_kdd_full.log 2>&1
-# full ncu captures (route_hist_level per workload, misc kernels, encode, csv) are taken separately: see profiles/r02_*_ncu.txt headers
+# full ncu captures (route_hist_level per workload, misc kernels, encode, csv) are taken separately (tools/summarize_profiles.py)
 timeout 300 python tools/bench_csv.py 1000000 > $O/csv_bench.json 2> $O/csv_bench.err
 python - <<'PY'
 import json,glob

@@ -1,5 +1,5 @@
 #!/bin/bash
-# final validation on ONE B200: GPU test-suite, smoke, one headline line, per-level profile
+# final validation on ONE H100: GPU test-suite, smoke, one headline line, per-level profile
 O=gpurun_out/final; mkdir -p $O
 timeout 500 python -m pytest tests -m gpu -q > $O/gpu_pytest.log 2>&1; echo "pytest rc=$?" >> $O/gpu_pytest.log; tail -3 $O/gpu_pytest.log
 timeout 100 python __graft_entry__.py smoke > $O/smoke.log 2>&1; tail -1 $O/smoke.log

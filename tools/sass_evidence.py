@@ -61,7 +61,7 @@ def ptxas():
         if not f.endswith(".ptxas.log"):
             continue
         txt = open(os.path.join(BUILD, f)).read()
-        for m in re.finditer(r"Compiling entry function '(\S+)' for 'sm_100a'\n.*?\n\s+(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n"
+        for m in re.finditer(r"Compiling entry function '(\S+)' for 'sm_90a'\n.*?\n\s+(\d+) bytes stack frame, (\d+) bytes spill stores, (\d+) bytes spill loads\n"
                              r"ptxas info\s+: Used (\d+) registers(?:, used \d+ barriers)?(?:, (\d+) bytes smem)?", txt):
             rows.append((m.group(1), m.group(5), m.group(3), m.group(4), m.group(6) or "0"))
     names = demangle([r[0] for r in rows])
@@ -69,8 +69,9 @@ def ptxas():
 
 
 if __name__ == "__main__":
+    os.makedirs(os.path.join(ROOT, "profiles"), exist_ok=True)
     with open(os.path.join(ROOT, "profiles", "r02_sass_evidence.txt"), "w") as f:
-        f.write("# SASS evidence (cuobjdump -sass libb200flow.so, sm_100a), round-2 final code: static instruction counts per kernel for the mnemonics that matter (tools/sass_evidence.py)\n")
+        f.write("# SASS evidence (cuobjdump -sass libb200flow.so, sm_90a): static instruction counts per kernel for the mnemonics that matter (tools/sass_evidence.py)\n")
         f.write("# UBLKCP = cp.async.bulk (TMA 1-D bulk copy), SYNCS = mbarrier ops, LDGSTS = cp.async, REDUX = redux.sync, ATOMS = shared atomics, REDG/ATOMG = global\n")
         f.write("# reductions/atomics, MATCH = match.any, .EF = evict-first (cache-streaming) global accesses, DFMA/DMUL/MUFU.RCP64H = fp64 (shared-reciprocal division)\n")
         f.write("# level kernel <M, warps, entries per lane, update>: the instantiations the BASELINE workloads launch — <7,8,2,2> KDD 5-class, <7,16,1,2> KDD 23-class,\n")
@@ -78,6 +79,6 @@ if __name__ == "__main__":
         f.write("# kernel | total | " + " | ".join(COLS) + "\n")
         f.write("\n".join(sass()) + "\n")
     with open(os.path.join(ROOT, "profiles", "r02_ptxas_resources.txt"), "w") as f:
-        f.write("# ptxas -v resource usage per kernel (nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -fmad=false), round-2 final code, from csrc/build/*.ptxas.log (tools/sass_evidence.py)\n")
+        f.write("# ptxas -v resource usage per kernel (nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false), from csrc/build/*.ptxas.log (tools/sass_evidence.py)\n")
         f.write("# kernel | registers | spill stores B | spill loads B | static smem B   (level kernel: only the instantiations the BASELINE workloads launch + the merge variant + the generic one)\n")
         f.write("\n".join(ptxas()) + "\n")
