@@ -290,8 +290,11 @@ int b200flow_partition_level(const uint8_t* tp, int32_t tp_stride,
  * advanced by one 64-bit atomic); without it only the child
  * histograms are built (ent_out / cursors may be NULL): the level-0 pass, whose segments do not change, and the
  * pass that builds the deepest scored level, whose entries are never read again. */
-int b200flow_route_hist_config(int32_t F, int32_t m, int32_t n_bins, int32_t C, int32_t* chunk_rows, int32_t* m_pass);
+int b200flow_route_hist_config(int32_t F, int32_t m, int32_t n_bins, int32_t C,
+                               int32_t rec_bytes /* packed record size, 0: byte records */, int32_t* chunk_rows, int32_t* m_pass);
 int b200flow_route_hist_level(const uint8_t* tp, int32_t tp_stride, int32_t F,
+                              const int32_t* field_desc /* device, F + 1 descriptors: tp holds packed records of tp_stride
+                                                           bytes (b200flow_pack_records); NULL: byte records */,
                               const void* ent, void* ent_out,
                               int32_t n_slots, const int64_t* seg_begin, const int64_t* seg_end,
                               const int64_t* chunk_off, const int64_t* n_chunks_dev /* = chunk_off[n_slots], on the device */,
@@ -301,6 +304,17 @@ int b200flow_route_hist_level(const uint8_t* tp, int32_t tp_stride, int32_t F,
                               void* chunk_scratch /* 16 bytes per chunk (n_chunks_max), 16-byte aligned */,
                               const uint16_t* subset_next, int32_t m, int32_t n_bins, int32_t C,
                               uint32_t* hist_next, int32_t flags, void* stream);
+
+/* Bit-packed TreePoint records for the level kernel (host-only, no device needed).  Field f < F holds a bin of feature f
+ * (feat_bins[f] values), field F the label (C values); each takes max(1, bits(values - 1)) bits, fields are placed
+ * first-fit-decreasing into 32-bit words and none crosses a word.  desc[f] (host, F + 1) = word | shift << 8 | mask << 16.
+ * *rec_bytes = the words rounded up to 16 bytes when that is at most 64 bytes and at least one 16-byte granule below the
+ * staged byte record, else 0 (keep the byte records; always for F > 255, which the level kernel does not take).  The layout
+ * depends only on (feat_bins, C). */
+int b200flow_packed_layout(int32_t F, const int32_t* feat_bins, int32_t C, int32_t* desc, int32_t* rec_bytes);
+/* byte records tp[n_rows][tp_stride] -> packed[n_rows][rec_bytes] (desc on the device, as b200flow_packed_layout wrote it) */
+int b200flow_pack_records(const uint8_t* tp, int32_t tp_stride, int64_t n_rows, int32_t F, const int32_t* desc,
+                          int32_t rec_bytes, uint32_t* packed, void* stream);
 
 /* routing plan of a scored level: n_chunks[s] = ceil(len(s) / chunk_rows) for a split parent with at least one non-leaf
  * child, else 0 (its exclusive scan is route_hist_level's chunk_off); also scatters split[s].gain into node_gain[slot_node[s]]

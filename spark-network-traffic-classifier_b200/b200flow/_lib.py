@@ -55,8 +55,9 @@ _SIGNATURES = {
     "b200flow_hist_level": [_P, _I32, _I32, _P, _I32, _P, _P, _P, _I64, _I32, _P, _I32, _I32, _I32, _P, _P],
     "b200flow_score_level": [_P, _I32, _P, _I32, _I32, _I32, _P, _P, _I32, _I32, _I32, _F64, _P, _P, _P, _P, _P],
     "b200flow_grow_level": [_I32, _P, _P, _P, _P, _P, _P, _P, _I32, _P, _P, _P, _P, _I64, _P, _P, _P, _P, _P, _P, _P],
-    "b200flow_route_hist_level": [_P, _I32, _I32, _P, _P, _I32, _P, _P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _I32, _I32,
+    "b200flow_route_hist_level": [_P, _I32, _I32, _P, _P, _P, _I32, _P, _P, _P, _P, _I64, _I32, _P, _P, _P, _P, _P, _I32, _I32,
                                   _I32, _P, _I32, _P],
+    "b200flow_pack_records": [_P, _I32, _I64, _I32, _P, _I32, _P, _P],
     "b200flow_partition_level": [_P, _I32, _P, _P, _I32, _P, _P, _P, _I64, _I32, _P, _P, _P],
     "b200flow_plan_route": [_I32, _P, _P, _P, _I32, _P, _P, _P, _P, _P],
     "b200flow_next_segments": [_I32, _P, _P, _P, _P, _P, _P, _P, _P],
@@ -73,7 +74,8 @@ _SIGNATURES = {
     "b200flow_csv_dictionary": [_P, _I64, _P, _I64, _I32, _I32, _P, _P, _P, _I32, _P, _P],
     "b200flow_csv_parse": [_P, _I64, _P, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _P, _I32, _P, _P],
 }
-EXPORTS = sorted(list(_SIGNATURES) + ["b200flow_last_error", "b200flow_version", "b200flow_route_hist_config"])
+EXPORTS = sorted(list(_SIGNATURES) + ["b200flow_last_error", "b200flow_version", "b200flow_route_hist_config",
+                                       "b200flow_packed_layout"])
 
 _lib = None
 launches = 0   # kernels of OURS launched so far (counted per C-ABI call); bench.py reads the delta over the timed region
@@ -95,17 +97,32 @@ def load():
             fn.restype = C.c_int
         lib.b200flow_last_error.restype = C.c_char_p
         lib.b200flow_version.restype = C.c_int
-        lib.b200flow_route_hist_config.argtypes = [_I32] * 4 + [C.POINTER(_I32), C.POINTER(_I32)]
+        lib.b200flow_route_hist_config.argtypes = [_I32] * 5 + [C.POINTER(_I32), C.POINTER(_I32)]
         lib.b200flow_route_hist_config.restype = C.c_int
+        lib.b200flow_packed_layout.argtypes = [_I32, _P, _I32, _P, C.POINTER(_I32)]
+        lib.b200flow_packed_layout.restype = C.c_int
         _lib = lib
     return _lib
 
 
-def route_hist_config(F, m, n_bins, n_classes):
-    """launch shape of the fused route + histogram kernel: (chunk_rows, m_pass) or None when it cannot run (host-only call)."""
+def route_hist_config(F, m, n_bins, n_classes, rec_bytes=0):
+    """launch shape of the fused route + histogram kernel: (chunk_rows, m_pass) or None when it cannot run (host-only call).
+    rec_bytes: size of the packed records it gathers (packed_layout), 0 for byte records."""
     ch, mp = _I32(0), _I32(0)
-    ok = load().b200flow_route_hist_config(int(F), int(m), int(n_bins), int(n_classes), C.byref(ch), C.byref(mp))
+    ok = load().b200flow_route_hist_config(int(F), int(m), int(n_bins), int(n_classes), int(rec_bytes), C.byref(ch), C.byref(mp))
     return (int(ch.value), int(mp.value)) if ok else None
+
+
+def packed_layout(feat_bins, n_classes):
+    """bit-packed TreePoint layout of the level kernel (host-only call): (desc int32[F + 1], rec_bytes); rec_bytes == 0 means
+    the byte records stay (packing would not save a 16-byte granule)."""
+    fb = np.ascontiguousarray(feat_bins, dtype=np.int32)
+    desc = np.zeros(fb.shape[0] + 1, np.int32)
+    rb = _I32(0)
+    lib = load()
+    if lib.b200flow_packed_layout(int(fb.shape[0]), fb.ctypes.data, int(n_classes), desc.ctypes.data, C.byref(rb)) != 0:
+        raise B200FlowError("b200flow_packed_layout failed: %s" % lib.b200flow_last_error().decode())
+    return desc, int(rb.value)
 
 
 def ptr(t):

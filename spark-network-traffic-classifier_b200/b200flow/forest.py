@@ -122,6 +122,14 @@ def build_metadata(n_rows, F, num_classes, arity, max_bins, num_trees, strategy=
     return mpb, kind, max(1, min(m, F))
 
 
+def pack_records(tp, F, field_desc, rec_bytes):
+    """byte TreePoint records tp[U][stride] -> bit-packed records [U][rec_bytes] (uint8) of the layout whose device
+    descriptors are field_desc (_lib.packed_layout)"""
+    packed = torch.empty((max(tp.shape[0], 1), rec_bytes), dtype=torch.uint8, device=tp.device)
+    call("b200flow_pack_records", ptr(tp), tp.shape[1], tp.shape[0], F, ptr(field_desc), rec_bytes, ptr(packed))
+    return packed
+
+
 def dedup_rows(tp, key_bytes, sync=True):
     """unique TreePoint records of a binned batch: -> (tp_unique [U, stride], uid int32 [n], U).  Flow records repeat
     massively (KDD99: 4.9 M rows, ~1.07 M distinct), so both the level loop and the batch predictor run per unique record."""
@@ -462,7 +470,8 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
             node_mask = ext(node_mask, (4,))
         cap_nodes = new_cap
 
-    head = torch.cat([bad.to(torch.int64), feat_bins.max().reshape(1).to(torch.int64), n_s_dev.to(torch.int64), u_dev]).cpu()
+    head = torch.cat([bad.to(torch.int64), feat_bins.max().reshape(1).to(torch.int64), n_s_dev.to(torch.int64), u_dev,
+                      feat_bins.to(torch.int64)]).cpu()
     if int(head[1]) != 0:
         raise InvalidRowsError("%d NaN/null cells or unseen labels in the training rows" % int(head[1]))
     if int(head[0]) != 0:
@@ -474,6 +483,20 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
         tp = tp[:U]
     if tp.shape[0] == 0:                                  # a rank without rows still walks the level loop (its collectives): give the
         tp = torch.zeros((1, stride), dtype=torch.uint8, device=dev)   # kernels a real pointer (data_ptr() of an empty tensor is NULL)
+    # launch shape of the fused kernel: entries per routing chunk and subset features per pass (wide nodes — many classes,
+    # or a DecisionTree's all-feature histograms — are accumulated in several feature passes, the first of which routes)
+    desc_host, rec_bytes = _lib.packed_layout(head[5:5 + F].numpy(), C) if FUSED else (None, 0)
+    cfg = _lib.route_hist_config(F, m, n_bins, C, rec_bytes) if FUSED else None
+    fused = cfg is not None
+    route_ch, m_pass = cfg if fused else (CHUNK_ROWS, m)
+    route_passes = -(-m // m_pass)
+    hsz = m * n_bins * C
+    # the fused kernel gathers bit-packed records when they save a 16-byte granule (KDD: 32 instead of 48 bytes staged);
+    # everything else (the unfused kernels, predict) keeps reading the byte records
+    rec_tp, rec_stride, field_desc = tp, stride, None
+    if fused and rec_bytes:
+        field_desc = _lib.h2d(desc_host, dev)
+        rec_tp, rec_stride = pack_records(tp, F, field_desc, rec_bytes), rec_bytes
     # ---- R6 bagging: W[tree][unique] = summed Poisson weights; entries = non-zero (unique, weight) pairs per tree
     nb = (U + 1023) // 1024
     W = torch.zeros(max(T * U, 1), dtype=torch.int32, device=dev)
@@ -514,14 +537,8 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
     group_slots = max(1, HIST_BUDGET_BYTES // per_slot_hist)
     stats = dict(levels=0, slots=0, entries=0, hist_launches=0, rows=n, unique_rows=U)
 
-    # launch shape of the fused kernel: entries per routing chunk and subset features per pass (wide nodes — many classes,
-    # or a DecisionTree's all-feature histograms — are accumulated in several feature passes, the first of which routes)
-    cfg = _lib.route_hist_config(F, m, n_bins, C) if FUSED else None
-    fused = cfg is not None
-    route_ch, m_pass = cfg if fused else (CHUNK_ROWS, m)
-    route_passes = -(-m // m_pass)
-    hsz = m * n_bins * C
     stats["route_chunk"], stats["route_passes"] = route_ch if fused else 0, route_passes if fused else 0
+    stats["record_format"], stats["record_bytes"] = ("packed", rec_bytes) if field_desc is not None else ("bytes", stride)
 
     def chunk_table(nch):
         off = torch.empty(nch.shape[0] + 1, dtype=torch.int64, device=dev)
@@ -601,7 +618,7 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
         hist_next = torch.zeros((n_next_cap + world - 1) * hsz, dtype=torch.int32, device=dev)   # + padding for the node-block scatter
         cmax = route_chunks_max + n_parents
         scratch = torch.empty(cmax * 4, dtype=torch.int32, device=dev)
-        _timed("route_hist_level", "b200flow_route_hist_level", ptr(tp), stride, F, ptr(ent), ptr(ent2), n_parents,
+        _timed("route_hist_level", "b200flow_route_hist_level", ptr(rec_tp), rec_stride, F, ptr(field_desc), ptr(ent), ptr(ent2), n_parents,
                ptr(seg_begin), ptr(seg_end), ptr(roff), ptr(rch_dev), cmax, route_ch, ptr(split_), ptr(child_slot_), ptr(cursors_),
                ptr(scratch), ptr(next_subset_), m, n_bins, C, ptr(hist_next), 1 if route else 0)
         _lib.launches += route_passes - 1

@@ -510,8 +510,9 @@ __global__ void __launch_bounds__(256) partition_level_kernel(
 // Persistent CTAs (a multiple of 132), each owning a contiguous range of chunks (<= CH entries of one SPLIT parent).
 // Software pipeline per WARP, all copies asynchronous (LDGSTS, no register staging):
 //     entries(t+2)  -->  record gather(t+1)  -->  route + histogram(t)
-//   * the gather brings each entry's 64-byte-aligned TreePoint record (one HBM burst) into a shared-memory tile,
-//     ONCE per entry per level — partition_level + hist_level gathered it twice and were bound by exactly that;
+//   * the gather brings each entry's TreePoint record (the 64-byte-aligned byte record, or its bit-packed copy when that
+//     saves a 16-byte granule: KDD's 32 bytes) into a shared-memory tile, ONCE per entry per level — partition_level +
+//     hist_level gathered it twice and were bound by exactly that;
 //   * every entry is routed by the parent's split and accumulated into its CHILD's histogram (child feature subset)
 //     in shared memory with shared atomics; lane i takes the child's subset features in the ROTATED order (i + t) % m, so
 //     that one warp instruction spreads over all m features: the byte reads of the tile fall on random banks instead of
@@ -537,6 +538,16 @@ __host__ __device__ inline int route_granules(int F) { return (F + 1 + kGran - 1
 __host__ __device__ inline int route_pitch(int F) { return kGran == 16 ? route_granules(F) : (route_granules(F) | 1); }
 constexpr bool kEvictFirst = B2F_EVICT_FIRST != 0;   // entry stream with L2::evict_first (records stay L2-resident)
 
+// Bit-packed TreePoint records (b200flow_packed_layout): field f of a record is (word[d & 0xff] >> ((d >> 8) & 0xff)) &
+// (d >> 16) with d = desc[f]; the label is field F.  Records are 16 to 64 bytes, always gathered in 16-byte granules.
+// In the staged tile the granules of entry i are swizzled (granule g stored at g ^ sw) so that one word read by a whole
+// warp falls on 8 banks (at most 4-way conflicts), as it does for the 48-byte pitch of KDD's byte records: a plain
+// 32-byte pitch would put every 4th entry on the same bank (8-way), a 64-byte pitch every 2nd (16-way).
+constexpr int kPackedMaxBytes = 64;
+__device__ __forceinline__ int packed_swizzle_words(int i, int nq) {      // word-index XOR of entry i (granule swizzle x 4)
+    return nq == 2 ? ((i >> 2) & 1) << 2 : nq == 4 ? ((i >> 1) & 3) << 2 : 0;
+}
+
 struct RouteChunk { int32_t slot; int32_t n; long long begin; };   // 16 bytes, one per chunk
 
 __global__ void route_chunks_kernel(const int64_t* __restrict__ chunk_off, int n_slots, const int64_t* __restrict__ n_chunks_dev,
@@ -552,6 +563,7 @@ __global__ void route_chunks_kernel(const int64_t* __restrict__ chunk_off, int n
 
 struct RouteArgs {
     const uint8_t* tp; int stride; int F;
+    const int32_t* field_desc;                  // packed records: F + 1 field descriptors (NULL: byte records)
     const b2f_entry* ent; b2f_entry* ent_out;
     const RouteChunk* chunks; const int64_t* n_chunks_dev;
     const int64_t* seg_begin; const int64_t* seg_end;
@@ -568,22 +580,24 @@ struct RouteArgs {
 //     write-out of step t-1 (its cursor reservation, a global atomic issued one step earlier, has landed by now)
 //     route + histogram of step t from the tile
 // CTA-wide barriers happen only when the parent slot changes (flush + re-zero of the two child histograms).
-template <int M, int NW, int KS, int MERGE>   // MERGE: 0 plain shared atomics (runtime m), 1 top-group merge, 2 rotated features
+template <int M, int NW, int KS, int MERGE, bool PACKED>   // MERGE: 0 plain shared atomics (runtime m), 1 top-group merge,
+                                                           // 2 rotated features; PACKED: bit-packed records (a.field_desc)
 __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) route_hist_level_kernel(const RouteArgs a) {
     extern __shared__ __align__(16) uint32_t sm_u32[];
     constexpr int kThreads = NW * 32, kSub = KS * 32;
+    constexpr int gran = PACKED ? 16 : kGran;
     const int m = M > 0 ? M : a.m;
     const int F = a.F;
     const int tid = threadIdx.x, lane = lane_id(), wid = warp_id();
-    const int nq = route_granules(F);                        // staged granules (16-byte quads by default) per record
-    const int rs = route_pitch(F) * kGran;                   // bytes per staged record
+    const int nq = PACKED ? a.stride / 16 : route_granules(F);   // staged granules (16-byte quads by default) per record
+    const int rs = PACKED ? a.stride : route_pitch(F) * kGran;   // bytes per staged record
     const int nbC = a.n_bins * a.C, hsz = m * nbC;
     const int tile_words = rs * kSub / 4;
     uint32_t* tile = sm_u32 + (size_t)wid * tile_words;      // this warp's [kSub][nq] quad tile (entry-major)
     uint32_t* sh_hist = sm_u32 + (size_t)NW * tile_words;    // [2][hsz]
-    int* sh_fpos = (int*)(sh_hist + 2 * hsz);                // [2][m]: byte offset of the feature inside a staged record
+    int* sh_fpos = (int*)(sh_hist + 2 * hsz);                // [2][m]: byte offset (packed: descriptor) of the feature in a record
     __shared__ b200flow_split sh_split;
-    __shared__ int sh_child[2];
+    __shared__ int sh_child[2], sh_route_field;              // sh_route_field: byte offset / descriptor of the split feature
 
     const int64_t n_chunks = *a.n_chunks_dev;
     const int64_t c0 = n_chunks * blockIdx.x / gridDim.x, c1 = n_chunks * (blockIdx.x + 1) / gridDim.x;
@@ -617,9 +631,10 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) rou
             uint32_t r = __shfl_sync(0xffffffffu, x[0].x, e & 31);
             if (KS == 2) { const uint32_t r1 = __shfl_sync(0xffffffffu, x[KS - 1].x, e & 31); r = e < 32 ? r : r1; }
             if (e < cn) {
-                uint8_t* dst = (uint8_t*)tile + e * rs + q * kGran;
-                const uint8_t* src = a.tp + (int64_t)r * a.stride + q * kGran;
-                if (kGran == 16) cp_async16(dst, src); else if (kGran == 8) cp_async8(dst, src); else cp_async4(dst, src);
+                const int qd = PACKED ? q ^ (packed_swizzle_words(e, nq) >> 2) : q;
+                uint8_t* dst = (uint8_t*)tile + e * rs + qd * gran;
+                const uint8_t* src = a.tp + (int64_t)r * a.stride + q * gran;
+                if (gran == 16) cp_async16(dst, src); else if (gran == 8) cp_async8(dst, src); else cp_async4(dst, src);
             }
         }
         cp_async_commit();
@@ -648,8 +663,14 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) rou
     entries_of(d0, e);
     entries_of(d1, f);
     int cur_slot = -1;
-    const int lab_pos = F;                                     // byte of the label inside a staged record
+    const int lab_pos = PACKED ? __ldg(a.field_desc + F) : F;  // byte (packed: descriptor) of the label inside a staged record
     const uint8_t* tile8 = (const uint8_t*)tile;               // [kSub entries][nq * 16 bytes]
+    // field of staged entry i at byte offset / descriptor d
+    auto field = [&](int i, int d) -> uint32_t {
+        if (!PACKED) return tile8[d + i * rs];
+        const uint32_t v = tile[i * (rs >> 2) + ((d & 0xff) ^ packed_swizzle_words(i, nq))];
+        return (v >> ((d >> 8) & 0xff)) & (uint32_t)(d >> 16);
+    };
     for (int64_t c = c0; c < c1; ++c) {
         entries_of(d2, g);                                     // prefetch, consumed two steps later
         const int4 d3 = desc_at(c + 3);
@@ -664,10 +685,11 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) rou
             __syncthreads();
             if (tid < 16) ((uint32_t*)&sh_split)[tid] = ((const uint32_t*)(a.split + s))[tid];
             if (tid < 2) sh_child[tid] = a.child_slot[2 * s + tid];
+            if (tid == 0) { const int fs = max(a.split[s].feat, 0); sh_route_field = PACKED ? a.field_desc[fs] : fs; }
             for (int j = tid; j < 2 * m; j += kThreads) {
                 const int cs = a.child_slot[2 * s + (j >= m)];
                 const int fidx = cs >= 0 ? a.subset_next[(int64_t)cs * a.m_total + a.j0 + (j < m ? j : j - m)] : 0;
-                sh_fpos[j] = fidx;
+                sh_fpos[j] = PACKED ? a.field_desc[fidx] : fidx;
             }
             cur_slot = s;
             __syncthreads();
@@ -675,7 +697,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) rou
         const int cnt = count_of(d0);
         if (cnt > 0) {
             const int cl = sh_child[0], cr = sh_child[1];
-            const int fs = sh_split.feat, kind = sh_split.kind, thr = sh_split.bin_thr;
+            const int fs = sh_route_field, kind = sh_split.kind, thr = sh_split.bin_thr;
             int nL = 0, nR = 0;
             uint32_t dec = 0;
 #pragma unroll
@@ -683,7 +705,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) rou
                 const int i = k * 32 + lane;
                 int d = 0;
                 if (i < cnt) {
-                    const int bin = tile8[fs + i * rs];
+                    const int bin = (int)field(i, fs);
                     const bool left = kind == 0 ? (bin <= thr) : ((sh_split.mask[bin >> 6] >> (bin & 63)) & 1ull);
                     d = left ? (cl >= 0 ? 1 : 0) : (cr >= 0 ? 2 : 0);
                 }
@@ -695,7 +717,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) rou
                     const int side = d - 1;
                     const int* fpos = sh_fpos + side * m;
                     uint32_t* hist = sh_hist + side * hsz;
-                    const uint32_t lab = tile8[lab_pos + i * rs];
+                    const uint32_t lab = field(i, lab_pos);
                     const uint32_t w = e[k].y;
                     if (M > 0 && MERGE == 1) {
                         // top-group merge: per feature, the lanes that share the first active lane's (bin, label, child) counter are
@@ -706,7 +728,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) rou
 #pragma unroll
                         for (int j = 0; j < M; ++j) {
                             const int fp = fpos[j];
-                            const uint32_t bin = tile8[fp + i * rs];
+                            const uint32_t bin = field(i, fp);
                             const uint32_t key = bin | tag;
                             uint32_t* addr = &hist[j * nbC + bin * a.C + lab];
                             const int l0 = __ffs(active) - 1;
@@ -722,14 +744,14 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) rou
 #pragma unroll
                         for (int t = 0; t < M; ++t) {
                             const int fp = fpos[j];
-                            const uint32_t bin = tile8[fp + i * rs];
+                            const uint32_t bin = field(i, fp);
                             atomicAdd(&hist[j * nbC + bin * a.C + lab], w);
                             j = j + 1 == M ? 0 : j + 1;
                         }
                     } else {
                         for (int j = 0; j < m; ++j) {
                             const int fp = fpos[j];
-                            const uint32_t bin = tile8[fp + i * rs];
+                            const uint32_t bin = field(i, fp);
                             atomicAdd(&hist[j * nbC + bin * a.C + lab], w);
                         }
                     }
@@ -763,8 +785,9 @@ struct RouteCfg { int nw, ks, m_pass, per_sm; size_t smem; };
 constexpr size_t kSmemPerSM = 227 * 1024;                  // 232,448 B usable per block on sm_90
 constexpr size_t kSmemCtaOverhead = 1024 + 128;            // driver reservation per CTA + the kernel's static shared memory
 
-static size_t route_hist_smem(int F, int mp, int n_bins, int C, int nw, int ks) {
-    return (size_t)nw * ks * 32 * route_pitch(F) * kGran + 2 * (size_t)mp * n_bins * C * 4 + 2 * (size_t)mp * 4 + 64;
+// rs = bytes per staged record: route_pitch(F) * kGran for byte records, the record size for packed ones
+static size_t route_hist_smem(int rs, int mp, int n_bins, int C, int nw, int ks) {
+    return (size_t)nw * ks * 32 * rs + 2 * (size_t)mp * n_bins * C * 4 + 2 * (size_t)mp * 4 + 64;
 }
 static int route_max_ctas(int nw) { return nw == 8 ? 3 : (nw == 16 ? 2 : 1); }   // __launch_bounds__ (8 warps: 3 CTAs, 85 registers)
 
@@ -772,12 +795,12 @@ static int route_max_ctas(int nw) { return nw == 8 ? 3 : (nw == 16 ? 2 : 1); }  
 // records again), then the most entries in flight per SM (resident warps x entries per lane) up to 48, then the smallest
 // chunk, then the most resident warps.  On an H100 (KDD99-full, level kernel per fit) 8x2 with 3 CTAs per SM took 26.6 ms,
 // 16x2 with 64 entries in flight 30.5, 8x1 28.3, 16x1 28.4, and 8x2 with 4 CTAs per SM (64 registers: spills) 35.0.
-static bool route_cfg(int F, int m, int n_bins, int C, RouteCfg* out) {
+static bool route_cfg(int F, int rs, int m, int n_bins, int C, RouteCfg* out) {
     static const int cand[5][2] = {{8, 2}, {8, 1}, {16, 2}, {16, 1}, {32, 1}};
     int force_nw = 0, force_ks = 0;                         // tuning / test knob, read per call: B200FLOW_ROUTE_SHAPE=<warps>x<entries per lane>
     { const char* e = getenv("B200FLOW_ROUTE_SHAPE"); if (e && sscanf(e, "%dx%d", &force_nw, &force_ks) != 2) force_nw = force_ks = 0; }
     if (F <= 0 || F > 255 || m <= 0 || n_bins <= 0 || C <= 0) return false;
-    auto fits = [&](int mp, int nw, int ks) { return route_hist_smem(F, mp, n_bins, C, nw, ks) + kSmemCtaOverhead <= kSmemPerSM; };
+    auto fits = [&](int mp, int nw, int ks) { return route_hist_smem(rs, mp, n_bins, C, nw, ks) + kSmemCtaOverhead <= kSmemPerSM; };
     int mp = m;
     while (mp >= 1 && !fits(mp, 8, 1)) --mp;                // (8, 1) has the smallest tiles
     if (mp < 1) return false;
@@ -788,7 +811,7 @@ static bool route_cfg(int F, int m, int n_bins, int C, RouteCfg* out) {
         const int nw = cand[i][0], ks = cand[i][1];
         if (force_nw > 0 && (nw != force_nw || ks != force_ks)) continue;
         if (!fits(mp, nw, ks)) continue;
-        const size_t smem = route_hist_smem(F, mp, n_bins, C, nw, ks);
+        const size_t smem = route_hist_smem(rs, mp, n_bins, C, nw, ks);
         int per_sm = (int)(kSmemPerSM / (smem + kSmemCtaOverhead));
         if (per_sm > route_max_ctas(nw)) per_sm = route_max_ctas(nw);
         const int warps = per_sm * nw > 32 ? 32 : per_sm * nw;
@@ -797,7 +820,7 @@ static bool route_cfg(int F, int m, int n_bins, int C, RouteCfg* out) {
     }
     if (best < 0) return false;
     out->nw = cand[best][0]; out->ks = cand[best][1]; out->m_pass = mp;
-    out->smem = route_hist_smem(F, mp, n_bins, C, out->nw, out->ks);
+    out->smem = route_hist_smem(rs, mp, n_bins, C, out->nw, out->ks);
     out->per_sm = (int)(kSmemPerSM / (out->smem + kSmemCtaOverhead));
     if (out->per_sm > route_max_ctas(out->nw)) out->per_sm = route_max_ctas(out->nw);
     return true;
@@ -812,7 +835,7 @@ static int route_hist_variant() {
     return 2;
 }
 
-template <int NW, int KS>
+template <int NW, int KS, bool PACKED>
 static cudaError_t route_launch(int M, int merge, unsigned grid_cap, size_t smem, int per_sm_hint, int waves, int64_t n_chunks_max,
                                 const RouteArgs& a, cudaStream_t st) {
     cudaError_t e = cudaSuccess;
@@ -831,18 +854,28 @@ static cudaError_t route_launch(int M, int merge, unsigned grid_cap, size_t smem
     }
 #define B2F_ROUTE_CASE(MM)                                                                                                     \
     case MM:                                                                                                                   \
-        if (merge == 1) B2F_ROUTE_GO((route_hist_level_kernel<MM, NW, KS, 1>))                                                 \
-        else if (merge == 2) B2F_ROUTE_GO((route_hist_level_kernel<MM, NW, KS, 2>))                                            \
-        else B2F_ROUTE_GO((route_hist_level_kernel<0, NW, KS, 0>))                                                             \
+        if (merge == 1) B2F_ROUTE_GO((route_hist_level_kernel<MM, NW, KS, 1, PACKED>))                                         \
+        else if (merge == 2) B2F_ROUTE_GO((route_hist_level_kernel<MM, NW, KS, 2, PACKED>))                                    \
+        else B2F_ROUTE_GO((route_hist_level_kernel<0, NW, KS, 0, PACKED>))                                                     \
         break;
     switch (M) {
         B2F_ROUTE_CASE(1) B2F_ROUTE_CASE(2) B2F_ROUTE_CASE(3) B2F_ROUTE_CASE(4) B2F_ROUTE_CASE(5) B2F_ROUTE_CASE(6)
         B2F_ROUTE_CASE(7) B2F_ROUTE_CASE(8) B2F_ROUTE_CASE(9) B2F_ROUTE_CASE(10) B2F_ROUTE_CASE(11) B2F_ROUTE_CASE(12)
-        default: B2F_ROUTE_GO((route_hist_level_kernel<0, NW, KS, 0>)) break;
+        default: B2F_ROUTE_GO((route_hist_level_kernel<0, NW, KS, 0, PACKED>)) break;
     }
 #undef B2F_ROUTE_CASE
 #undef B2F_ROUTE_GO
     return cudaGetLastError();
+}
+
+template <bool PACKED>
+static cudaError_t route_shape(const RouteCfg& cfg, int M, int merge, size_t smem, int waves, int64_t n_chunks_max, const RouteArgs& a,
+                               cudaStream_t st) {
+    if (cfg.nw == 8 && cfg.ks == 2) return route_launch<8, 2, PACKED>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+    if (cfg.nw == 8) return route_launch<8, 1, PACKED>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+    if (cfg.nw == 16 && cfg.ks == 2) return route_launch<16, 2, PACKED>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+    if (cfg.nw == 16) return route_launch<16, 1, PACKED>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+    return route_launch<32, 1, PACKED>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
 }
 
 __global__ void next_segments_kernel(int n_next, const int64_t* __restrict__ n_next_dev, const int32_t* __restrict__ next_parent,
@@ -976,15 +1009,49 @@ extern "C" int b200flow_finalize_forest(int64_t n_nodes, const uint32_t* pool_co
     return check_launch("finalize_forest");
 }
 
-extern "C" int b200flow_route_hist_config(int32_t F, int32_t m, int32_t n_bins, int32_t C, int32_t* chunk_rows, int32_t* m_pass) {
+extern "C" int b200flow_packed_layout(int32_t F, const int32_t* feat_bins, int32_t C, int32_t* desc, int32_t* rec_bytes) {
+    B2F_REQUIRE(feat_bins && desc && rec_bytes && F > 0 && C > 0 && C <= 256, "packed_layout: bad arguments");
+    *rec_bytes = 0;
+    if (F > 255) return B200FLOW_OK;                         // no fused level kernel for such records (route_cfg): keep bytes
+    int width[256], order[256], used[256];
+    auto bits = [](int v) { int b = 0; while (v > 0) { ++b; v >>= 1; } return b > 0 ? b : 1; };
+    for (int f = 0; f <= F; ++f) {
+        const int nb = f < F ? feat_bins[f] : C;
+        B2F_REQUIRE(nb >= 1 && nb <= 256, "packed_layout: field %d has %d values", f, nb);
+        width[f] = bits(nb - 1);
+        order[f] = f;
+    }
+    for (int i = 1; i <= F; ++i) {                           // stable sort by width, widest first
+        const int f = order[i]; int k = i - 1;
+        while (k >= 0 && width[order[k]] < width[f]) { order[k + 1] = order[k]; --k; }
+        order[k + 1] = f;
+    }
+    int nw = 0;
+    for (int i = 0; i <= F; ++i) {                           // first fit: no field crosses a 32-bit word
+        const int f = order[i];
+        int w = 0;
+        while (w < nw && used[w] + width[f] > 32) ++w;
+        if (w == nw) used[nw++] = 0;
+        desc[f] = w | (used[w] << 8) | (((1 << width[f]) - 1) << 16);
+        used[w] += width[f];
+    }
+    const int bytes = (nw * 4 + 15) / 16 * 16;
+    // packed only when it saves at least one 16-byte granule of the staged byte record, up to kPackedMaxBytes
+    *rec_bytes = bytes <= kPackedMaxBytes && bytes + 16 <= route_pitch(F) * kGran ? bytes : 0;
+    return B200FLOW_OK;
+}
+
+extern "C" int b200flow_route_hist_config(int32_t F, int32_t m, int32_t n_bins, int32_t C, int32_t rec_bytes, int32_t* chunk_rows,
+                                          int32_t* m_pass) {
     RouteCfg cfg;
-    if (!route_cfg(F, m, n_bins, C, &cfg)) return 0;
+    if (rec_bytes < 0 || !route_cfg(F, rec_bytes > 0 ? rec_bytes : route_pitch(F) * kGran, m, n_bins, C, &cfg)) return 0;
     if (chunk_rows) *chunk_rows = cfg.nw * cfg.ks * 32;
     if (m_pass) *m_pass = cfg.m_pass;
     return 1;
 }
 
-extern "C" int b200flow_route_hist_level(const uint8_t* tp, int32_t tp_stride, int32_t F, const void* ent, void* ent_out,
+extern "C" int b200flow_route_hist_level(const uint8_t* tp, int32_t tp_stride, int32_t F, const int32_t* field_desc,
+                                         const void* ent, void* ent_out,
                                          int32_t n_slots, const int64_t* seg_begin, const int64_t* seg_end, const int64_t* chunk_off,
                                          const int64_t* n_chunks_dev, int64_t n_chunks_max, int32_t chunk_rows,
                                          const b200flow_split* split, const int32_t* child_slot,
@@ -994,10 +1061,15 @@ extern "C" int b200flow_route_hist_level(const uint8_t* tp, int32_t tp_stride, i
                     subset_next && hist_next, "route_hist_level: null pointer");
     const bool route = (flags & 1) != 0;
     B2F_REQUIRE(!route || (ent_out && cursors && ((uintptr_t)cursors & 7) == 0), "route_hist_level: routing needs ent_out and 8-byte aligned cursors");
-    B2F_REQUIRE((tp_stride & 15) == 0 && tp_stride >= (F + 1 + 15) / 16 * 16 && ((uintptr_t)tp & 15) == 0, "route_hist_level: bad TreePoint stride/alignment");
+    if (field_desc)
+        B2F_REQUIRE((tp_stride & 15) == 0 && tp_stride > 0 && tp_stride <= kPackedMaxBytes && ((uintptr_t)tp & 15) == 0,
+                    "route_hist_level: packed records must be 16-byte multiples up to %d bytes, 16-byte aligned", kPackedMaxBytes);
+    else
+        B2F_REQUIRE((tp_stride & 15) == 0 && tp_stride >= (F + 1 + 15) / 16 * 16 && ((uintptr_t)tp & 15) == 0, "route_hist_level: bad TreePoint stride/alignment");
     B2F_REQUIRE(((uintptr_t)chunk_scratch & 15) == 0, "route_hist_level: chunk_scratch must be 16-byte aligned");
     RouteCfg cfg;
-    B2F_REQUIRE(route_cfg(F, m, n_bins, C, &cfg), "route_hist_level: one feature's child histograms exceed shared memory (use partition_level + hist_level)");
+    const int rs = field_desc ? tp_stride : route_pitch(F) * kGran;
+    B2F_REQUIRE(route_cfg(F, rs, m, n_bins, C, &cfg), "route_hist_level: one feature's child histograms exceed shared memory (use partition_level + hist_level)");
     B2F_REQUIRE(chunk_rows == cfg.nw * cfg.ks * 32, "route_hist_level: chunk_rows must be the value of b200flow_route_hist_config (%d)", cfg.nw * cfg.ks * 32);
     if (n_slots <= 0 || n_chunks_max <= 0) return B200FLOW_OK;
     cudaStream_t st = (cudaStream_t)stream;
@@ -1005,7 +1077,7 @@ extern "C" int b200flow_route_hist_level(const uint8_t* tp, int32_t tp_stride, i
     route_chunks_kernel<<<(unsigned)((n_chunks_max + 255) / 256), 256, 0, st>>>(chunk_off, n_slots, n_chunks_dev, seg_begin,
                                                                              seg_end, chunk_rows, chunks);
     RouteArgs a;
-    a.tp = tp; a.stride = tp_stride; a.F = F; a.ent = (const b2f_entry*)ent; a.ent_out = (b2f_entry*)ent_out; a.chunks = chunks; a.n_chunks_dev = n_chunks_dev;
+    a.tp = tp; a.stride = tp_stride; a.F = F; a.field_desc = field_desc; a.ent = (const b2f_entry*)ent; a.ent_out = (b2f_entry*)ent_out; a.chunks = chunks; a.n_chunks_dev = n_chunks_dev;
     a.seg_begin = seg_begin; a.seg_end = seg_end; a.split = split; a.child_slot = child_slot; a.cursors = cursors;
     a.subset_next = subset_next; a.m_total = m; a.n_bins = n_bins; a.C = C; a.hist_next = hist_next;
     static int waves = -1;                                    // CTAs per resident slot: > 1 lets the block scheduler even out the tail
@@ -1015,13 +1087,9 @@ extern "C" int b200flow_route_hist_level(const uint8_t* tp, int32_t tp_stride, i
     for (int j0 = 0, pass = 0; j0 < m; j0 += cfg.m_pass, ++pass) {
         a.j0 = j0; a.m = m - j0 < cfg.m_pass ? m - j0 : cfg.m_pass; a.route = (route && pass == 0) ? 1 : 0;
         const int M = a.m <= 12 ? a.m : 0;
-        const size_t smem = route_hist_smem(F, a.m, n_bins, C, cfg.nw, cfg.ks);
-        cudaError_t e;
-        if (cfg.nw == 8 && cfg.ks == 2) e = route_launch<8, 2>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
-        else if (cfg.nw == 8) e = route_launch<8, 1>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
-        else if (cfg.nw == 16 && cfg.ks == 2) e = route_launch<16, 2>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
-        else if (cfg.nw == 16) e = route_launch<16, 1>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
-        else e = route_launch<32, 1>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+        const size_t smem = route_hist_smem(rs, a.m, n_bins, C, cfg.nw, cfg.ks);
+        cudaError_t e = field_desc ? route_shape<true>(cfg, M, merge, smem, waves, n_chunks_max, a, st)
+                                   : route_shape<false>(cfg, M, merge, smem, waves, n_chunks_max, a, st);
         if (e != cudaSuccess) { set_error("route_hist_level: %s", cudaGetErrorString(e)); return B200FLOW_ERR_CUDA; }
     }
     return check_launch("route_hist_level");

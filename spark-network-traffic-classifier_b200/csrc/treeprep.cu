@@ -518,9 +518,38 @@ __global__ void __launch_bounds__(256) bag_fill_kernel(const uint32_t* __restric
         if (w[k]) { ent[pos] = make_uint2((uint32_t)(ub + k), w[k]); ++pos; }
 }
 
+// byte TreePoint records -> bit-packed records (layout of b200flow_packed_layout): one thread per (record, 32-bit word) ORs in
+// the fields placed in its word; the F + 1 bytes of a record are read by the rw threads of that record together.
+__global__ void __launch_bounds__(256) pack_records_kernel(const uint8_t* __restrict__ tp, int stride, int64_t n_rows, int F,
+                                                           const int32_t* __restrict__ desc, int rw, uint32_t* packed) {
+    __shared__ int32_t sh_desc[256];
+    for (int f = threadIdx.x; f <= F; f += blockDim.x) sh_desc[f] = desc[f];
+    __syncthreads();
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n_rows * rw) return;
+    const int64_t r = t / rw; const int w = (int)(t - r * rw);
+    const uint8_t* rec = tp + r * stride;
+    uint32_t v = 0;
+    for (int f = 0; f <= F; ++f) {
+        const int d = sh_desc[f];
+        if ((d & 0xff) == w) v |= ((uint32_t)__ldg(rec + f) & (uint32_t)(d >> 16)) << ((d >> 8) & 0xff);
+    }
+    packed[t] = v;
+}
+
 }  // namespace b200flow
 
 using namespace b200flow;
+
+extern "C" int b200flow_pack_records(const uint8_t* tp, int32_t tp_stride, int64_t n_rows, int32_t F, const int32_t* desc,
+                                     int32_t rec_bytes, uint32_t* packed, void* stream) {
+    if (n_rows <= 0) return B200FLOW_OK;
+    B2F_REQUIRE(tp && desc && packed, "pack_records: null pointer");
+    B2F_REQUIRE(F > 0 && F <= 255 && tp_stride >= F + 1 && rec_bytes > 0 && (rec_bytes & 15) == 0, "pack_records: bad shape");
+    const int rw = rec_bytes / 4;
+    pack_records_kernel<<<(unsigned)((n_rows * rw + 255) / 256), 256, 0, (cudaStream_t)stream>>>(tp, tp_stride, n_rows, F, desc, rw, packed);
+    return check_launch("pack_records");
+}
 
 extern "C" int b200flow_exclusive_scan_i32_to_i64(const int32_t* in, int64_t n, int64_t* out, int64_t* total, void* stream) {
     B2F_REQUIRE(in && out && n >= 0, "scan: bad arguments");

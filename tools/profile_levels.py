@@ -1,6 +1,8 @@
 #!/usr/bin/env python
 """Per-level timings of one resident fit: routed entries, parent slots, route+hist time and the implied entry rate.
-Tells whether a level is bound by the shared-atomic rate (constant entries/us) or by per-slot overheads (deep levels)."""
+Tells whether a level is bound by the shared-atomic rate (constant entries/us) or by per-slot overheads (deep levels).
+Also prints the fit's unique record count U and the TreePoint record format the level kernel gathered, with its footprint:
+whether the record set fits the L2 decides the gather rate."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "spark-network-traffic-classifier_b200"))
@@ -14,10 +16,13 @@ for _ in range(2):
 torch.cuda.synchronize()
 forest.PROFILE = {}
 t0 = torch.cuda.Event(enable_timing=True); t1 = torch.cuda.Event(enable_timing=True)
-t0.record(); bench.step_resident(wl, rec, dicts, a, None); t1.record()
+t0.record(); _, _, st, _ = bench.step_resident(wl, rec, dicts, a, None); t1.record()
 torch.cuda.synchronize()
 P = forest.PROFILE
 print("step %.2f ms (with per-kernel events)" % t0.elapsed_time(t1))
+U, rb = st["unique_rows"], st.get("record_bytes", 0)
+print("rows %d  unique records U %d  record format %s, %d bytes  footprint %.1f MB"
+      % (st["rows"], U, st.get("record_format", "bytes"), rb, U * rb / 1e6))
 ents = [int(e) for e in P.get("_route_entries", [])]
 rt = [x.elapsed_time(y) for x, y in P.get("route_hist_level", [])]
 sc = [x.elapsed_time(y) for x, y in P.get("score_level", [])]
