@@ -580,22 +580,33 @@ struct RouteArgs {
 //     write-out of step t-1 (its cursor reservation, a global atomic issued one step earlier, has landed by now)
 //     route + histogram of step t from the tile
 // CTA-wide barriers happen only when the parent slot changes (flush + re-zero of the two child histograms).
-template <int M, int NW, int KS, int MERGE, bool PACKED>   // MERGE: 0 plain shared atomics (runtime m), 1 top-group merge,
-                                                           // 2 rotated features; PACKED: bit-packed records (a.field_desc)
+// Packed records with the rotated update read each (entry, feature) through a per-lane descriptor table, built once per
+// parent slot: entry [side][t][lane] describes the feature lane `lane` visits at step t for that side (subset position
+// j = (lane % M + t) % M), with the granule swizzle of the lane's entries already applied.  .x = byte offset of the field's
+// word in the staged record, .y = shift (bits 0-4, read by a wrapping funnel shift) | value mask << 8 | word index of the
+// (side, j) histogram << 16.  The lane-major layout keeps every table read conflict-free.
+__host__ __device__ inline size_t route_tab_bytes(int mp, bool packed) { return packed && mp <= 12 ? (size_t)2 * mp * 32 * 8 : 0; }
+
+template <int M, int NW, int KS, int MERGE, int NQ>   // MERGE: 0 plain shared atomics (runtime m), 1 top-group merge,
+                                                      // 2 rotated features; NQ: 16-byte granules of a bit-packed record
+                                                      // (a.field_desc, a.stride == 16 * NQ), 0: byte records
 __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) route_hist_level_kernel(const RouteArgs a) {
     extern __shared__ __align__(16) uint32_t sm_u32[];
+    constexpr bool PACKED = NQ > 0;
+    constexpr bool kTab = PACKED && M > 0 && MERGE == 2;     // histogram update through the per-lane descriptor table
     constexpr int kThreads = NW * 32, kSub = KS * 32;
     constexpr int gran = PACKED ? 16 : kGran;
     const int m = M > 0 ? M : a.m;
     const int F = a.F;
     const int tid = threadIdx.x, lane = lane_id(), wid = warp_id();
-    const int nq = PACKED ? a.stride / 16 : route_granules(F);   // staged granules (16-byte quads by default) per record
-    const int rs = PACKED ? a.stride : route_pitch(F) * kGran;   // bytes per staged record
+    const int nq = PACKED ? NQ : route_granules(F);            // staged granules (16-byte quads by default) per record
+    const int rs = PACKED ? NQ * 16 : route_pitch(F) * kGran;  // bytes per staged record
     const int nbC = a.n_bins * a.C, hsz = m * nbC;
     const int tile_words = rs * kSub / 4;
     uint32_t* tile = sm_u32 + (size_t)wid * tile_words;      // this warp's [kSub][nq] quad tile (entry-major)
     uint32_t* sh_hist = sm_u32 + (size_t)NW * tile_words;    // [2][hsz]
     int* sh_fpos = (int*)(sh_hist + 2 * hsz);                // [2][m]: byte offset (packed: descriptor) of the feature in a record
+    uint2* sh_tab = (uint2*)(sh_fpos + 2 * m);               // kTab: [2][M][32] descriptor table (route_tab_bytes)
     __shared__ b200flow_split sh_split;
     __shared__ int sh_child[2], sh_route_field;              // sh_route_field: byte offset / descriptor of the split feature
 
@@ -623,18 +634,43 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) rou
     // The tile is entry-major ([kSub entries][nq quads]) and its kSub * nq 16-byte chunks are copied in linear order, lane
     // after lane: neighbouring lanes fetch neighbouring quads of the SAME record (same 32-byte sector) into neighbouring
     // shared addresses, which the L1 can fill with fewer wavefronts than one scattered 16-byte fill per lane.
+    // Packed records: the KS * NQ granule copies of a lane are unrolled with the geometry known at compile time, so entry,
+    // granule and swizzle fold to per-lane constants plus an immediate per copy, and each copy shuffles its record index out
+    // of one known x[k] (entry 32k starts at granule 32k * NQ, a multiple of 32).  For NQ = 2 and 4 a copy covers 32 / NQ
+    // whole entries and the swizzle of entry it * 32 / NQ + lane / NQ depends on the lane alone.
+    constexpr int kNQ = PACKED ? NQ : 1;
+    constexpr bool kPow2 = (kNQ & (kNQ - 1)) == 0;
+    const int g_e0 = kPow2 ? lane / kNQ : 0, g_q0 = kPow2 ? lane % kNQ : 0;
+    const int g_sw = packed_swizzle_words(g_e0, NQ) >> 2;
+    const uint8_t* g_src = a.tp + g_q0 * 16;
+    uint8_t* g_dst = (uint8_t*)tile + g_e0 * rs + (g_q0 ^ g_sw) * 16;
     const uint32_t inv_nq = (1u << 20) / (uint32_t)nq + 1u;     // c / nq == (c * inv_nq) >> 20 for c * nq < 2^20
     auto issue_gather = [&](const int4& d, const b2f_entry* x) {
         const int cn = count_of(d);
-        for (int c = lane; c < kSub * nq; c += 32) {           // uniform trip count (KS * nq)
-            const int e = (int)(((uint32_t)c * inv_nq) >> 20), q = c - e * nq;
-            uint32_t r = __shfl_sync(0xffffffffu, x[0].x, e & 31);
-            if (KS == 2) { const uint32_t r1 = __shfl_sync(0xffffffffu, x[KS - 1].x, e & 31); r = e < 32 ? r : r1; }
-            if (e < cn) {
-                const int qd = PACKED ? q ^ (packed_swizzle_words(e, nq) >> 2) : q;
-                uint8_t* dst = (uint8_t*)tile + e * rs + qd * gran;
-                const uint8_t* src = a.tp + (int64_t)r * a.stride + q * gran;
-                if (gran == 16) cp_async16(dst, src); else if (gran == 8) cp_async8(dst, src); else cp_async4(dst, src);
+        if (PACKED) {
+#pragma unroll
+            for (int it = 0; it < KS * kNQ; ++it) {
+                const int k = it / kNQ;
+                if (kPow2) {
+                    const int e = it * (32 / kNQ) + g_e0;
+                    const uint32_t r = __shfl_sync(0xffffffffu, x[k].x, e & 31);
+                    if (e < cn) cp_async16(g_dst + it * 512, g_src + (size_t)r * (kNQ * 16));
+                } else {                                        // NQ = 3: a copy straddles entries, divide by the constant
+                    const int c = it * 32 + lane, e = c / kNQ, q = c - e * kNQ;
+                    const uint32_t r = __shfl_sync(0xffffffffu, x[k].x, e & 31);
+                    if (e < cn) cp_async16((uint8_t*)tile + e * rs + q * 16, a.tp + (size_t)r * (kNQ * 16) + q * 16);
+                }
+            }
+        } else {
+            for (int c = lane; c < kSub * nq; c += 32) {       // uniform trip count (KS * nq)
+                const int e = (int)(((uint32_t)c * inv_nq) >> 20), q = c - e * nq;
+                uint32_t r = __shfl_sync(0xffffffffu, x[0].x, e & 31);
+                if (KS == 2) { const uint32_t r1 = __shfl_sync(0xffffffffu, x[KS - 1].x, e & 31); r = e < 32 ? r : r1; }
+                if (e < cn) {
+                    uint8_t* dst = (uint8_t*)tile + e * rs + q * gran;
+                    const uint8_t* src = a.tp + (int64_t)r * a.stride + q * gran;
+                    if (gran == 16) cp_async16(dst, src); else if (gran == 8) cp_async8(dst, src); else cp_async4(dst, src);
+                }
             }
         }
         cp_async_commit();
@@ -686,10 +722,22 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) rou
             if (tid < 16) ((uint32_t*)&sh_split)[tid] = ((const uint32_t*)(a.split + s))[tid];
             if (tid < 2) sh_child[tid] = a.child_slot[2 * s + tid];
             if (tid == 0) { const int fs = max(a.split[s].feat, 0); sh_route_field = PACKED ? a.field_desc[fs] : fs; }
-            for (int j = tid; j < 2 * m; j += kThreads) {
-                const int cs = a.child_slot[2 * s + (j >= m)];
-                const int fidx = cs >= 0 ? a.subset_next[(int64_t)cs * a.m_total + a.j0 + (j < m ? j : j - m)] : 0;
-                sh_fpos[j] = PACKED ? a.field_desc[fidx] : fidx;
+            if (kTab) {
+                constexpr int kM = M > 0 ? M : 1;
+                for (int idx = tid; idx < 2 * kM * 32; idx += kThreads) {
+                    const int side = idx / (kM * 32), t = idx / 32 % kM, ln = idx % 32, j = (ln % kM + t) % kM;
+                    const int cs = a.child_slot[2 * s + side];
+                    const int fidx = cs >= 0 ? a.subset_next[(int64_t)cs * a.m_total + a.j0 + j] : 0;
+                    const uint32_t d = (uint32_t)__ldg(a.field_desc + fidx);
+                    const uint32_t word = (d & 0xffu) ^ (uint32_t)packed_swizzle_words(ln, NQ);   // lane swizzle == entry swizzle
+                    sh_tab[idx] = make_uint2(word * 4u, ((d >> 8) & 31u) | ((d >> 16) << 8) | ((uint32_t)(side * hsz + j * nbC) << 16));
+                }
+            } else {
+                for (int j = tid; j < 2 * m; j += kThreads) {
+                    const int cs = a.child_slot[2 * s + (j >= m)];
+                    const int fidx = cs >= 0 ? a.subset_next[(int64_t)cs * a.m_total + a.j0 + (j < m ? j : j - m)] : 0;
+                    sh_fpos[j] = PACKED ? a.field_desc[fidx] : fidx;
+                }
             }
             cur_slot = s;
             __syncthreads();
@@ -735,6 +783,18 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) rou
                             const bool top = key == __shfl_sync(active, key, l0);          // same counter as the first active lane
                             const uint32_t sum = __reduce_add_sync(active, top ? w : 0u);  // no divergence: the others contribute 0
                             if (!top || lane == l0) atomicAdd(addr, top ? sum : w);
+                        }
+                    } else if (kTab) {
+                        // rotated features through the descriptor table: one table read, one tile read, one shared atomic
+                        const uint2* tab = sh_tab + side * (M * 32) + lane;
+                        const uint8_t* rec = (const uint8_t*)tile + i * rs;
+                        uint32_t* hl = sh_hist + lab;
+#pragma unroll
+                        for (int t = 0; t < M; ++t) {
+                            const uint2 dd = tab[t * 32];
+                            const uint32_t v = *(const uint32_t*)(rec + dd.x);
+                            const uint32_t bin = __funnelshift_r(v, 0u, dd.y) & ((dd.y >> 8) & 0xffu);
+                            atomicAdd(hl + (dd.y >> 16) + bin * a.C, w);
                         }
                     } else if (M > 0 && MERGE == 2) {
                         // rotated features: lane i walks the subset positions in the order (i + t) % M, so that one warp
@@ -786,8 +846,8 @@ constexpr size_t kSmemPerSM = 227 * 1024;                  // 232,448 B usable p
 constexpr size_t kSmemCtaOverhead = 1024 + 128;            // driver reservation per CTA + the kernel's static shared memory
 
 // rs = bytes per staged record: route_pitch(F) * kGran for byte records, the record size for packed ones
-static size_t route_hist_smem(int rs, int mp, int n_bins, int C, int nw, int ks) {
-    return (size_t)nw * ks * 32 * rs + 2 * (size_t)mp * n_bins * C * 4 + 2 * (size_t)mp * 4 + 64;
+static size_t route_hist_smem(int rs, bool packed, int mp, int n_bins, int C, int nw, int ks) {
+    return (size_t)nw * ks * 32 * rs + 2 * (size_t)mp * n_bins * C * 4 + 2 * (size_t)mp * 4 + route_tab_bytes(mp, packed) + 64;
 }
 static int route_max_ctas(int nw) { return nw == 8 ? 3 : (nw == 16 ? 2 : 1); }   // __launch_bounds__ (8 warps: 3 CTAs, 85 registers)
 
@@ -795,12 +855,12 @@ static int route_max_ctas(int nw) { return nw == 8 ? 3 : (nw == 16 ? 2 : 1); }  
 // records again), then the most entries in flight per SM (resident warps x entries per lane) up to 48, then the smallest
 // chunk, then the most resident warps.  On an H100 (KDD99-full, level kernel per fit) 8x2 with 3 CTAs per SM took 26.6 ms,
 // 16x2 with 64 entries in flight 30.5, 8x1 28.3, 16x1 28.4, and 8x2 with 4 CTAs per SM (64 registers: spills) 35.0.
-static bool route_cfg(int F, int rs, int m, int n_bins, int C, RouteCfg* out) {
+static bool route_cfg(int F, int rs, bool packed, int m, int n_bins, int C, RouteCfg* out) {
     static const int cand[5][2] = {{8, 2}, {8, 1}, {16, 2}, {16, 1}, {32, 1}};
     int force_nw = 0, force_ks = 0;                         // tuning / test knob, read per call: B200FLOW_ROUTE_SHAPE=<warps>x<entries per lane>
     { const char* e = getenv("B200FLOW_ROUTE_SHAPE"); if (e && sscanf(e, "%dx%d", &force_nw, &force_ks) != 2) force_nw = force_ks = 0; }
     if (F <= 0 || F > 255 || m <= 0 || n_bins <= 0 || C <= 0) return false;
-    auto fits = [&](int mp, int nw, int ks) { return route_hist_smem(rs, mp, n_bins, C, nw, ks) + kSmemCtaOverhead <= kSmemPerSM; };
+    auto fits = [&](int mp, int nw, int ks) { return route_hist_smem(rs, packed, mp, n_bins, C, nw, ks) + kSmemCtaOverhead <= kSmemPerSM; };
     int mp = m;
     while (mp >= 1 && !fits(mp, 8, 1)) --mp;                // (8, 1) has the smallest tiles
     if (mp < 1) return false;
@@ -811,7 +871,7 @@ static bool route_cfg(int F, int rs, int m, int n_bins, int C, RouteCfg* out) {
         const int nw = cand[i][0], ks = cand[i][1];
         if (force_nw > 0 && (nw != force_nw || ks != force_ks)) continue;
         if (!fits(mp, nw, ks)) continue;
-        const size_t smem = route_hist_smem(rs, mp, n_bins, C, nw, ks);
+        const size_t smem = route_hist_smem(rs, packed, mp, n_bins, C, nw, ks);
         int per_sm = (int)(kSmemPerSM / (smem + kSmemCtaOverhead));
         if (per_sm > route_max_ctas(nw)) per_sm = route_max_ctas(nw);
         const int warps = per_sm * nw > 32 ? 32 : per_sm * nw;
@@ -820,7 +880,7 @@ static bool route_cfg(int F, int rs, int m, int n_bins, int C, RouteCfg* out) {
     }
     if (best < 0) return false;
     out->nw = cand[best][0]; out->ks = cand[best][1]; out->m_pass = mp;
-    out->smem = route_hist_smem(rs, mp, n_bins, C, out->nw, out->ks);
+    out->smem = route_hist_smem(rs, packed, mp, n_bins, C, out->nw, out->ks);
     out->per_sm = (int)(kSmemPerSM / (out->smem + kSmemCtaOverhead));
     if (out->per_sm > route_max_ctas(out->nw)) out->per_sm = route_max_ctas(out->nw);
     return true;
@@ -835,7 +895,7 @@ static int route_hist_variant() {
     return 2;
 }
 
-template <int NW, int KS, bool PACKED>
+template <int NW, int KS, int NQ>
 static cudaError_t route_launch(int M, int merge, unsigned grid_cap, size_t smem, int per_sm_hint, int waves, int64_t n_chunks_max,
                                 const RouteArgs& a, cudaStream_t st) {
     cudaError_t e = cudaSuccess;
@@ -854,28 +914,28 @@ static cudaError_t route_launch(int M, int merge, unsigned grid_cap, size_t smem
     }
 #define B2F_ROUTE_CASE(MM)                                                                                                     \
     case MM:                                                                                                                   \
-        if (merge == 1) B2F_ROUTE_GO((route_hist_level_kernel<MM, NW, KS, 1, PACKED>))                                         \
-        else if (merge == 2) B2F_ROUTE_GO((route_hist_level_kernel<MM, NW, KS, 2, PACKED>))                                    \
-        else B2F_ROUTE_GO((route_hist_level_kernel<0, NW, KS, 0, PACKED>))                                                     \
+        if (merge == 1) B2F_ROUTE_GO((route_hist_level_kernel<MM, NW, KS, 1, NQ>))                                         \
+        else if (merge == 2) B2F_ROUTE_GO((route_hist_level_kernel<MM, NW, KS, 2, NQ>))                                    \
+        else B2F_ROUTE_GO((route_hist_level_kernel<0, NW, KS, 0, NQ>))                                                     \
         break;
     switch (M) {
         B2F_ROUTE_CASE(1) B2F_ROUTE_CASE(2) B2F_ROUTE_CASE(3) B2F_ROUTE_CASE(4) B2F_ROUTE_CASE(5) B2F_ROUTE_CASE(6)
         B2F_ROUTE_CASE(7) B2F_ROUTE_CASE(8) B2F_ROUTE_CASE(9) B2F_ROUTE_CASE(10) B2F_ROUTE_CASE(11) B2F_ROUTE_CASE(12)
-        default: B2F_ROUTE_GO((route_hist_level_kernel<0, NW, KS, 0, PACKED>)) break;
+        default: B2F_ROUTE_GO((route_hist_level_kernel<0, NW, KS, 0, NQ>)) break;
     }
 #undef B2F_ROUTE_CASE
 #undef B2F_ROUTE_GO
     return cudaGetLastError();
 }
 
-template <bool PACKED>
+template <int NQ>
 static cudaError_t route_shape(const RouteCfg& cfg, int M, int merge, size_t smem, int waves, int64_t n_chunks_max, const RouteArgs& a,
                                cudaStream_t st) {
-    if (cfg.nw == 8 && cfg.ks == 2) return route_launch<8, 2, PACKED>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
-    if (cfg.nw == 8) return route_launch<8, 1, PACKED>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
-    if (cfg.nw == 16 && cfg.ks == 2) return route_launch<16, 2, PACKED>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
-    if (cfg.nw == 16) return route_launch<16, 1, PACKED>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
-    return route_launch<32, 1, PACKED>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+    if (cfg.nw == 8 && cfg.ks == 2) return route_launch<8, 2, NQ>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+    if (cfg.nw == 8) return route_launch<8, 1, NQ>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+    if (cfg.nw == 16 && cfg.ks == 2) return route_launch<16, 2, NQ>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+    if (cfg.nw == 16) return route_launch<16, 1, NQ>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+    return route_launch<32, 1, NQ>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
 }
 
 __global__ void next_segments_kernel(int n_next, const int64_t* __restrict__ n_next_dev, const int32_t* __restrict__ next_parent,
@@ -1044,7 +1104,7 @@ extern "C" int b200flow_packed_layout(int32_t F, const int32_t* feat_bins, int32
 extern "C" int b200flow_route_hist_config(int32_t F, int32_t m, int32_t n_bins, int32_t C, int32_t rec_bytes, int32_t* chunk_rows,
                                           int32_t* m_pass) {
     RouteCfg cfg;
-    if (rec_bytes < 0 || !route_cfg(F, rec_bytes > 0 ? rec_bytes : route_pitch(F) * kGran, m, n_bins, C, &cfg)) return 0;
+    if (rec_bytes < 0 || !route_cfg(F, rec_bytes > 0 ? rec_bytes : route_pitch(F) * kGran, rec_bytes > 0, m, n_bins, C, &cfg)) return 0;
     if (chunk_rows) *chunk_rows = cfg.nw * cfg.ks * 32;
     if (m_pass) *m_pass = cfg.m_pass;
     return 1;
@@ -1069,7 +1129,7 @@ extern "C" int b200flow_route_hist_level(const uint8_t* tp, int32_t tp_stride, i
     B2F_REQUIRE(((uintptr_t)chunk_scratch & 15) == 0, "route_hist_level: chunk_scratch must be 16-byte aligned");
     RouteCfg cfg;
     const int rs = field_desc ? tp_stride : route_pitch(F) * kGran;
-    B2F_REQUIRE(route_cfg(F, rs, m, n_bins, C, &cfg), "route_hist_level: one feature's child histograms exceed shared memory (use partition_level + hist_level)");
+    B2F_REQUIRE(route_cfg(F, rs, field_desc != nullptr, m, n_bins, C, &cfg), "route_hist_level: one feature's child histograms exceed shared memory (use partition_level + hist_level)");
     B2F_REQUIRE(chunk_rows == cfg.nw * cfg.ks * 32, "route_hist_level: chunk_rows must be the value of b200flow_route_hist_config (%d)", cfg.nw * cfg.ks * 32);
     if (n_slots <= 0 || n_chunks_max <= 0) return B200FLOW_OK;
     cudaStream_t st = (cudaStream_t)stream;
@@ -1087,9 +1147,15 @@ extern "C" int b200flow_route_hist_level(const uint8_t* tp, int32_t tp_stride, i
     for (int j0 = 0, pass = 0; j0 < m; j0 += cfg.m_pass, ++pass) {
         a.j0 = j0; a.m = m - j0 < cfg.m_pass ? m - j0 : cfg.m_pass; a.route = (route && pass == 0) ? 1 : 0;
         const int M = a.m <= 12 ? a.m : 0;
-        const size_t smem = route_hist_smem(rs, a.m, n_bins, C, cfg.nw, cfg.ks);
-        cudaError_t e = field_desc ? route_shape<true>(cfg, M, merge, smem, waves, n_chunks_max, a, st)
-                                   : route_shape<false>(cfg, M, merge, smem, waves, n_chunks_max, a, st);
+        const size_t smem = route_hist_smem(rs, field_desc != nullptr, a.m, n_bins, C, cfg.nw, cfg.ks);
+        cudaError_t e;
+        switch (field_desc ? tp_stride / 16 : 0) {               // packed: granules per record, a compile-time gather geometry
+            case 1: e = route_shape<1>(cfg, M, merge, smem, waves, n_chunks_max, a, st); break;
+            case 2: e = route_shape<2>(cfg, M, merge, smem, waves, n_chunks_max, a, st); break;
+            case 3: e = route_shape<3>(cfg, M, merge, smem, waves, n_chunks_max, a, st); break;
+            case 4: e = route_shape<4>(cfg, M, merge, smem, waves, n_chunks_max, a, st); break;
+            default: e = route_shape<0>(cfg, M, merge, smem, waves, n_chunks_max, a, st); break;
+        }
         if (e != cudaSuccess) { set_error("route_hist_level: %s", cudaGetErrorString(e)); return B200FLOW_ERR_CUDA; }
     }
     return check_launch("route_hist_level");
