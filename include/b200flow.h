@@ -360,9 +360,23 @@ int b200flow_gather_rows(const void* src, int32_t row_bytes, const int32_t* idx,
 int b200flow_confusion(const double* pred, const double* label, int64_t n_rows, int32_t C,
                        int64_t* cm, void* stream);
 
+/* Model selection (CrossValidator / TrainValidationSplit over numTrees x maxDepth, DESIGN.md §5a): confusion matrices of
+ * every truncated forest (first T_i trees, cut at depth d_j) on the validation records, from ONE walk of each tree.
+ * tp[n_rows][tp_stride] = UNIQUE binned records with the label at byte F; mult[n_rows] = rows per unique record.
+ * tree_cuts_host: 1 <= T_1 < ... < T_I <= T (I <= 256); depth_cuts_host: 0 <= d_1 < ... < d_J <= 30.
+ * cm int64 [I][J][cm_side][cm_side] (cm_side >= C, caller zeroes): cm[i][j][label][pred] += mult, where pred is what
+ * b200flow_predict gives for the truncated forest; labels >= cm_side are not counted.  max_depth_cuts_per_launch: 0 = as many
+ * as shared memory holds (the result does not depend on it). */
+int b200flow_predict_grid_confusion(const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows, const int32_t* mult,
+                                    const b200flow_node* nodes, const uint64_t* node_mask, const double* leaf_prob,
+                                    const uint32_t* pool_counts, int32_t T, int32_t C, int32_t dt_mode,
+                                    const void* top_nodes, int32_t top_levels, const int32_t* tree_cuts_host,
+                                    int32_t n_tree_cuts, const int32_t* depth_cuts_host, int32_t n_depth_cuts,
+                                    int32_t cm_side, int32_t max_depth_cuts_per_launch, int64_t* cm, void* stream);
+
 /* -------------------------------------------------- either side of the path ---
  * DataFrame.randomSplit (kdd99.py:52, cicids17.py:56): split id per row from a uniform keyed
- * by (seed, global row): first k with u < cum_bounds[k] (n_splits <= 8).  out uint8[n]. */
+ * by (seed, global row): first k with u < cum_bounds[k] (n_splits <= 32).  out uint8[n]. */
 int b200flow_random_split(uint64_t seed, int64_t row_offset, int64_t n_rows,
                           const double* cum_bounds_host, int32_t n_splits, uint8_t* split_id,
                           void* stream);

@@ -66,6 +66,8 @@ _SIGNATURES = {
     "b200flow_build_top_nodes": [_P, _P, _I64, _I32, _I32, _P, _P],
     "b200flow_gather_rows": [_P, _I32, _P, _I64, _P, _P],
     "b200flow_confusion": [_P, _P, _I64, _I32, _P, _P],
+    "b200flow_predict_grid_confusion": [_P, _I32, _I32, _I64, _P, _P, _P, _P, _P, _I32, _I32, _I32, _P, _I32, _P, _I32, _P, _I32,
+                                        _I32, _I32, _P, _P],
     "b200flow_random_split": [_U64, _I64, _I64, _P, _I32, _P, _P],
     "b200flow_compact_rows": [_P, _I64, _I32, _P, _I32, _P, _P, _P, _P],
     "b200flow_csv_count_lines": [_P, _I64, _P, _P, _P],

@@ -301,6 +301,45 @@ class ForestModel:
             return out
         return spread(raw_u, self.C), spread(prob_u, self.C), spread(pred_u, 1)
 
+    def grid_confusion(self, x_or_records, tree_cuts, depth_cuts, labels=None, plan=None, round_f32=False, cm_side=None,
+                       group=None, max_depth_cuts_per_launch=0):
+        """confusion matrices of every truncated forest on labelled validation rows: -> int64 [I, J, S, S] (host), where
+        [i, j] counts (label, prediction) of the first tree_cuts[i] trees cut at depth depth_cuts[j] — exactly what
+        confusion_matrix(predict(...)) gives for the (tree_cuts[i], depth_cuts[j]) forest fitted on its own (DESIGN.md §5a).
+        Dense path: x [n, F] and int labels [n]; record path: raw records + an encode plan with its label column set.
+        S = max(C, cm_side); labels >= S are not counted.  Under torch.distributed the counts are summed over the ranks."""
+        from . import dist as bdist
+        tree_cuts = np.ascontiguousarray(sorted(set(int(t) for t in tree_cuts)), np.int32)
+        depth_cuts = np.ascontiguousarray(sorted(set(int(d) for d in depth_cuts)), np.int32)
+        if plan is None:
+            if labels is None:
+                raise ValueError("grid_confusion: the dense path needs the labels")
+            src = _DenseSource(x_or_records, labels)
+        else:
+            if plan.label is None:
+                raise ValueError("grid_confusion: the encode plan has no label column (EncodePlan.set_label)")
+            src = _RecordSource(x_or_records, plan, round_f32)
+        if src.F != self.F:
+            raise ValueError("expected %d features, got %d" % (self.F, src.F))
+        S = max(self.C, int(cm_side or 0))
+        dev = src.device
+        cm = torch.zeros((len(tree_cuts), len(depth_cuts), S, S), dtype=torch.int64, device=dev)
+        n = src.n
+        if n > 0:
+            bad = torch.zeros(2, dtype=torch.int32, device=dev)
+            tp, _ = src.bin(self.thresholds, self.n_thr, self._arity_dev, self.max_bins, bad)
+            tpu, uid, U = dedup_rows(tp, self.F + 1)        # a validation record's identity includes its label
+            gsize = torch.empty(U, dtype=torch.int32, device=dev); cursor = torch.empty(U, dtype=torch.int32, device=dev)
+            goff = torch.empty(U + 1, dtype=torch.int64, device=dev)
+            perm = torch.empty(n, dtype=torch.int32, device=dev); uperm = torch.empty(n, dtype=torch.int32, device=dev)
+            _timed("group_rows", "b200flow_group_rows", ptr(uid), n, U, ptr(gsize), ptr(goff), ptr(cursor), ptr(perm), ptr(uperm))
+            top, K = self._top_table()
+            _timed("predict_grid", "b200flow_predict_grid_confusion", ptr(tpu), tpu.shape[1], self.F, U, ptr(gsize), ptr(self.nodes),
+                   ptr(self.node_mask), ptr(self.leaf_prob), ptr(self.pool_counts), self.T, self.C, 1 if self.dt_mode else 0,
+                   ptr(top), K, tree_cuts.ctypes.data, len(tree_cuts), depth_cuts.ctypes.data, len(depth_cuts), S,
+                   int(max_depth_cuts_per_launch), ptr(cm))
+        return bdist.all_reduce_sum_(cm, group).cpu()
+
     def export(self):
         """Canonical host copy, nodes ordered by (tree, MLlib node id) — what parity tests compare."""
         n = self.n_nodes

@@ -148,8 +148,119 @@ __global__ void __launch_bounds__(256) confusion_kernel(const double* __restrict
     }
 }
 
+// ------------------------------------------------------------------ grid prediction -> confusion matrices (model selection)
+// For fixed other params, the forest fitted with (T, d) is the first T trees of the (T_max, d_max) forest cut at depth d
+// (DESIGN.md §5a).  One thread owns one UNIQUE validation record (label at byte F, multiplicity mult[row]) and walks each
+// tree once, down to a leaf or to the deepest depth cut of this launch.  The node met at depth cut j (or the leaf the walk
+// ended on above it) adds its payload to votes[j] in tree order, from 0.0: the fp64 adds predict_kernel performs for the
+// truncated forest.  After tree T_i - 1 the first argmax of every votes[j] (predict_kernel's `v > best` rule) is counted
+// into cm[i][j][label][pred].  A launch covers depth cuts [j0, j0 + jn) of J.
+constexpr int kGridMaxTreeCuts = 256;
+constexpr int kGridMaxDepthCuts = 31;                 // depths 0..30
+struct GridCuts { int32_t tree[kGridMaxTreeCuts]; int32_t depth[kGridMaxDepthCuts]; };
+
+__global__ void __launch_bounds__(128) predict_grid_kernel(const uint8_t* __restrict__ tp, int stride, int F, int64_t n,
+                                                           const int32_t* __restrict__ mult,
+                                                           const b200flow_node* __restrict__ nodes,
+                                                           const unsigned long long* __restrict__ node_mask,
+                                                           const double* __restrict__ leaf_prob,
+                                                           const uint32_t* __restrict__ pool_counts, int C, int dt_mode,
+                                                           const int4* __restrict__ top, int K, const GridCuts cuts, int I,
+                                                           int J, int j0, int jn, int L, unsigned long long* cm, int use_smem) {
+    extern __shared__ __align__(16) uint8_t sm[];
+    const int bd = blockDim.x, tid = threadIdx.x;
+    const int words = stride / 4;
+    uint32_t* binw = (uint32_t*)sm;                                           // [words][bd]
+    double* votes = (double*)(sm + (size_t)words * bd * 4);                   // [jn][C][bd]
+    const int topn = top ? (1 << K) : 0;
+    int4* topbuf = (int4*)(votes + (size_t)jn * C * bd);                      // [2][topn] when the top table is given
+    unsigned long long* sh_cm = (unsigned long long*)(topbuf + 2 * topn);     // [I][jn][L][L] when use_smem
+    const int T = cuts.tree[I - 1];
+    const int cm_cells = I * jn * L * L;
+    if (use_smem) { for (int i = tid; i < cm_cells; i += bd) sh_cm[i] = 0ull; __syncthreads(); }
+    auto stage_top = [&](int t, int buf) {
+        if (t < T) for (int i = tid; i < topn; i += bd) cp_async16(topbuf + (size_t)buf * topn + i, top + ((int64_t)t << K) + i);
+        cp_async_commit();
+    };
+    const int4* nodes4 = (const int4*)nodes;                                  // {feat, kind<<16|bin, left, nid}
+    const uint32_t* bw = binw + tid;                                          // this thread's column of the transposed bins
+    double* vt = votes + tid;
+    for (int64_t base = (int64_t)blockIdx.x * bd; base < n; base += (int64_t)gridDim.x * bd) {
+        const int64_t row = base + tid;
+        const bool live = row < n;
+        int lab = 0; unsigned long long w = 0;
+        if (live) {
+            const uint4* src = (const uint4*)(tp + row * stride);
+            for (int q = 0; q < words / 4; ++q) {
+                const uint4 v = ld_stream_u4(src + q);
+                binw[(4 * q + 0) * bd + tid] = v.x; binw[(4 * q + 1) * bd + tid] = v.y;
+                binw[(4 * q + 2) * bd + tid] = v.z; binw[(4 * q + 3) * bd + tid] = v.w;
+            }
+            lab = tp[row * stride + F];
+            w = (unsigned long long)mult[row];
+        }
+        for (int k = 0; k < jn * C; ++k) vt[(size_t)k * bd] = 0.0;
+        if (top) stage_top(0, 0);
+        int ic = 0;                                                           // next tree cut
+        for (int t = 0; t < T; ++t) {
+            const int4* tb = topbuf + (size_t)(t & 1) * topn;
+            if (top) {
+                cp_async_wait_all();
+                __syncthreads();                                              // table of tree t landed; everybody left tree t-1
+                stage_top(t + 1, (t + 1) & 1);
+            }
+            if (live) {
+                int idx = t; uint32_t nid = 1u; int4 nd = top ? tb[1] : __ldg(nodes4 + t);
+                int depth = 0, jj = 0;
+                auto add = [&](int node, int j) {
+                    double* v = vt + (size_t)j * C * bd;
+                    if (dt_mode) { for (int k = 0; k < C; ++k) v[(size_t)k * bd] += (double)pool_counts[(int64_t)node * C + k]; }
+                    else { for (int k = 0; k < C; ++k) v[(size_t)k * bd] += leaf_prob[(int64_t)node * C + k]; }
+                };
+                while (true) {
+                    if (cuts.depth[j0 + jj] == depth) { add(idx, jj); ++jj; }  // cuts ascend: at most one per depth
+                    if (jj == jn || nd.x < 0) break;
+                    const int f = nd.x;
+                    const int bin = (bw[(f >> 2) * bd] >> ((f & 3) * 8)) & 0xff;
+                    const int right = nd.y < 65536 ? (bin > nd.y)
+                                                    : !((node_mask[(int64_t)idx * 4 + (bin >> 6)] >> (bin & 63)) & 1ull);
+                    idx = nd.z + right;
+                    nid = 2u * nid + (uint32_t)right;
+                    ++depth;
+                    nd = nid < (uint32_t)topn ? tb[nid] : __ldg(nodes4 + idx);
+                }
+                for (; jj < jn; ++jj) add(idx, jj);                           // a leaf above the remaining cuts
+            }
+            if (t + 1 == cuts.tree[ic]) {
+                if (live && lab < L) {
+                    for (int j = 0; j < jn; ++j) {
+                        const double* v = vt + (size_t)j * C * bd;
+                        int arg = 0; double best = v[0];
+                        for (int k = 0; k < C; ++k) { const double x = v[(size_t)k * bd]; if (x > best) { best = x; arg = k; } }
+                        const int64_t cell = (((int64_t)ic * jn + j) * L + lab) * L + arg;
+                        if (use_smem) atomicAdd(&sh_cm[cell], w);
+                        else atomicAdd(&cm[((((int64_t)ic * J + j0 + j) * L + lab) * L) + arg], w);
+                    }
+                }
+                ++ic;
+            }
+        }
+        if (top) { cp_async_wait_all(); __syncthreads(); }                  // the look-ahead copy of the last tree is a no-op commit
+    }
+    if (use_smem) {
+        __syncthreads();
+        for (int c = tid; c < cm_cells; c += bd) {
+            const unsigned long long v = sh_cm[c];
+            if (!v) continue;
+            const int p = c % L, l = (c / L) % L, j = (c / (L * L)) % jn, i = c / (L * L * jn);
+            atomicAdd(&cm[(((int64_t)i * J + j0 + j) * L + l) * L + p], v);
+        }
+    }
+}
+
 // ------------------------------------------------------------------ randomSplit
-struct SplitBounds { double cum[8]; int n; };
+constexpr int kMaxSplits = 32;                     // randomSplit weights / CrossValidator folds
+struct SplitBounds { double cum[kMaxSplits]; int n; };
 
 __global__ void __launch_bounds__(256) random_split_kernel(uint64_t seed, int64_t row_offset, int64_t n, SplitBounds bnd,
                                                            uint8_t* out) {
@@ -267,12 +378,74 @@ extern "C" int b200flow_confusion(const double* pred, const double* label, int64
     return check_launch("confusion");
 }
 
+extern "C" int b200flow_predict_grid_confusion(const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows, const int32_t* mult,
+                                               const b200flow_node* nodes, const uint64_t* node_mask, const double* leaf_prob,
+                                               const uint32_t* pool_counts, int32_t T, int32_t C, int32_t dt_mode,
+                                               const void* top_nodes, int32_t top_levels, const int32_t* tree_cuts_host,
+                                               int32_t n_tree_cuts, const int32_t* depth_cuts_host, int32_t n_depth_cuts,
+                                               int32_t cm_side, int32_t max_depth_cuts_per_launch, int64_t* cm, void* stream) {
+    const int I = n_tree_cuts, J = n_depth_cuts, L = cm_side;
+    B2F_REQUIRE(tree_cuts_host && depth_cuts_host && I >= 1 && I <= kGridMaxTreeCuts && J >= 1 && J <= kGridMaxDepthCuts,
+                "predict_grid_confusion: 1..%d tree cuts and 1..%d depth cuts", kGridMaxTreeCuts, kGridMaxDepthCuts);
+    GridCuts cuts;
+    for (int i = 0; i < I; ++i) {
+        B2F_REQUIRE(tree_cuts_host[i] >= 1 && tree_cuts_host[i] <= T && (i == 0 || tree_cuts_host[i] > tree_cuts_host[i - 1]),
+                    "predict_grid_confusion: tree cuts must ascend strictly within [1, %d]", T);
+        cuts.tree[i] = tree_cuts_host[i];
+    }
+    for (int j = 0; j < J; ++j) {
+        B2F_REQUIRE(depth_cuts_host[j] >= 0 && depth_cuts_host[j] <= 30 && (j == 0 || depth_cuts_host[j] > depth_cuts_host[j - 1]),
+                    "predict_grid_confusion: depth cuts must ascend strictly within [0, 30]");
+        cuts.depth[j] = depth_cuts_host[j];
+    }
+    if (n_rows <= 0) return B200FLOW_OK;            // empty shard: nothing to count (pointers may be NULL)
+    B2F_REQUIRE(tp && mult && nodes && cm && T > 0 && C > 0 && L >= C && F >= 0 && F < tp_stride && (tp_stride & 15) == 0,
+                "predict_grid_confusion: bad arguments");
+    B2F_REQUIRE(dt_mode ? pool_counts != nullptr : leaf_prob != nullptr, "predict_grid_confusion: missing leaf payload");
+    B2F_REQUIRE(((uintptr_t)tp & 15) == 0, "predict_grid_confusion: tp must be 16-byte aligned");
+    B2F_REQUIRE(!top_nodes || (top_levels >= 1 && top_levels <= 10 && ((uintptr_t)top_nodes & 15) == 0),
+                "predict_grid_confusion: bad top table");
+    // shared memory per launch: transposed bins + votes of jc depth cuts per thread, the top table, and the confusion
+    // matrices of the launch when they fit as well.  The widest block that holds every depth cut is taken; when not even 32
+    // threads hold them, the depth cuts are split over launches (each launch walks the trees again; counts do not change).
+    const size_t kBudget = 200 * 1024;
+    const size_t top_bytes = top_nodes ? (size_t)2 * 16 * ((size_t)1 << top_levels) : 0;
+    const int want = max_depth_cuts_per_launch > 0 && max_depth_cuts_per_launch < J ? max_depth_cuts_per_launch : J;
+    auto cuts_that_fit = [&](int bd) -> int {
+        const size_t fixed = (size_t)bd * tp_stride + top_bytes;
+        if (fixed >= kBudget) return 0;
+        const size_t per_cut = (size_t)bd * C * 8;
+        return (int)((kBudget - fixed) / per_cut < (size_t)want ? (kBudget - fixed) / per_cut : (size_t)want);
+    };
+    int bd = 128;
+    while (bd > 32 && cuts_that_fit(bd) < want) bd >>= 1;
+    const int jc = cuts_that_fit(bd);
+    B2F_REQUIRE(jc >= 1, "predict_grid_confusion: too many classes/features for shared memory");
+    const int grid = grid_for(n_rows, bd, kNumSMs * 16);
+    for (int j0 = 0; j0 < J; j0 += jc) {
+        const int jn = J - j0 < jc ? J - j0 : jc;
+        size_t smem = (size_t)bd * ((size_t)tp_stride + (size_t)jn * C * 8) + top_bytes;
+        const size_t cm_bytes = (size_t)I * jn * L * L * 8;
+        const int use_smem = smem + cm_bytes <= kBudget;
+        if (use_smem) smem += cm_bytes;
+        cudaError_t e = cudaFuncSetAttribute(predict_grid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) { set_error("predict_grid_confusion: %s", cudaGetErrorString(e)); return B200FLOW_ERR_CUDA; }
+        predict_grid_kernel<<<grid, bd, smem, (cudaStream_t)stream>>>(tp, tp_stride, F, n_rows, mult, nodes,
+                                                                      (const unsigned long long*)node_mask, leaf_prob, pool_counts, C,
+                                                                      dt_mode, (const int4*)top_nodes, top_levels, cuts, I, J, j0, jn,
+                                                                      L, (unsigned long long*)cm, use_smem);
+        const int rc = check_launch("predict_grid_confusion");
+        if (rc) return rc;
+    }
+    return B200FLOW_OK;
+}
+
 extern "C" int b200flow_random_split(uint64_t seed, int64_t row_offset, int64_t n_rows, const double* cum_bounds_host,
                                      int32_t n_splits, uint8_t* split_id, void* stream) {
     if (n_rows <= 0) return B200FLOW_OK;            // empty batch: nothing to do (pointers may be NULL)
-    B2F_REQUIRE(cum_bounds_host && split_id && n_splits >= 1 && n_splits <= 8, "random_split: bad arguments");
+    B2F_REQUIRE(cum_bounds_host && split_id && n_splits >= 1 && n_splits <= kMaxSplits, "random_split: bad arguments");
     SplitBounds b; b.n = n_splits;
-    for (int i = 0; i < 8; ++i) b.cum[i] = i < n_splits ? cum_bounds_host[i] : 2.0;
+    for (int i = 0; i < kMaxSplits; ++i) b.cum[i] = i < n_splits ? cum_bounds_host[i] : 2.0;
     int grid = grid_for(n_rows, 256 * 4, kNumSMs * 8);
     random_split_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(seed, row_offset, n_rows, b, split_id);
     return check_launch("random_split");

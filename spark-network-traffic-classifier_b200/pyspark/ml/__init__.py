@@ -1,5 +1,5 @@
 """pyspark.ml shim: Estimator / Transformer / Model / Pipeline (kdd99.py:36-37)."""
-from .param import Params
+from .param import Param, Params
 
 
 class Transformer(Params):
@@ -9,6 +9,9 @@ class Transformer(Params):
 
 class Estimator(Params):
     def fit(self, dataset, params=None):
+        """params: a param map (keyed by names or Params) applied to a copy, or a list / tuple of maps -> one model each."""
+        if isinstance(params, (list, tuple)):
+            return [self.fit(dataset, p) for p in params]
         return (self.copy(params) if params else self)._fit(dataset)
 
 
@@ -25,6 +28,14 @@ class Pipeline(Estimator):
 
     def getStages(self):
         return list(self.getOrDefault("stages") or [])
+
+    def copy(self, extra=None):
+        """as in pyspark, the Params of a map reach the stages that own them (fit(df, {rf.numTrees: 50}) on a pipeline)."""
+        c = super().copy(extra)
+        staged = {k: v for k, v in (extra or {}).items() if isinstance(k, Param)}
+        if staged and c.getOrDefault("stages") is not None:
+            c._paramMap["stages"] = [s.copy(staged) for s in c.getStages()]
+        return c
 
     def _fit(self, dataset):
         stages = self.getStages()
