@@ -373,6 +373,37 @@ int b200flow_predict_grid_confusion(const uint8_t* tp, int32_t tp_stride, int32_
                                     const void* top_nodes, int32_t top_levels, const int32_t* tree_cuts_host,
                                     int32_t n_tree_cuts, const int32_t* depth_cuts_host, int32_t n_depth_cuts,
                                     int32_t cm_side, int32_t max_depth_cuts_per_launch, int64_t* cm, void* stream);
+/* The same walk, for BinaryClassificationEvaluator: scores double [I][J][n_rows] (device) gets votes[1] of every truncated
+ * forest for every record — rawPrediction[1] of that (tree_cuts[i], depth_cuts[j]) forest fitted on its own, bit for bit.
+ * C >= 2; the records' label byte and multiplicities are not read. */
+int b200flow_predict_grid_scores(const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows,
+                                 const b200flow_node* nodes, const uint64_t* node_mask, const double* leaf_prob,
+                                 const uint32_t* pool_counts, int32_t T, int32_t C, int32_t dt_mode,
+                                 const void* top_nodes, int32_t top_levels, const int32_t* tree_cuts_host,
+                                 int32_t n_tree_cuts, const int32_t* depth_cuts_host, int32_t n_depth_cuts,
+                                 int32_t max_depth_cuts_per_launch, double* scores, void* stream);
+
+/* BinaryClassificationMetrics (BinaryClassificationEvaluator areaUnderROC / areaUnderPR, DESIGN.md §5b).
+ * b200flow_binary_counts: S segments (1 <= S <= 65536, S * n < 2^32) of n fp64 scores, segment s at scores + s * score_stride;
+ * int32 positive / negative counts per item at pos / neg + s * count_stride + i (count_stride 0: every segment shares them).
+ * Items with pos + neg == 0 are ignored; a NaN score with a non-zero count is counted into *n_nan (device int64) and ignored.
+ * Writes the distinct scores of every segment in DESCENDING order (-0.0 == +0.0) with their summed counts:
+ * d_score / d_pos / d_neg [S][cap] (cap >= n, entries past n_distinct[s] untouched) and n_distinct int64 [S] (device).
+ * scratch: device, 256-byte aligned, b200flow_binary_counts_scratch(S, n) bytes (host-only query, no device needed).
+ * Integer counts throughout: the result does not depend on the order of the items. */
+int b200flow_binary_counts_scratch(int32_t S, int64_t n, int64_t* scratch_bytes);
+int b200flow_binary_counts(const double* scores, int64_t score_stride, const int32_t* pos, const int32_t* neg,
+                           int64_t count_stride, int32_t S, int64_t n, void* scratch, int64_t scratch_bytes,
+                           double* d_score, int64_t* d_pos, int64_t* d_neg, int64_t cap, int64_t* n_distinct,
+                           int64_t* n_nan, void* stream);
+/* b200flow_binary_curve: distinct triples (as binary_counts writes them) -> auc[S][2] = {areaUnderROC, areaUnderPR} and the
+ * curve points c_score / c_tp / c_fp [S][cap] (score, cumulative positives, cumulative negatives), c_n[S] of them.  num_bins
+ * >= 0 down-samples as Spark does (g = n_distinct / num_bins; g >= 2 keeps ranks g-1, 2g-1, ... and the last).  Each area
+ * is summed sequentially from 0.0 in curve order.  work: 2 * S * cap doubles of device scratch.  A segment with no
+ * distinct score gets NaN areas. */
+int b200flow_binary_curve(const double* d_score, const int64_t* d_pos, const int64_t* d_neg, int64_t cap,
+                          const int64_t* n_distinct, int32_t S, int32_t num_bins, double* auc, double* c_score,
+                          int64_t* c_tp, int64_t* c_fp, int64_t* c_n, double* work, void* stream);
 
 /* -------------------------------------------------- either side of the path ---
  * DataFrame.randomSplit (kdd99.py:52, cicids17.py:56): split id per row from a uniform keyed

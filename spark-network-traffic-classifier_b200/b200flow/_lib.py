@@ -68,6 +68,10 @@ _SIGNATURES = {
     "b200flow_confusion": [_P, _P, _I64, _I32, _P, _P],
     "b200flow_predict_grid_confusion": [_P, _I32, _I32, _I64, _P, _P, _P, _P, _P, _I32, _I32, _I32, _P, _I32, _P, _I32, _P, _I32,
                                         _I32, _I32, _P, _P],
+    "b200flow_predict_grid_scores": [_P, _I32, _I32, _I64, _P, _P, _P, _P, _I32, _I32, _I32, _P, _I32, _P, _I32, _P, _I32, _I32,
+                                     _P],
+    "b200flow_binary_counts": [_P, _I64, _P, _P, _I64, _I32, _I64, _P, _I64, _P, _P, _P, _I64, _P, _P, _P],
+    "b200flow_binary_curve": [_P, _P, _P, _I64, _P, _I32, _I32, _P, _P, _P, _P, _P, _P, _P],
     "b200flow_random_split": [_U64, _I64, _I64, _P, _I32, _P, _P],
     "b200flow_compact_rows": [_P, _I64, _I32, _P, _I32, _P, _P, _P, _P],
     "b200flow_csv_count_lines": [_P, _I64, _P, _P, _P],
@@ -77,7 +81,7 @@ _SIGNATURES = {
     "b200flow_csv_parse": [_P, _I64, _P, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _P, _I32, _P, _P],
 }
 EXPORTS = sorted(list(_SIGNATURES) + ["b200flow_last_error", "b200flow_version", "b200flow_route_hist_config",
-                                       "b200flow_packed_layout"])
+                                       "b200flow_packed_layout", "b200flow_binary_counts_scratch"])
 
 _lib = None
 launches = 0   # kernels of OURS launched so far (counted per C-ABI call); bench.py reads the delta over the timed region
@@ -103,6 +107,8 @@ def load():
         lib.b200flow_route_hist_config.restype = C.c_int
         lib.b200flow_packed_layout.argtypes = [_I32, _P, _I32, _P, C.POINTER(_I32)]
         lib.b200flow_packed_layout.restype = C.c_int
+        lib.b200flow_binary_counts_scratch.argtypes = [_I32, _I64, C.POINTER(_I64)]
+        lib.b200flow_binary_counts_scratch.restype = C.c_int
         _lib = lib
     return _lib
 
@@ -125,6 +131,15 @@ def packed_layout(feat_bins, n_classes):
     if lib.b200flow_packed_layout(int(fb.shape[0]), fb.ctypes.data, int(n_classes), desc.ctypes.data, C.byref(rb)) != 0:
         raise B200FlowError("b200flow_packed_layout failed: %s" % lib.b200flow_last_error().decode())
     return desc, int(rb.value)
+
+
+def binary_counts_scratch(S, n):
+    """bytes of device scratch b200flow_binary_counts needs for S segments of n scores (host-only call)."""
+    out = _I64(0)
+    lib = load()
+    if lib.b200flow_binary_counts_scratch(int(S), int(n), C.byref(out)) != 0:
+        raise B200FlowError("b200flow_binary_counts_scratch failed: %s" % lib.b200flow_last_error().decode())
+    return int(out.value)
 
 
 def ptr(t):

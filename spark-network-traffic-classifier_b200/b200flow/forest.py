@@ -340,6 +340,71 @@ class ForestModel:
                    int(max_depth_cuts_per_launch), ptr(cm))
         return bdist.all_reduce_sum_(cm, group).cpu()
 
+    GRID_SCORE_BUDGET = 2 << 30            # bytes of [tree cuts, J, U] fp64 scores per grid_binary_metrics block
+
+    def grid_binary_metrics(self, x_or_records, tree_cuts, depth_cuts, labels=None, plan=None, num_bins=1000, group=None,
+                            round_f32=False, max_depth_cuts_per_launch=0):
+        """areaUnderROC / areaUnderPR of every truncated forest on labelled validation rows: -> float64 [I, J, 2] (host), where
+        [i, j] is what BinaryClassificationEvaluator(numBins=num_bins) gives on rawPrediction[1] of the (tree_cuts[i],
+        depth_cuts[j]) forest fitted on its own (DESIGN.md §5a, §5b).  A row is positive iff its label >= 1.  The rows are
+        de-duplicated on (bins, label) with their multiplicities as integer counts, predict_grid_scores writes every grid
+        point's score per distinct record, and binary_metrics runs over the I·J segments (in blocks of tree cuts when the
+        scores would exceed GRID_SCORE_BUDGET bytes).  Under torch.distributed every rank returns the same bits."""
+        from . import dist as bdist
+        from .metrics import binary_metrics
+        if self.C < 2:
+            raise ValueError("grid_binary_metrics: the score is rawPrediction[1], the forest has %d class(es)" % self.C)
+        tree_cuts = np.ascontiguousarray(sorted(set(int(t) for t in tree_cuts)), np.int32)
+        depth_cuts = np.ascontiguousarray(sorted(set(int(d) for d in depth_cuts)), np.int32)
+        if plan is None:
+            if labels is None:
+                raise ValueError("grid_binary_metrics: the dense path needs the labels")
+            src = _DenseSource(x_or_records, labels)
+        else:
+            if plan.label is None:
+                raise ValueError("grid_binary_metrics: the encode plan has no label column (EncodePlan.set_label)")
+            src = _RecordSource(x_or_records, plan, round_f32)
+        if src.F != self.F:
+            raise ValueError("expected %d features, got %d" % (self.F, src.F))
+        dev = src.device
+        I, J = len(tree_cuts), len(depth_cuts)
+        U = 0
+        if src.n > 0:
+            bad = torch.zeros(2, dtype=torch.int32, device=dev)
+            tp, _ = src.bin(self.thresholds, self.n_thr, self._arity_dev, self.max_bins, bad)
+            tpu, uid, U = dedup_rows(tp, self.F + 1)        # a validation record's identity includes its label
+            tpu = tpu.contiguous()
+            gsize = torch.empty(U, dtype=torch.int32, device=dev); cursor = torch.empty(U, dtype=torch.int32, device=dev)
+            goff = torch.empty(U + 1, dtype=torch.int64, device=dev)
+            perm = torch.empty(src.n, dtype=torch.int32, device=dev); uperm = torch.empty(src.n, dtype=torch.int32, device=dev)
+            _timed("group_rows", "b200flow_group_rows", ptr(uid), src.n, U, ptr(gsize), ptr(goff), ptr(cursor), ptr(perm), ptr(uperm))
+            positive = tpu[:, self.F] >= 1
+            pos = torch.where(positive, gsize, 0).contiguous()
+            neg = torch.where(positive, 0, gsize).contiguous()
+        else:
+            pos = neg = torch.zeros(0, dtype=torch.int32, device=dev)
+        mx = torch.tensor([U], dtype=torch.int64, device=dev)   # every rank takes the same blocks: size them by the widest shard
+        grp = group if group is not None else bdist.group()
+        if grp is not None:
+            import torch.distributed as dist
+            bdist.all_reduce_(mx, grp, op=dist.ReduceOp.MAX)
+        per_cut = J * max(int(mx.item()), 1) * 8
+        step = max(1, min(I, self.GRID_SCORE_BUDGET // per_cut))
+        out = np.empty((I, J, 2), np.float64)
+        top, K = self._top_table()
+        for i0 in range(0, I, step):
+            cuts = np.ascontiguousarray(tree_cuts[i0:i0 + step])
+            scores = torch.empty((len(cuts), J, U), dtype=torch.float64, device=dev)
+            if U > 0:
+                _timed("predict_grid", "b200flow_predict_grid_scores", ptr(tpu), tpu.shape[1], self.F, U, ptr(self.nodes),
+                       ptr(self.node_mask), ptr(self.leaf_prob), ptr(self.pool_counts), self.T, self.C, 1 if self.dt_mode else 0,
+                       ptr(top), K, cuts.ctypes.data, len(cuts), depth_cuts.ctypes.data, J, int(max_depth_cuts_per_launch),
+                       ptr(scores))
+            r = binary_metrics(scores.reshape(len(cuts) * J, U), pos=pos, neg=neg, num_bins=num_bins, group=grp)
+            out[i0:i0 + len(cuts), :, 0] = np.asarray(r["areaUnderROC"]).reshape(len(cuts), J)
+            out[i0:i0 + len(cuts), :, 1] = np.asarray(r["areaUnderPR"]).reshape(len(cuts), J)
+        return out
+
     def export(self):
         """Canonical host copy, nodes ordered by (tree, MLlib node id) — what parity tests compare."""
         n = self.n_nodes
@@ -820,8 +885,10 @@ def confusion_matrix(pred, label, C):
     return cm
 
 
-def metrics_from_confusion(cm):
-    """MulticlassMetrics (A.8) + macro-F1 from the C x C counts (host, C^2 numbers)."""
+def metrics_from_confusion(cm, metric_label=0.0, beta=1.0):
+    """MulticlassMetrics (A.8) + macro-F1 from the C x C counts (host, C^2 numbers).  L = the true labels with support > 0.
+    The by-label metrics (…ByLabel) are for metric_label and are left out when it is not in L (Spark's tpByClass(label)
+    raises); fMeasure uses beta.  fpr(l) = fp(l) / (N - support(l)) is an IEEE division (0/0 is NaN, as on the JVM)."""
     cm = np.asarray(cm, np.float64)
     N = cm.sum()
     sup = cm.sum(1); predl = cm.sum(0); tp = np.diag(cm)
@@ -830,7 +897,19 @@ def metrics_from_confusion(cm):
         p = np.where(predl > 0, tp / predl, 0.0)
         r = np.where(sup > 0, tp / sup, 0.0)
         f1 = np.where(p + r > 0, 2 * p * r / (p + r), 0.0)
+        b2 = beta * beta
+        fb = np.where(p + r > 0, (1 + b2) * p * r / (b2 * p + r), 0.0)
+        fpr = (predl - tp) / (N - sup)
     w = sup / N if N else sup
-    return dict(accuracy=float(tp[labs].sum() / N) if N else 0.0,
-                weightedPrecision=float((p * w)[labs].sum()), weightedRecall=float((r * w)[labs].sum()),
-                f1=float((f1 * w)[labs].sum()), macroF1=float(f1[labs].mean()) if labs.any() else 0.0)
+    out = dict(accuracy=float(tp[labs].sum() / N) if N else 0.0,
+               weightedPrecision=float((p * w)[labs].sum()), weightedRecall=float((r * w)[labs].sum()),
+               f1=float((f1 * w)[labs].sum()), macroF1=float(f1[labs].mean()) if labs.any() else 0.0)
+    out.update(weightedTruePositiveRate=out["weightedRecall"], weightedFalsePositiveRate=float((fpr * w)[labs].sum()),
+               weightedFMeasure=float((fb * w)[labs].sum()),
+               hammingLoss=float((N - tp.sum()) / N) if N else 0.0)
+    ml = float(metric_label)
+    li = int(ml) if np.isfinite(ml) and ml == int(ml) else -1
+    if 0 <= li < cm.shape[0] and labs[li]:
+        out.update(truePositiveRateByLabel=float(r[li]), falsePositiveRateByLabel=float(fpr[li]), precisionByLabel=float(p[li]),
+                   recallByLabel=float(r[li]), fMeasureByLabel=float(fb[li]))
+    return out

@@ -159,6 +159,9 @@ constexpr int kGridMaxTreeCuts = 256;
 constexpr int kGridMaxDepthCuts = 31;                 // depths 0..30
 struct GridCuts { int32_t tree[kGridMaxTreeCuts]; int32_t depth[kGridMaxDepthCuts]; };
 
+// kScores: instead of counting argmaxes, write votes[1] of every (tree cut, depth cut) to scores[i][j][row] — rawPrediction[1]
+// of that truncated forest, the score BinaryClassificationEvaluator reads (mult and cm are not used).
+template <bool kScores>
 __global__ void __launch_bounds__(128) predict_grid_kernel(const uint8_t* __restrict__ tp, int stride, int F, int64_t n,
                                                            const int32_t* __restrict__ mult,
                                                            const b200flow_node* __restrict__ nodes,
@@ -166,7 +169,8 @@ __global__ void __launch_bounds__(128) predict_grid_kernel(const uint8_t* __rest
                                                            const double* __restrict__ leaf_prob,
                                                            const uint32_t* __restrict__ pool_counts, int C, int dt_mode,
                                                            const int4* __restrict__ top, int K, const GridCuts cuts, int I,
-                                                           int J, int j0, int jn, int L, unsigned long long* cm, int use_smem) {
+                                                           int J, int j0, int jn, int L, unsigned long long* cm, int use_smem,
+                                                           double* scores) {
     extern __shared__ __align__(16) uint8_t sm[];
     const int bd = blockDim.x, tid = threadIdx.x;
     const int words = stride / 4;
@@ -196,8 +200,10 @@ __global__ void __launch_bounds__(128) predict_grid_kernel(const uint8_t* __rest
                 binw[(4 * q + 0) * bd + tid] = v.x; binw[(4 * q + 1) * bd + tid] = v.y;
                 binw[(4 * q + 2) * bd + tid] = v.z; binw[(4 * q + 3) * bd + tid] = v.w;
             }
-            lab = tp[row * stride + F];
-            w = (unsigned long long)mult[row];
+            if (!kScores) {
+                lab = tp[row * stride + F];
+                w = (unsigned long long)mult[row];
+            }
         }
         for (int k = 0; k < jn * C; ++k) vt[(size_t)k * bd] = 0.0;
         if (top) stage_top(0, 0);
@@ -232,7 +238,12 @@ __global__ void __launch_bounds__(128) predict_grid_kernel(const uint8_t* __rest
                 for (; jj < jn; ++jj) add(idx, jj);                           // a leaf above the remaining cuts
             }
             if (t + 1 == cuts.tree[ic]) {
-                if (live && lab < L) {
+                if (kScores) {
+                    if (live) {
+                        double* out = scores + ((int64_t)ic * J + j0) * n + row;
+                        for (int j = 0; j < jn; ++j) out[(int64_t)j * n] = vt[((size_t)j * C + 1) * bd];
+                    }
+                } else if (live && lab < L) {
                     for (int j = 0; j < jn; ++j) {
                         const double* v = vt + (size_t)j * C * bd;
                         int arg = 0; double best = v[0];
@@ -378,33 +389,37 @@ extern "C" int b200flow_confusion(const double* pred, const double* label, int64
     return check_launch("confusion");
 }
 
-extern "C" int b200flow_predict_grid_confusion(const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows, const int32_t* mult,
-                                               const b200flow_node* nodes, const uint64_t* node_mask, const double* leaf_prob,
-                                               const uint32_t* pool_counts, int32_t T, int32_t C, int32_t dt_mode,
-                                               const void* top_nodes, int32_t top_levels, const int32_t* tree_cuts_host,
-                                               int32_t n_tree_cuts, const int32_t* depth_cuts_host, int32_t n_depth_cuts,
-                                               int32_t cm_side, int32_t max_depth_cuts_per_launch, int64_t* cm, void* stream) {
+// the launches of predict_grid_kernel<kScores> (confusion matrices, or scores) over the depth cuts
+template <bool kScores>
+static int predict_grid_launch(const char* what, const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows, const int32_t* mult,
+                               const b200flow_node* nodes, const uint64_t* node_mask, const double* leaf_prob,
+                               const uint32_t* pool_counts, int32_t T, int32_t C, int32_t dt_mode,
+                               const void* top_nodes, int32_t top_levels, const int32_t* tree_cuts_host,
+                               int32_t n_tree_cuts, const int32_t* depth_cuts_host, int32_t n_depth_cuts,
+                               int32_t cm_side, int32_t max_depth_cuts_per_launch, int64_t* cm, double* scores, void* stream) {
     const int I = n_tree_cuts, J = n_depth_cuts, L = cm_side;
     B2F_REQUIRE(tree_cuts_host && depth_cuts_host && I >= 1 && I <= kGridMaxTreeCuts && J >= 1 && J <= kGridMaxDepthCuts,
-                "predict_grid_confusion: 1..%d tree cuts and 1..%d depth cuts", kGridMaxTreeCuts, kGridMaxDepthCuts);
+                "%s: 1..%d tree cuts and 1..%d depth cuts", what, kGridMaxTreeCuts, kGridMaxDepthCuts);
     GridCuts cuts;
     for (int i = 0; i < I; ++i) {
         B2F_REQUIRE(tree_cuts_host[i] >= 1 && tree_cuts_host[i] <= T && (i == 0 || tree_cuts_host[i] > tree_cuts_host[i - 1]),
-                    "predict_grid_confusion: tree cuts must ascend strictly within [1, %d]", T);
+                    "%s: tree cuts must ascend strictly within [1, %d]", what, T);
         cuts.tree[i] = tree_cuts_host[i];
     }
     for (int j = 0; j < J; ++j) {
         B2F_REQUIRE(depth_cuts_host[j] >= 0 && depth_cuts_host[j] <= 30 && (j == 0 || depth_cuts_host[j] > depth_cuts_host[j - 1]),
-                    "predict_grid_confusion: depth cuts must ascend strictly within [0, 30]");
+                    "%s: depth cuts must ascend strictly within [0, 30]", what);
         cuts.depth[j] = depth_cuts_host[j];
     }
     if (n_rows <= 0) return B200FLOW_OK;            // empty shard: nothing to count (pointers may be NULL)
-    B2F_REQUIRE(tp && mult && nodes && cm && T > 0 && C > 0 && L >= C && F >= 0 && F < tp_stride && (tp_stride & 15) == 0,
-                "predict_grid_confusion: bad arguments");
-    B2F_REQUIRE(dt_mode ? pool_counts != nullptr : leaf_prob != nullptr, "predict_grid_confusion: missing leaf payload");
-    B2F_REQUIRE(((uintptr_t)tp & 15) == 0, "predict_grid_confusion: tp must be 16-byte aligned");
+    if (kScores) B2F_REQUIRE(tp && nodes && scores && T > 0 && C >= 2 && F >= 0 && F < tp_stride && (tp_stride & 15) == 0,
+                             "predict_grid_scores: bad arguments (C >= 2: the score is votes[1])");
+    else B2F_REQUIRE(tp && mult && nodes && cm && T > 0 && C > 0 && L >= C && F >= 0 && F < tp_stride && (tp_stride & 15) == 0,
+                     "predict_grid_confusion: bad arguments");
+    B2F_REQUIRE(dt_mode ? pool_counts != nullptr : leaf_prob != nullptr, "%s: missing leaf payload", what);
+    B2F_REQUIRE(((uintptr_t)tp & 15) == 0, "%s: tp must be 16-byte aligned", what);
     B2F_REQUIRE(!top_nodes || (top_levels >= 1 && top_levels <= 10 && ((uintptr_t)top_nodes & 15) == 0),
-                "predict_grid_confusion: bad top table");
+                "%s: bad top table", what);
     // shared memory per launch: transposed bins + votes of jc depth cuts per thread, the top table, and the confusion
     // matrices of the launch when they fit as well.  The widest block that holds every depth cut is taken; when not even 32
     // threads hold them, the depth cuts are split over launches (each launch walks the trees again; counts do not change).
@@ -420,24 +435,47 @@ extern "C" int b200flow_predict_grid_confusion(const uint8_t* tp, int32_t tp_str
     int bd = 128;
     while (bd > 32 && cuts_that_fit(bd) < want) bd >>= 1;
     const int jc = cuts_that_fit(bd);
-    B2F_REQUIRE(jc >= 1, "predict_grid_confusion: too many classes/features for shared memory");
+    B2F_REQUIRE(jc >= 1, "%s: too many classes/features for shared memory", what);
     const int grid = grid_for(n_rows, bd, kNumSMs * 16);
     for (int j0 = 0; j0 < J; j0 += jc) {
         const int jn = J - j0 < jc ? J - j0 : jc;
         size_t smem = (size_t)bd * ((size_t)tp_stride + (size_t)jn * C * 8) + top_bytes;
-        const size_t cm_bytes = (size_t)I * jn * L * L * 8;
-        const int use_smem = smem + cm_bytes <= kBudget;
+        const size_t cm_bytes = kScores ? 0 : (size_t)I * jn * L * L * 8;
+        const int use_smem = !kScores && smem + cm_bytes <= kBudget;
         if (use_smem) smem += cm_bytes;
-        cudaError_t e = cudaFuncSetAttribute(predict_grid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) { set_error("predict_grid_confusion: %s", cudaGetErrorString(e)); return B200FLOW_ERR_CUDA; }
-        predict_grid_kernel<<<grid, bd, smem, (cudaStream_t)stream>>>(tp, tp_stride, F, n_rows, mult, nodes,
-                                                                      (const unsigned long long*)node_mask, leaf_prob, pool_counts, C,
-                                                                      dt_mode, (const int4*)top_nodes, top_levels, cuts, I, J, j0, jn,
-                                                                      L, (unsigned long long*)cm, use_smem);
-        const int rc = check_launch("predict_grid_confusion");
+        cudaError_t e = cudaFuncSetAttribute(predict_grid_kernel<kScores>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e != cudaSuccess) { set_error("%s: %s", what, cudaGetErrorString(e)); return B200FLOW_ERR_CUDA; }
+        predict_grid_kernel<kScores><<<grid, bd, smem, (cudaStream_t)stream>>>(tp, tp_stride, F, n_rows, mult, nodes,
+                                                                               (const unsigned long long*)node_mask, leaf_prob,
+                                                                               pool_counts, C, dt_mode, (const int4*)top_nodes,
+                                                                               top_levels, cuts, I, J, j0, jn, L,
+                                                                               (unsigned long long*)cm, use_smem, scores);
+        const int rc = check_launch(what);
         if (rc) return rc;
     }
     return B200FLOW_OK;
+}
+
+extern "C" int b200flow_predict_grid_confusion(const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows, const int32_t* mult,
+                                               const b200flow_node* nodes, const uint64_t* node_mask, const double* leaf_prob,
+                                               const uint32_t* pool_counts, int32_t T, int32_t C, int32_t dt_mode,
+                                               const void* top_nodes, int32_t top_levels, const int32_t* tree_cuts_host,
+                                               int32_t n_tree_cuts, const int32_t* depth_cuts_host, int32_t n_depth_cuts,
+                                               int32_t cm_side, int32_t max_depth_cuts_per_launch, int64_t* cm, void* stream) {
+    return predict_grid_launch<false>("predict_grid_confusion", tp, tp_stride, F, n_rows, mult, nodes, node_mask, leaf_prob,
+                                      pool_counts, T, C, dt_mode, top_nodes, top_levels, tree_cuts_host, n_tree_cuts,
+                                      depth_cuts_host, n_depth_cuts, cm_side, max_depth_cuts_per_launch, cm, nullptr, stream);
+}
+
+extern "C" int b200flow_predict_grid_scores(const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows,
+                                            const b200flow_node* nodes, const uint64_t* node_mask, const double* leaf_prob,
+                                            const uint32_t* pool_counts, int32_t T, int32_t C, int32_t dt_mode,
+                                            const void* top_nodes, int32_t top_levels, const int32_t* tree_cuts_host,
+                                            int32_t n_tree_cuts, const int32_t* depth_cuts_host, int32_t n_depth_cuts,
+                                            int32_t max_depth_cuts_per_launch, double* scores, void* stream) {
+    return predict_grid_launch<true>("predict_grid_scores", tp, tp_stride, F, n_rows, nullptr, nodes, node_mask, leaf_prob,
+                                     pool_counts, T, C, dt_mode, top_nodes, top_levels, tree_cuts_host, n_tree_cuts,
+                                     depth_cuts_host, n_depth_cuts, C, max_depth_cuts_per_launch, nullptr, scores, stream);
 }
 
 extern "C" int b200flow_random_split(uint64_t seed, int64_t row_offset, int64_t n_rows, const double* cum_bounds_host,

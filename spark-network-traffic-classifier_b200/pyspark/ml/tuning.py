@@ -1,10 +1,14 @@
 """pyspark.ml.tuning shim: ParamGridBuilder, CrossValidator and TrainValidationSplit.
 
 A RandomForestClassifier / DecisionTreeClassifier scored by a MulticlassClassificationEvaluator on the estimator's own label
-and prediction columns takes the fast path: per fold and per fit group (b200flow.tuning.fit_groups) ONE forest fit at
-(T_max, d_max), then ONE ForestModel.grid_confusion pass that yields the confusion matrix of every (numTrees, maxDepth) point.
-Each point's metric equals what fitting that point on its own and evaluating it would give, bit for bit (DESIGN.md §5a).
-Every other estimator / evaluator (and collectSubModels=True) runs the generic loop: fit, transform, evaluate per map.
+and prediction columns, with any metric derived from the confusion matrix (every metric but logLoss; by-label metrics with
+the evaluator's metricLabel and beta), takes the fast path: per fold and per fit group (b200flow.tuning.fit_groups) ONE
+forest fit at (T_max, d_max), then ONE ForestModel.grid_confusion pass that yields the confusion matrix of every
+(numTrees, maxDepth) point.  A BinaryClassificationEvaluator on the estimator's label and rawPrediction columns takes the
+same path through ForestModel.grid_binary_metrics (the score of every grid point per distinct validation record, then the
+device sort-and-scan over the I·J segments).  Each point's metric equals what fitting that point on its own and evaluating
+it would give, bit for bit (DESIGN.md §5a, §5b).  Every other estimator / evaluator (logLoss, and collectSubModels=True)
+runs the generic loop: fit, transform, evaluate per map.
 """
 import itertools
 
@@ -12,13 +16,12 @@ import numpy as np
 import torch
 
 from b200flow import dist as bdist
-from b200flow import forest as fr
 from b200flow import tuning as _tuning
 
 from . import Estimator, Model
 from .classification import (DecisionTreeClassifier, RandomForestClassifier, _default_seed, _lazy_plan,
                              _records_fit_inputs)
-from .evaluation import MulticlassClassificationEvaluator
+from .evaluation import BinaryClassificationEvaluator, MulticlassClassificationEvaluator
 from .param import Param
 
 
@@ -76,15 +79,18 @@ class _ValidatorParams:
 
 def _grid_metrics(est, maps, ev, train, val):
     """the fast path (module docstring) -> list of metrics, or None when the inputs do not qualify."""
-    if type(est) not in (RandomForestClassifier, DecisionTreeClassifier) or type(ev) is not MulticlassClassificationEvaluator:
+    binary = type(ev) is BinaryClassificationEvaluator
+    if type(est) not in (RandomForestClassifier, DecisionTreeClassifier) or \
+            (type(ev) is not MulticlassClassificationEvaluator and not binary):
         return None
-    name = ev.getOrDefault("metricName")
-    if name not in ev._metrics:
-        raise ValueError("metricName must be one of %s, got %r" % (list(ev._metrics), name))
+    name = ev._check()
+    if name == "logLoss":                                  # reads the probability column: no confusion matrix gives it
+        return None
     resolved = [est.copy(m) for m in maps]
     values = [{k: e.getOrDefault(k) for k in e._all_defaults()} for e in resolved]
-    lcol, pcol = ev.getOrDefault("labelCol"), ev.getOrDefault("predictionCol")
-    if any(v["labelCol"] != lcol or v["predictionCol"] != pcol for v in values):
+    lcol = ev.getOrDefault("labelCol")
+    ocol, key = ("rawPredictionCol", "rawPredictionCol") if binary else ("predictionCol", "predictionCol")
+    if any(v["labelCol"] != lcol or v[key] != ev.getOrDefault(ocol) for v in values):
         return None
     dt = type(est) is DecisionTreeClassifier
     out = [None] * len(maps)
@@ -94,26 +100,39 @@ def _grid_metrics(est, maps, ev, train, val):
         forest = rep.fit(train)._forest
         tree_cuts = sorted({t for _, t, _ in members})
         depth_cuts = sorted({d for _, _, d in members})
-        cm = _grid_confusion(forest, rep, val, tree_cuts, depth_cuts).numpy()
+        if binary:
+            if forest.C < 2:                               # no rawPrediction[1]: the generic loop raises as evaluate does
+                return None
+            auc = _grid_on_val(forest, rep, val, tree_cuts, depth_cuts, int(ev.getOrDefault("numBins")))
+            col = 0 if name == "areaUnderROC" else 1
+            for i, t, d in members:
+                out[i] = float(auc[tree_cuts.index(t), depth_cuts.index(d), col])
+            continue
+        cm = _grid_on_val(forest, rep, val, tree_cuts, depth_cuts).numpy()
         for i, t, d in members:
             c = cm[tree_cuts.index(t), depth_cuts.index(d)]
             nz = np.nonzero(c)
             side = int(max(nz[0].max(), nz[1].max())) + 1 if nz[0].size else 1     # the evaluator's max(label, prediction) + 1
-            out[i] = fr.metrics_from_confusion(c[:side, :side])[name]
+            out[i] = ev._metric_from_confusion(c[:side, :side], name)
     return out
 
 
-def _grid_confusion(forest, est, val, tree_cuts, depth_cuts):
-    """grid_confusion on the validation frame through the path model.transform would take (raw records or the dense vector)."""
+def _grid_on_val(forest, est, val, tree_cuts, depth_cuts, num_bins=None):
+    """grid_confusion (num_bins None) or grid_binary_metrics on the validation frame, through the path model.transform would
+    take (raw records or the dense vector)."""
     fcol, lcol = est.getOrDefault("featuresCol"), est.getOrDefault("labelCol")
     grp = bdist.group()
     plan = _lazy_plan(val, fcol)
     fused = _records_fit_inputs(val, est) if plan is not None and plan.n_out == forest.F else None
     if fused is not None:                                  # lazy features and indexed label: fused encode -> bins, labels < C
         rec, plan_l, _, _ = fused
+        if num_bins is not None:
+            return forest.grid_binary_metrics(rec, tree_cuts, depth_cuts, plan=plan_l, num_bins=num_bins, group=grp)
         return forest.grid_confusion(rec, tree_cuts, depth_cuts, plan=plan_l, group=grp)
     x = val._cols[fcol].data
     y = val._column_tensor(lcol).to(torch.float64)
+    if num_bins is not None:
+        return forest.grid_binary_metrics(x, tree_cuts, depth_cuts, labels=y.to(torch.int32), num_bins=num_bins, group=grp)
     mx = (y.max() if y.numel() else torch.zeros((), dtype=torch.float64, device=y.device)).reshape(1)
     if grp is not None:
         import torch.distributed as dist

@@ -544,6 +544,14 @@ class DataFrameReader:
         return DataFrame._from_records(rec, rschema, dicts, self._session)
 
 
+def _vector_column(s, name):
+    """a column of DenseVector / number lists -> f64 [n, D]; every row must have the same length."""
+    rows = [np.asarray(v.toArray() if hasattr(v, "toArray") else v, np.float64) for v in s]
+    if any(r.ndim != 1 for r in rows) or len({r.shape[0] for r in rows}) != 1:
+        raise NotImplementedError("createDataFrame: column %s must hold DenseVectors or number lists of one length" % name)
+    return np.ascontiguousarray(np.stack(rows))
+
+
 def _is_str(s):
     import pandas as pd
     return s.dtype == object or pd.api.types.is_string_dtype(s.dtype)
@@ -616,16 +624,18 @@ class SparkSession:
         return DataFrameReader(self)
 
     def createDataFrame(self, data, schema=None):
-        """host rows / pandas frame -> DataFrame (numeric columns as f64 fields, strings as dictionary codes)."""
+        """host rows / pandas frame -> DataFrame (numeric columns as f64 fields, strings as dictionary codes, DenseVector or
+        equal-length number-list columns as f64 vector columns)."""
         import pandas as pd
         _lib.require_cuda()
         pdf = data if isinstance(data, pd.DataFrame) else pd.DataFrame(list(data), columns=list(schema) if schema else None)
         fields, dicts = [], {}
-        host_cols = {}
+        host_cols, vectors = {}, {}
         for name in pdf.columns:
             s = pdf[name]
             if s.dtype == object and len(s) and not isinstance(s.iloc[0], str):
-                raise NotImplementedError("createDataFrame: vector/object columns are not supported; use numeric/string columns")
+                vectors[str(name)] = _vector_column(s, name)
+                continue
             if _is_str(s):
                 codes, uniq = pd.factorize(s, sort=False)
                 fields.append((str(name), "code")); host_cols[str(name)] = codes.astype(np.int32); dicts[str(name)] = [str(u) for u in uniq]
@@ -636,7 +646,12 @@ class SparkSession:
         for k, v in host_cols.items():
             host[k] = v
         rec = torch.from_numpy(host.view(np.uint8).reshape(len(pdf), rs.row_bytes)).to("cuda")
-        return DataFrame._from_records(rec, rs, dicts, self)
+        df = DataFrame._from_records(rec, rs, dicts, self)
+        if vectors:                                          # keep the frame's column order
+            cols = {str(k): (ColumnData("vector", torch.from_numpy(vectors[str(k)]).to("cuda"), "f64") if str(k) in vectors
+                             else df._cols[str(k)]) for k in pdf.columns}
+            df = df._with(cols=cols)
+        return df
 
     def stop(self):
         SparkSession._active = None

@@ -1,10 +1,13 @@
 """Time a 3-fold CrossValidator over numTrees {20, 50, 100} x maxDepth {5, 10, 16} on a seeded KDD99-full-shaped synthetic
-set (5 classes), twice: through the pyspark.ml shim (one forest fit per fold + grid_confusion, then the refit) and as the
+set (5 classes by default), twice: through the pyspark.ml shim (one forest fit per fold + grid_confusion, then the refit) and as the
 hand-written generic loop (fit -> transform -> evaluate for every fold and map, then the refit).  After one untimed run of
 each arm, the arms alternate --repeats times; the median of each is reported with every run's time.  Also prints the fit
 counts, whether avgMetrics are equal, and the card name and power limit read in the same run.  One JSON line.
 
-    python tools/bench_tuning.py [--rows 4898431] [--folds 3] [--repeats 3]
+    python tools/bench_tuning.py [--rows 4898431] [--folds 3] [--repeats 3] [--metric f1] [--classes 5]
+
+--metric areaUnderROC / areaUnderPR scores with a BinaryClassificationEvaluator (its fast path: grid_binary_metrics); any
+other name is a MulticlassClassificationEvaluator metric.
 """
 import argparse
 import json
@@ -33,12 +36,12 @@ def card():
     return out
 
 
-def frame(n, seed):
+def frame(n, seed, classes=5):
     from b200flow import synth
     from pyspark.ml import Pipeline
     from pyspark.ml.feature import StringIndexer, VectorAssembler
     from pyspark.sql import DataFrame
-    rec, dicts = synth.make_kdd(n, 5, seed=seed, device="cuda")
+    rec, dicts = synth.make_kdd(n, classes, seed=seed, device="cuda")
     df = DataFrame.fromRecords(rec, synth.kdd_schema(), dicts)
     cats = synth.KDD_CATEGORICAL
     df = Pipeline(stages=[StringIndexer(inputCol=c, outputCol=c + "_num") for c in cats + ["label"]]).fit(df).transform(df)
@@ -52,11 +55,13 @@ def main():
     ap.add_argument("--folds", type=int, default=3)
     ap.add_argument("--seed", type=int, default=2019)
     ap.add_argument("--repeats", type=int, default=3, help="timed runs of each arm, alternated; the median is reported")
+    ap.add_argument("--metric", default="f1", help="evaluator metric (areaUnderROC / areaUnderPR: the binary evaluator)")
+    ap.add_argument("--classes", type=int, default=5, help="label classes of the synthetic set")
     a = ap.parse_args()
     from b200flow import forest as fr
     from b200flow.rows import random_split_ids
     from pyspark.ml.classification import RandomForestClassifier
-    from pyspark.ml.evaluation import MulticlassClassificationEvaluator
+    from pyspark.ml.evaluation import BinaryClassificationEvaluator, MulticlassClassificationEvaluator
     from pyspark.ml.tuning import CrossValidator, ParamGridBuilder
 
     fits = [0]
@@ -68,10 +73,14 @@ def main():
             return _orig(*args, **kw)
         setattr(fr, name, wrapped)
 
-    df = frame(a.rows, a.seed)
+    df = frame(a.rows, a.seed, a.classes)
     rf = RandomForestClassifier(labelCol="label_num", featuresCol="features", maxBins=70, seed=a.seed)
     grid = ParamGridBuilder().addGrid(rf.numTrees, [20, 50, 100]).addGrid(rf.maxDepth, [5, 10, 16]).build()
-    ev = MulticlassClassificationEvaluator(labelCol="label_num", metricName="f1")
+    if a.metric in ("areaUnderROC", "areaUnderPR"):
+        ev = BinaryClassificationEvaluator(labelCol="label_num", metricName=a.metric)
+    else:
+        ev = MulticlassClassificationEvaluator(labelCol="label_num", metricName=a.metric)
+    better = 1 if ev.isLargerBetter() else -1
 
     def fast():
         fits[0] = 0
@@ -87,7 +96,7 @@ def main():
             for j, m in enumerate(grid):
                 sums[j] += ev.evaluate(rf.fit(train, m).transform(val))
         avg = [s / a.folds for s in sums]
-        return avg, rf.fit(df, grid[max(range(len(avg)), key=lambda j: (avg[j], -j))]), fits[0]
+        return avg, rf.fit(df, grid[max(range(len(avg)), key=lambda j: (better * avg[j], -j))]), fits[0]
 
     def timed(fn):
         torch.cuda.synchronize()
@@ -105,6 +114,7 @@ def main():
     same_best = bool(best._forest.T == best_f._forest.T and
                      all((best._forest.export()[k] == best_f._forest.export()[k]).all() for k in ("nid", "feat", "counts")))
     print(json.dumps({"metric": "3-fold CrossValidator, numTrees {20,50,100} x maxDepth {5,10,16}", "rows": a.rows,
+                      "evaluator_metric": a.metric, "classes": a.classes,
                       "fast_s": round(fast_s, 3), "generic_s": round(gen_s, 3),
                       "fast_runs_s": [round(t, 3) for t in times["fast"]],
                       "generic_runs_s": [round(t, 3) for t in times["generic"]], "speedup": round(gen_s / fast_s, 2),
