@@ -405,6 +405,38 @@ int b200flow_binary_curve(const double* d_score, const int64_t* d_pos, const int
                           const int64_t* n_distinct, int32_t S, int32_t num_bins, double* auc, double* c_score,
                           int64_t* c_tp, int64_t* c_fp, int64_t* c_n, double* work, void* stream);
 
+/* ---------------------------------------------------------------- clustering ---
+ * KMeans (k-means|| init + Lloyd) and ClusteringEvaluator (silhouette), DESIGN.md §5c.  Features are dense row-major f64
+ * x[n_rows][ld], 1 <= D <= 256.
+ * b200flow_kmeans_assign: centers [k][D] -> cluster[i] = first argmin center, dist[i] = its squared distance, summed in
+ * feature order from 0.0 as acc = acc + t*t, t = x_j - c_j (no FMA, no norm trick). */
+int b200flow_kmeans_assign(const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* centers, int32_t k,
+                           int32_t* cluster, double* dist, void* stream);
+/* Grouped sums.  Global rows are cut into chunks of 4096 (chunk b = global rows [4096 b, 4096 (b + 1))).  Rows
+ * [0, n_rows) of values [n_rows][ld] are global rows row_offset + i; they touch b200flow_group_sums_chunks(row_offset, n_rows)
+ * chunks (host-only query), starting with chunk row_offset / 4096.  partials [n_chunks][G][W] (device): the sequential sum, in
+ * row order from +0.0, of column w of the rows of that chunk with ids[i] == g (ids NULL: G == 1, every row); +0.0 where a
+ * chunk has no member.  counts int64 [G] (optional, caller zeroes) += the member rows; ids outside [0, G) are skipped.
+ * G <= 4096.  b200flow_group_sums_chain: totals [G][W] (device, in: the running totals, e.g. +0.0) += partials of chunk 0,
+ * then chunk 1, ... sequentially, in place. */
+int b200flow_group_sums_chunks(int64_t row_offset, int64_t n_rows, int64_t* n_chunks);
+int b200flow_group_sums(const double* values, int64_t ld, const int32_t* ids, int64_t n_rows, int32_t W, int32_t G,
+                        int64_t row_offset, double* partials, int64_t* counts, void* stream);
+int b200flow_group_sums_chain(const double* partials, int64_t n_chunks, int32_t G, int32_t W, double* totals, void* stream);
+/* keys[i] = (w0 << 32 | w1) ^ 2^63 as int64 (signed order = unsigned key order), (w0, w1) = the first two words of
+ * Philox(seed, 'KMNS', (row_lo, row_hi, 0, 0)) of global row row_offset + i: the first-center / random-init key. */
+int b200flow_kmeans_row_keys(uint64_t seed, int64_t row_offset, int64_t n_rows, int64_t* keys, void* stream);
+/* k-means|| round `step` >= 1: flag[i] = u < ((2.0 * cost[i]) * k) / sum_cost, u = ((w0 << 21) | (w1 >> 11)) * 2^-53 from
+ * Philox(seed, 'KMNS', (row_lo, row_hi, step, 0)). */
+int b200flow_kmeans_select(uint64_t seed, int64_t row_offset, int64_t n_rows, int32_t step, const double* cost, int32_t k,
+                           double sum_cost, uint8_t* flag, void* stream);
+/* silhouette coefficient per row from the cluster statistics Y [G][D] (feature sums), psi [G] (sums of squared norms),
+ * N int64 [G] (sizes; 0 = absent): d(g) = (norms[i] + psi[g] / N[g]) - (2 * (x . Y[g])) / N[g], dot sequential in j;
+ * a = d(own) * N / (N - 1), b = min over the other present clusters; out = 1 - a/b (a < b), b/a - 1 (a > b), else 0, and 0
+ * when the row's cluster has one member. */
+int b200flow_silhouette_rows(const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* norms, const int32_t* cluster,
+                             const double* Y, const double* psi, const int64_t* N, int32_t G, double* out, void* stream);
+
 /* -------------------------------------------------- either side of the path ---
  * DataFrame.randomSplit (kdd99.py:52, cicids17.py:56): split id per row from a uniform keyed
  * by (seed, global row): first k with u < cum_bounds[k] (n_splits <= 32).  out uint8[n]. */

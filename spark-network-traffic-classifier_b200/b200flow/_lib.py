@@ -72,6 +72,12 @@ _SIGNATURES = {
                                      _P],
     "b200flow_binary_counts": [_P, _I64, _P, _P, _I64, _I32, _I64, _P, _I64, _P, _P, _P, _I64, _P, _P, _P],
     "b200flow_binary_curve": [_P, _P, _P, _I64, _P, _I32, _I32, _P, _P, _P, _P, _P, _P, _P],
+    "b200flow_kmeans_assign": [_P, _I64, _I32, _I64, _P, _I32, _P, _P, _P],
+    "b200flow_group_sums": [_P, _I64, _P, _I64, _I32, _I32, _I64, _P, _P, _P],
+    "b200flow_group_sums_chain": [_P, _I64, _I32, _I32, _P, _P],
+    "b200flow_kmeans_row_keys": [_U64, _I64, _I64, _P, _P],
+    "b200flow_kmeans_select": [_U64, _I64, _I64, _I32, _P, _I32, _F64, _P, _P],
+    "b200flow_silhouette_rows": [_P, _I64, _I32, _I64, _P, _P, _P, _P, _P, _I32, _P, _P],
     "b200flow_random_split": [_U64, _I64, _I64, _P, _I32, _P, _P],
     "b200flow_compact_rows": [_P, _I64, _I32, _P, _I32, _P, _P, _P, _P],
     "b200flow_csv_count_lines": [_P, _I64, _P, _P, _P],
@@ -81,7 +87,8 @@ _SIGNATURES = {
     "b200flow_csv_parse": [_P, _I64, _P, _I64, _I32, _I32, _P, _P, _P, _P, _I32, _P, _I32, _P, _P],
 }
 EXPORTS = sorted(list(_SIGNATURES) + ["b200flow_last_error", "b200flow_version", "b200flow_route_hist_config",
-                                       "b200flow_packed_layout", "b200flow_binary_counts_scratch"])
+                                       "b200flow_packed_layout", "b200flow_binary_counts_scratch",
+                                       "b200flow_group_sums_chunks"])
 
 _lib = None
 launches = 0   # kernels of OURS launched so far (counted per C-ABI call); bench.py reads the delta over the timed region
@@ -109,6 +116,8 @@ def load():
         lib.b200flow_packed_layout.restype = C.c_int
         lib.b200flow_binary_counts_scratch.argtypes = [_I32, _I64, C.POINTER(_I64)]
         lib.b200flow_binary_counts_scratch.restype = C.c_int
+        lib.b200flow_group_sums_chunks.argtypes = [_I64, _I64, C.POINTER(_I64)]
+        lib.b200flow_group_sums_chunks.restype = C.c_int
         _lib = lib
     return _lib
 
@@ -139,6 +148,15 @@ def binary_counts_scratch(S, n):
     lib = load()
     if lib.b200flow_binary_counts_scratch(int(S), int(n), C.byref(out)) != 0:
         raise B200FlowError("b200flow_binary_counts_scratch failed: %s" % lib.b200flow_last_error().decode())
+    return int(out.value)
+
+
+def group_sums_chunks(row_offset, n_rows):
+    """number of 4096-row global chunks that rows [row_offset, row_offset + n_rows) touch (host-only call)."""
+    out = _I64(0)
+    lib = load()
+    if lib.b200flow_group_sums_chunks(int(row_offset), int(n_rows), C.byref(out)) != 0:
+        raise B200FlowError("b200flow_group_sums_chunks failed: %s" % lib.b200flow_last_error().decode())
     return int(out.value)
 
 

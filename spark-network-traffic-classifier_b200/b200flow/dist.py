@@ -65,6 +65,36 @@ def all_gather_list(t, grp):
     return parts
 
 
+def send(t, dst, grp):
+    """point-to-point send to group rank dst (staged through host memory under gloo)."""
+    d = dist.get_global_rank(grp, dst)
+    dist.send(t.cpu() if _staged(t, grp) else t, dst=d, group=grp)
+
+
+def recv_(t, src, grp):
+    """point-to-point receive from group rank src into t, in place."""
+    s = dist.get_global_rank(grp, src)
+    if _staged(t, grp):
+        c = t.cpu()
+        dist.recv(c, src=s, group=grp)
+        t.copy_(c)
+    else:
+        dist.recv(t, src=s, group=grp)
+    return t
+
+
+def broadcast_(t, src, grp):
+    """in-place broadcast from group rank src."""
+    s = dist.get_global_rank(grp, src)
+    if _staged(t, grp):
+        c = t.cpu()
+        dist.broadcast(c, src=s, group=grp)
+        t.copy_(c)
+    else:
+        dist.broadcast(t, src=s, group=grp)
+    return t
+
+
 def all_reduce_sum_(t, grp=None):
     """in-place sum over ranks (integer tensors stay exact -> bit-identical models for any world size)."""
     grp = grp if grp is not None else group()

@@ -2,7 +2,7 @@
 
 MulticlassClassificationEvaluator: confusion counts by the b200flow kernel (R10), metrics per MulticlassMetrics (A.8) +
 macro-F1; logLoss from the probability column.  BinaryClassificationEvaluator: areaUnderROC / areaUnderPR by the device
-sort-and-scan of b200flow.metrics (DESIGN.md §5b)."""
+sort-and-scan of b200flow.metrics (DESIGN.md §5b).  ClusteringEvaluator: the silhouette of b200flow.kmeans (DESIGN.md §5c)."""
 import math
 
 import torch
@@ -11,10 +11,10 @@ from b200flow import dist as bdist
 from b200flow import forest as fr
 from b200flow import metrics as bm
 
-from .feature import IllegalArgumentException
+from .feature import IllegalArgumentException, _materialize
 from .param import Params
 
-__all__ = ["BinaryClassificationEvaluator", "MulticlassClassificationEvaluator"]
+__all__ = ["BinaryClassificationEvaluator", "ClusteringEvaluator", "MulticlassClassificationEvaluator"]
 
 
 class MulticlassClassificationEvaluator(Params):
@@ -142,6 +142,47 @@ class BinaryClassificationEvaluator(Params):
         try:
             return bm.binary_metrics(scores, labels, num_bins=int(ev.getOrDefault("numBins")))[name]
         except bm.InvalidScoresError as e:
+            raise IllegalArgumentException(str(e)) from None
+
+    def isLargerBetter(self):
+        return True
+
+
+class ClusteringEvaluator(Params):
+    """silhouette with the squared Euclidean distance (Spark's SquaredEuclideanSilhouette), by b200flow.kmeans.silhouette:
+    the cluster statistics come from one grouped sum, so the value is the same bits for any world size.  Deviations from
+    Spark: distanceMeasure="cosine" and weightCol are not supported."""
+    _defaults = {"featuresCol": "features", "predictionCol": "prediction", "metricName": "silhouette",
+                 "distanceMeasure": "squaredEuclidean", "weightCol": None}
+
+    def __init__(self, predictionCol=None, featuresCol=None, metricName=None, distanceMeasure=None, weightCol=None):
+        super().__init__(predictionCol=predictionCol, featuresCol=featuresCol, metricName=metricName,
+                         distanceMeasure=distanceMeasure, weightCol=weightCol)
+
+    def _check(self):
+        if self.getOrDefault("metricName") != "silhouette":
+            raise IllegalArgumentException("metricName must be 'silhouette', got %r" % (self.getOrDefault("metricName"),))
+        dm = self.getOrDefault("distanceMeasure")
+        if dm == "cosine":
+            raise IllegalArgumentException("distanceMeasure='cosine' is not supported by this evaluator (out of scope); use "
+                                           "'squaredEuclidean'")
+        if dm != "squaredEuclidean":
+            raise IllegalArgumentException("distanceMeasure must be 'squaredEuclidean' or 'cosine', got %r" % (dm,))
+        if self.getOrDefault("weightCol"):
+            raise IllegalArgumentException("weightCol is not supported by this evaluator (out of scope)")
+
+    def evaluate(self, dataset, params=None):
+        from b200flow import kmeans as bk
+        ev = self.copy(params) if params else self
+        ev._check()
+        fcol = ev.getOrDefault("featuresCol")
+        if fcol not in dataset._cols or dataset._cols[fcol].kind != "vector":
+            raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+        x = _materialize(dataset, fcol)
+        cl = dataset._column_tensor(ev.getOrDefault("predictionCol"))
+        try:
+            return bk.silhouette(x, cl)
+        except ValueError as e:
             raise IllegalArgumentException(str(e)) from None
 
     def isLargerBetter(self):

@@ -1,0 +1,96 @@
+"""KMeans and the silhouette over TWO RANKS: the grouped sums keep their chunk order across shards (a straddling chunk is
+summed by the rank holding its first row, running totals pass rank to rank), so centers, cost, sizes, iteration count
+and silhouette equal the single-process result byte for byte — for even and uneven shards, a shard shorter than one
+4096-row chunk and an empty shard.  Two gloo ranks share one GPU (as in tests/test_two_ranks_one_gpu.py); the NCCL case
+needs two GPUs and is skipped otherwise."""
+import json
+import os
+import time
+import traceback
+
+import numpy as np
+import pytest
+import torch
+
+from test_tuning_two_ranks import _free_port
+
+pytestmark = pytest.mark.gpu
+
+N = 30000
+SPLITS = {"even": 15000, "uneven": 11000, "short_first": 2500, "short_last": 28000, "empty_last": N, "empty_first": 0}
+
+
+def _data():
+    rng = np.random.default_rng(8)
+    means = rng.normal(0.0, 3.0, (9, 41))
+    return np.ascontiguousarray(means[rng.integers(0, 9, N)] + rng.normal(0.0, 1.0, (N, 41)))
+
+
+def _run(x, dev):
+    from b200flow import kmeans as bk
+    xt = torch.from_numpy(x).to(dev)
+    out = {}
+    for init, k in (("k-means||", 12), ("random", 5)):
+        r = bk.kmeans_fit(xt, k, init=init, max_iter=8, seed=21)
+        out[init] = [[v.hex() for v in r.centers.cpu().numpy().ravel()], float(r.training_cost).hex(), r.num_iter,
+                     r.cluster_sizes.tolist(), bk.silhouette(xt, r.cluster).hex()]
+    return out
+
+
+def _worker(rank, world, port, out_dir, backend):
+    import torch.distributed as dist
+    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
+    gpu = rank if backend == "nccl" else 0
+    torch.cuda.set_device(gpu)
+    kw = {"device_id": torch.device("cuda", gpu)} if backend == "nccl" else {}
+    dist.init_process_group(backend, rank=rank, world_size=world, **kw)
+    try:
+        x = _data()
+        res = {}
+        for name, cut in SPLITS.items():
+            lo, hi = (0, cut) if rank == 0 else (cut, N)
+            res[name] = _run(x[lo:hi], torch.device("cuda", gpu))
+        open(os.path.join(out_dir, "res%d.json" % rank), "w").write(json.dumps(res))
+    except Exception:
+        open(os.path.join(out_dir, "error%d.txt" % rank), "w").write(traceback.format_exc())
+        raise
+    finally:
+        try:
+            dist.destroy_process_group()
+        except Exception:
+            pass
+
+
+def _two_ranks(tmp_path, backend):
+    import torch.multiprocessing as mp
+    ctx = mp.start_processes(_worker, args=(2, _free_port(), str(tmp_path), backend), nprocs=2, join=False, start_method="spawn")
+    deadline = time.time() + 600
+    failed = None
+    try:
+        while not ctx.join(timeout=5):
+            if time.time() > deadline:
+                failed = "workers hung"
+                break
+    except Exception as e:
+        failed = "worker failed: %s" % e
+    if failed:
+        for pr in ctx.processes:
+            if pr.is_alive():
+                pr.kill()
+        errs = "\n".join("--- rank %d\n%s" % (r, open(tmp_path / ("error%d.txt" % r)).read()) for r in (0, 1)
+                         if (tmp_path / ("error%d.txt" % r)).exists())
+        pytest.fail("%s\n%s" % (failed, errs))
+    want = json.loads(json.dumps(_run(_data(), torch.device("cuda", 0))))
+    for rank in (0, 1):
+        got = json.loads(open(tmp_path / ("res%d.json" % rank)).read())
+        for name in SPLITS:
+            assert got[name] == want, (rank, name)
+
+
+def test_kmeans_two_gloo_ranks_equal_one_process(tmp_path):
+    _two_ranks(tmp_path, "gloo")
+
+
+@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs two GPUs")
+def test_kmeans_two_nccl_ranks_equal_one_process(tmp_path):
+    _two_ranks(tmp_path, "nccl")
