@@ -390,7 +390,7 @@ void orc_bin_rows(const double* x, int64_t n, int32_t F, const double* threshold
             double v = x[i * F + f];
             if (arity[f] > 0) {
                 int b = (int)v;
-                if (!((double)b == v) || b < 0 || b >= arity[f]) { rowbad = true; b = arity[f] < 255 ? arity[f] : 255; }   // not in any left set: goes right (Node.scala CategoricalSplit.shouldGoLeft)
+                if (!((double)b == v) || b < 0 || b >= arity[f]) { rowbad = true; b = arity[f] < 255 ? arity[f] : 255; }   // bin `arity` is no category when arity <= 255 (build_metadata refuses 256): not in any left set, goes right
                 r[f] = (uint8_t)b;
             } else {
                 const double* thr = thresholds + (size_t)f * (max_bins - 1);

@@ -99,6 +99,10 @@ def build_metadata(n_rows, F, num_classes, arity, max_bins, num_trees, strategy=
                          "categorical feature, but a categorical feature has %d values. Consider removing this and other "
                          "categorical features with a large number of values, or add more training examples."
                          % (mpb, int(arity.max())))
+    if arity.size and int(arity.max()) > 255:
+        raise UnsupportedParamError("a categorical feature with %d categories is not supported: bins are stored as uint8, and "
+                                    "with 256 categories no bin is left for a value unseen at fit time (at most 255)"
+                                    % int(arity.max()))
     kind = np.zeros(F, np.int32)
     U = int(math.floor(math.log(mpb // 2 + 1) / math.log(2.0) + 1)) if num_classes > 2 else 0
     for f in range(F):
@@ -264,8 +268,9 @@ class ForestModel:
     def predict(self, x, want_raw=True, want_prob=True):
         """RandomForestClassificationModel.transform (R9): rawPrediction, probability, prediction.  The trees are walked
         once per UNIQUE binned record; the results are then spread back to the rows.  A categorical value outside
-        [0, arity) is binned to a value no left-set contains, so it goes right at every split on that feature — what
-        MLlib's CategoricalSplit.shouldGoLeft does with an unseen category."""
+        [0, arity) is binned to `arity` (at most 255, see build_metadata), which no left set contains, so it goes right at
+        every split on that feature — what MLlib's CategoricalSplit.shouldGoLeft does with an unseen category when the
+        split's left set holds at most half of the categories."""
         tp, _ = self.bin(x)
         return self._predict_tp(tp, want_raw, want_prob)
 

@@ -450,7 +450,7 @@ __global__ void __launch_bounds__(kBinMaxThreads) encode_bins_kernel(const Encod
 #pragma unroll
                     for (int q = 0; q < RPL; ++q) {
                         b[q] = (int)v[q];
-                        if (!((double)b[q] == v[q]) || b[q] < 0 || b[q] >= ar) { b[q] = ar < 255 ? ar : 255; if (lane + 32 * q < rows) ++n_bad; }   // never inside a left-set mask
+                        if (!((double)b[q] == v[q]) || b[q] < 0 || b[q] >= ar) { b[q] = ar < 255 ? ar : 255; if (lane + 32 * q < rows) ++n_bad; }   // bin `arity` is no category (arity <= 255, build_metadata): never inside a left-set mask
                     }
                 } else {
 #pragma unroll
@@ -616,13 +616,17 @@ extern "C" int b200flow_encode(const void* records, int64_t n_rows, int32_t row_
     size_t smem = (size_t)stages * a.in_stride + kEncOutBufs * (size_t)a.out_stride + kEncStages * 8 + (2 * R + 2) * 4 +
                   (size_t)n_out * sizeof(b200flow_slot) + (a.lut_in_smem ? (size_t)a.lut_total * 4 : 0) + 16 +
                   3 * (kEncMaxCat + 1) * 4 + (size_t)R * kEncMaxCat * 4 + 4 * ((size_t)n_out + 1);
-    B2F_REQUIRE(smem <= 227 * 1024, "encode: record too wide for shared memory (row_bytes=%d n_out=%d)", row_bytes, n_out);
+    // the kernel's static shared memory (sh_ncat, padded to the 128-byte alignment of the dynamic window) counts against the
+    // same 227 KB per block: without it the widest plans passed this check and failed in cudaFuncSetAttribute instead
+    cudaFuncAttributes fa;
+    cudaError_t e = cudaFuncGetAttributes(&fa, out_dtype == B200FLOW_F32 ? (const void*)encode_kernel<float> : (const void*)encode_kernel<double>);
+    if (e != cudaSuccess) { cudaGetLastError(); set_error("encode: cudaFuncGetAttributes: %s", cudaGetErrorString(e)); return B200FLOW_ERR_CUDA; }
+    B2F_REQUIRE(smem + fa.sharedSizeBytes <= 227 * 1024, "encode: record too wide for shared memory (row_bytes=%d n_out=%d)", row_bytes, n_out);
     const int64_t n_tiles = (n_rows + R - 1) / R;
     int ctas_per_sm = (int)((220 * 1024) / (smem + 1024));
     if (ctas_per_sm < 1) ctas_per_sm = 1;
     if (ctas_per_sm > 8) ctas_per_sm = 8;
     int grid = (int)(n_tiles < (int64_t)kNumSMs * ctas_per_sm ? n_tiles : (int64_t)kNumSMs * ctas_per_sm);
-    cudaError_t e;
     if (out_dtype == B200FLOW_F32) {
         e = cudaFuncSetAttribute(encode_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e == cudaSuccess) encode_kernel<float><<<grid, kEncThreads, smem, (cudaStream_t)stream>>>(a);
@@ -630,7 +634,9 @@ extern "C" int b200flow_encode(const void* records, int64_t n_rows, int32_t row_
         e = cudaFuncSetAttribute(encode_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e == cudaSuccess) encode_kernel<double><<<grid, kEncThreads, smem, (cudaStream_t)stream>>>(a);
     }
-    if (e != cudaSuccess) { set_error("encode: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return B200FLOW_ERR_CUDA; }
+    if (e != cudaSuccess) {               // clear the error too: left pending, the next unrelated CUDA call would report it
+        cudaGetLastError(); set_error("encode: cudaFuncSetAttribute: %s", cudaGetErrorString(e)); return B200FLOW_ERR_CUDA;
+    }
     return check_launch("encode");
 }
 

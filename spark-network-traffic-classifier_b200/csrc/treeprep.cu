@@ -269,7 +269,7 @@ __global__ void __launch_bounds__(256) bin_rows_kernel(const T* __restrict__ x, 
                     int b;
                     if (ar > 0) {
                         b = (int)v;
-                        if (!((double)b == v) || b < 0 || b >= ar) { b = ar < 255 ? ar : 255; atomicAdd(bad_rows, 1); }   // a bin no left-set mask contains: routes right, like an unseen category in MLlib's predict
+                        if (!((double)b == v) || b < 0 || b >= ar) { b = ar < 255 ? ar : 255; atomicAdd(bad_rows, 1); }   // bin `arity` is no category (arity <= 255, build_metadata): no left-set mask contains it, it routes right
                     } else {
                         int lo = 0, hi = nt;              // lower_bound: first b with v <= thr[b]
                         while (lo < hi) { int mid = (lo + hi) >> 1; if (v <= thr[mid]) hi = mid; else lo = mid + 1; }
