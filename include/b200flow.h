@@ -437,6 +437,27 @@ int b200flow_kmeans_select(uint64_t seed, int64_t row_offset, int64_t n_rows, in
 int b200flow_silhouette_rows(const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* norms, const int32_t* cluster,
                              const double* Y, const double* psi, const int64_t* N, int32_t G, double* out, void* stream);
 
+/* ---------------------------------------------------------- neural network ---
+ * MultilayerPerceptronClassifier, DESIGN.md §5d.  layers (host int32 [n_layers]) = [D, h_1, ..., h_k, K]: affine +
+ * sigmoid per hidden layer, affine on top (softmax in the loss).  weights (device f64 [P]) in Spark's layout: per layer W
+ * (out x in, column-major: (o, i) at o + i*out) then b (out), P = sum (in*out + out).  Features x [n_rows][ld] are f32
+ * (x_dtype B200FLOW_F32) or f64 (B200FLOW_F64), converted to f64 before any arithmetic: equal values give equal bits.
+ * Limits: at most 8 affine layers; sum over layers of ceil(out/8) * ceil((in+1)/8) <= 256 (the gradient's 8x8 tiles,
+ * held in registers); 8 * (sum of padded W blocks + 32 * sum of padded activation widths) <= 226 KiB of shared memory
+ * (b200flow_mlp_config reports both; [78,100,50,15] and [119,64,32,5] fit).
+ * b200flow_mlp_config (host-only): *n_params = P, *smem_bytes = the kernels' dynamic shared memory; error beyond limits. */
+int b200flow_mlp_config(const int32_t* layers, int32_t n_layers, int64_t* n_params, int64_t* smem_bytes);
+/* partials [n_chunks][P + 1] (device; n_chunks = b200flow_group_sums_chunks(row_offset, n_rows)): for each 4096-row
+ * global chunk the rows [0, n_rows) (global rows row_offset + i) touch, slot 0 = the sum over its rows of
+ * logsumexp(z) - z[y] (z = the top affine output, labels int32 in [0, K)), slots 1..P = the sum of the gradient of that
+ * loss in the weights' layout.  A chunk's partial depends only on which of its rows are present. */
+int b200flow_mlp_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, const int32_t* labels,
+                           const int32_t* layers, int32_t n_layers, const double* weights, int64_t row_offset,
+                           double* partials, void* stream);
+/* raw [n_rows][K] f64: the top affine output (Spark 3's predictRaw) of every row. */
+int b200flow_mlp_forward(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, const int32_t* layers, int32_t n_layers,
+                         const double* weights, double* raw, void* stream);
+
 /* -------------------------------------------------- either side of the path ---
  * DataFrame.randomSplit (kdd99.py:52, cicids17.py:56): split id per row from a uniform keyed
  * by (seed, global row): first k with u < cum_bounds[k] (n_splits <= 32).  out uint8[n]. */

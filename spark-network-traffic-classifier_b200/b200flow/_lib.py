@@ -78,6 +78,8 @@ _SIGNATURES = {
     "b200flow_kmeans_row_keys": [_U64, _I64, _I64, _P, _P],
     "b200flow_kmeans_select": [_U64, _I64, _I64, _I32, _P, _I32, _F64, _P, _P],
     "b200flow_silhouette_rows": [_P, _I64, _I32, _I64, _P, _P, _P, _P, _P, _I32, _P, _P],
+    "b200flow_mlp_loss_grad": [_P, _I32, _I64, _I64, _P, _P, _I32, _P, _I64, _P, _P],
+    "b200flow_mlp_forward": [_P, _I32, _I64, _I64, _P, _I32, _P, _P, _P],
     "b200flow_random_split": [_U64, _I64, _I64, _P, _I32, _P, _P],
     "b200flow_compact_rows": [_P, _I64, _I32, _P, _I32, _P, _P, _P, _P],
     "b200flow_csv_count_lines": [_P, _I64, _P, _P, _P],
@@ -88,7 +90,7 @@ _SIGNATURES = {
 }
 EXPORTS = sorted(list(_SIGNATURES) + ["b200flow_last_error", "b200flow_version", "b200flow_route_hist_config",
                                        "b200flow_packed_layout", "b200flow_binary_counts_scratch",
-                                       "b200flow_group_sums_chunks"])
+                                       "b200flow_group_sums_chunks", "b200flow_mlp_config"])
 
 _lib = None
 launches = 0   # kernels of OURS launched so far (counted per C-ABI call); bench.py reads the delta over the timed region
@@ -118,6 +120,8 @@ def load():
         lib.b200flow_binary_counts_scratch.restype = C.c_int
         lib.b200flow_group_sums_chunks.argtypes = [_I64, _I64, C.POINTER(_I64)]
         lib.b200flow_group_sums_chunks.restype = C.c_int
+        lib.b200flow_mlp_config.argtypes = [_P, _I32, C.POINTER(_I64), C.POINTER(_I64)]
+        lib.b200flow_mlp_config.restype = C.c_int
         _lib = lib
     return _lib
 
@@ -158,6 +162,17 @@ def group_sums_chunks(row_offset, n_rows):
     if lib.b200flow_group_sums_chunks(int(row_offset), int(n_rows), C.byref(out)) != 0:
         raise B200FlowError("b200flow_group_sums_chunks failed: %s" % lib.b200flow_last_error().decode())
     return int(out.value)
+
+
+def mlp_config(layers):
+    """(P, shared-memory bytes) of the MLP kernels for a layer list (host-only call); raises UnsupportedParamError beyond
+    the kernels' limits."""
+    la = np.ascontiguousarray(layers, dtype=np.int32)
+    P, sm = _I64(0), _I64(0)
+    lib = load()
+    if lib.b200flow_mlp_config(la.ctypes.data, int(la.shape[0]), C.byref(P), C.byref(sm)) != 0:
+        raise UnsupportedParamError("layers %s: %s" % (list(map(int, la)), lib.b200flow_last_error().decode()))
+    return int(P.value), int(sm.value)
 
 
 def ptr(t):

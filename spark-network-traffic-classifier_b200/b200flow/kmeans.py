@@ -14,7 +14,8 @@ from . import _lib
 from . import dist as bdist
 from ._lib import call, ptr
 
-CHUNK = 4096
+CHUNK = bdist.CHUNK
+_Shards = bdist.Shards
 MAX_D = 256            # kmeans_assign stages a row tile and a center tile of every feature in shared memory
 MAX_GROUPS = 4096      # group_sums counting-sorts a chunk by group in shared memory
 PURPOSE_KMNS = 0x4B4D4E53
@@ -68,50 +69,15 @@ def assign(x, centers):
     return cl[:n], d[:n]
 
 
-class _Shards:
-    """the global row layout: every rank's (first global row, row count), gathered once per fit."""
-
-    def __init__(self, n, row_offset, grp, device):
-        self.grp = grp
-        if grp is None:
-            self.rank, self.offs, self.ns = 0, [int(row_offset)], [int(n)]
-        else:
-            import torch.distributed as dist
-            self.rank = dist.get_rank(grp)
-            parts = bdist.all_gather_list(torch.tensor([int(row_offset), int(n)], dtype=torch.int64, device=device), grp)
-            self.offs = [int(p[0]) for p in parts]
-            self.ns = [int(p[1]) for p in parts]
-        self.total = sum(self.ns)
-        # rows at the head of a shard that belong to a chunk starting on an earlier rank
-        self.lead = [min(m, (-o) % CHUNK) for o, m in zip(self.offs, self.ns)]
-        self.owner = [self._holder(CHUNK * (o // CHUNK)) if ld else -1 for o, ld in zip(self.offs, self.lead)]
-
-    def _holder(self, row):
-        return next(r for r, (o, m) in enumerate(zip(self.offs, self.ns)) if o <= row < o + m)
-
-
 def grouped_sum(values, ids, G, sh):
     """(totals f64 [G, W], counts int64 [G]) of values [n, W] f64 grouped by ids int32 [n] (None: one group), summed in the
     fixed chunk order of the module docstring; the same bits on every rank."""
     n, W = values.shape
     dev = values.device
     values = values.contiguous()
-    rank, grp = sh.rank, sh.grp
-    off, lead = sh.offs[rank], sh.lead[rank]
-    nfull = max(n - lead, 0) // CHUNK
-    t0 = lead + nfull * CHUNK                              # first row of this rank's trailing (possibly straddling) chunk
-    tail_v, tail_i = values[t0:], (ids[t0:] if ids is not None else None)
-    if grp is not None and any(sh.lead):                   # the owner of a straddling chunk collects the rows of later ranks
-        buf = torch.zeros((CHUNK - 1, W + 1), dtype=torch.float64, device=dev)
-        buf[:lead, :W] = values[:lead]
-        if ids is not None:
-            buf[:lead, W] = ids[:lead].to(torch.float64)
-        parts = bdist.all_gather_list(buf, grp)
-        extra = [parts[s][:sh.lead[s]] for s in range(len(parts)) if sh.owner[s] == rank]
-        if extra:
-            ex = torch.cat(extra)
-            tail_v = torch.cat([tail_v, ex[:, :W]]).contiguous()
-            tail_i = torch.cat([tail_i, ex[:, W].to(torch.int32)]).contiguous() if ids is not None else None
+    off, lead = sh.offs[sh.rank], sh.lead[sh.rank]
+    t0, tail_v, tail_i = bdist.chunk_tail(values, ids, sh)
+    nfull = (t0 - lead) // CHUNK
     n_tail = tail_v.shape[0]
     n_chunks = nfull + (1 if n_tail else 0)
     partials = torch.empty((max(n_chunks, 1), G, W), dtype=torch.float64, device=dev)
@@ -122,16 +88,9 @@ def grouped_sum(values, ids, G, sh):
     if n_tail:
         call("b200flow_group_sums", ptr(tail_v), W, ptr(tail_i) if ids is not None else None, n_tail, W, G, off + t0,
              ptr(partials[nfull:]), ptr(counts))
-    totals = torch.zeros((G, W), dtype=torch.float64, device=dev)
-    world = len(sh.ns)
-    if grp is not None and rank > 0:
-        bdist.recv_(totals, rank - 1, grp)
-    call("b200flow_group_sums_chain", ptr(partials), n_chunks, G, W, ptr(totals))
-    if grp is not None:
-        if rank < world - 1:
-            bdist.send(totals, rank + 1, grp)
-        bdist.broadcast_(totals, world - 1, grp)
-        bdist.all_reduce_(counts, grp)
+    totals = bdist.chunk_chain(partials, n_chunks, G, W, sh)
+    if sh.grp is not None:
+        bdist.all_reduce_(counts, sh.grp)
     return totals, counts
 
 

@@ -106,6 +106,71 @@ def _pseudo_gradient(x, g, c):
     return torch.where(x > 0, right, torch.where(x < 0, left, at0))
 
 
+def lbfgs(smooth, v, max_iter, tol, history=10, l1=None):
+    """minimise smooth(v) -> (f, gradient) from v: L-BFGS with `history` corrections, backtracking (Armijo 1e-4, halving,
+    at most 40 trials), stopping after max_iter iterations or once the relative decrease (F - Fn) / max(|Fn|, |F|) falls
+    to tol after the first iteration.  l1 (one weight per variable) makes it OWL-QN for f + sum l1 |v|: the direction
+    is kept to the components that descend along the pseudo-gradient and the steps are projected onto the orthant; None
+    is plain L-BFGS (Breeze LBFGS, what Spark runs without an L1 term).  -> (v, objective history, iterations)."""
+    def full(v, f):
+        return f if l1 is None else f + (l1 * v.abs()).sum()
+
+    f, g = smooth(v)
+    F = float(full(v, f).item())
+    hist = [F]
+    S, Y, RHO = [], [], []
+    it = 0
+    while it < int(max_iter):
+        pg = g if l1 is None else _pseudo_gradient(v, g, l1)
+        if float(pg.norm().item()) <= 1e-14:
+            break
+        q = pg.clone()                                                 # two-loop recursion on the pseudo-gradient
+        al = []
+        for s_, y_, r_ in zip(reversed(S), reversed(Y), reversed(RHO)):
+            a = r_ * (s_ @ q)
+            al.append(a)
+            q -= a * y_
+        if S:
+            q *= (S[-1] @ Y[-1]) / (Y[-1] @ Y[-1])
+        for (s_, y_, r_), a in zip(zip(S, Y, RHO), reversed(al)):
+            q += (a - r_ * (y_ @ q)) * s_
+        d = -q
+        if l1 is not None:
+            d = torch.where(d * pg < 0, d, torch.zeros_like(d))        # keep only components that descend along -pg
+            if not bool((d != 0).any()):
+                d = -pg
+            orth = torch.where(v != 0, torch.sign(v), torch.sign(-pg)) # the orthant the step must stay in
+        dir_deriv = float((pg @ d).item())
+        step = 1.0 if S else min(1.0, 1.0 / max(float(pg.norm().item()), 1e-300))
+        ok = False
+        for _ in range(40):
+            vn = v + step * d
+            if l1 is not None:
+                vn = torch.where(vn * orth < 0, torch.zeros_like(vn), vn)  # projection onto the orthant
+            fn, gn = smooth(vn)
+            Fn = float(full(vn, fn).item())
+            if Fn <= F + 1e-4 * float((pg @ (vn - v)).item()):
+                ok = True
+                break
+            step *= 0.5
+        if not ok or dir_deriv >= 0 and not S:
+            break
+        s_, y_ = vn - v, gn - g
+        sy = float((s_ @ y_).item())
+        if sy > 1e-300:
+            S.append(s_); Y.append(y_); RHO.append(1.0 / sy)
+            if len(S) > history:
+                S.pop(0); Y.pop(0); RHO.pop(0)
+        v, g, f = vn, gn, fn
+        it += 1
+        hist.append(Fn)
+        improved = (F - Fn) / max(abs(Fn), abs(F), 1e-300)
+        F = Fn
+        if improved <= tol and it > 1:
+            break
+    return v, hist, it
+
+
 def lr_fit(x, y, num_classes, max_iter=100, reg_param=0.0, elastic_net=0.0, tol=1e-6, fit_intercept=True, standardization=True,
            family="auto", history=10, group=None):
     x = x.to(torch.float64)
@@ -152,61 +217,7 @@ def lr_fit(x, y, num_classes, max_iter=100, reg_param=0.0, elastic_net=0.0, tol=
         f, gB, gb = lr_loss_grad(xs, y1h, Bv, bv, l2w_row, binomial, fit_intercept, n, group)
         return f, torch.cat([gB.reshape(-1), gb])
 
-    def full(v, f):
-        return f + (cw * v.abs()).sum()
-
-    v = torch.cat([B.reshape(-1), b])
-    f, g = smooth(v)
-    F = float(full(v, f).item())
-    hist = [F]
-    S, Y, RHO = [], [], []
-    it = 0
-    while it < int(max_iter):
-        pg = _pseudo_gradient(v, g, cw)
-        if float(pg.norm().item()) <= 1e-14:
-            break
-        q = pg.clone()                                                 # two-loop recursion on the pseudo-gradient
-        al = []
-        for s_, y_, r_ in zip(reversed(S), reversed(Y), reversed(RHO)):
-            a = r_ * (s_ @ q)
-            al.append(a)
-            q -= a * y_
-        if S:
-            q *= (S[-1] @ Y[-1]) / (Y[-1] @ Y[-1])
-        for (s_, y_, r_), a in zip(zip(S, Y, RHO), reversed(al)):
-            q += (a - r_ * (y_ @ q)) * s_
-        d = -q
-        d = torch.where(d * pg < 0, d, torch.zeros_like(d))            # keep only components that descend along -pg
-        if not bool((d != 0).any()):
-            d = -pg
-        orth = torch.where(v != 0, torch.sign(v), torch.sign(-pg))     # the orthant the step must stay in
-        dir_deriv = float((pg @ d).item())
-        step = 1.0 if S else min(1.0, 1.0 / max(float(pg.norm().item()), 1e-300))
-        ok = False
-        for _ in range(40):
-            vn = v + step * d
-            vn = torch.where(vn * orth < 0, torch.zeros_like(vn), vn)  # projection onto the orthant
-            fn, gn = smooth(vn)
-            Fn = float(full(vn, fn).item())
-            if Fn <= F + 1e-4 * float((pg @ (vn - v)).item()):
-                ok = True
-                break
-            step *= 0.5
-        if not ok or dir_deriv >= 0 and not S:
-            break
-        s_, y_ = vn - v, gn - g
-        sy = float((s_ @ y_).item())
-        if sy > 1e-300:
-            S.append(s_); Y.append(y_); RHO.append(1.0 / sy)
-            if len(S) > history:
-                S.pop(0); Y.pop(0); RHO.pop(0)
-        v, g, f = vn, gn, fn
-        it += 1
-        hist.append(Fn)
-        improved = (F - Fn) / max(abs(Fn), abs(F), 1e-300)
-        F = Fn
-        if improved <= tol and it > 1:
-            break
+    v, hist, it = lbfgs(smooth, torch.cat([B.reshape(-1), b]), max_iter, tol, history, l1=cw)
     B, b = unpack(v)
     coef = B * inv                                                      # back to the original feature scale
     if fit_intercept and not binomial:

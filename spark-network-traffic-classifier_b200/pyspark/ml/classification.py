@@ -2,6 +2,8 @@
 
 RandomForestClassifier / DecisionTreeClassifier (kdd99.py:61,64; cicids17.py:65,68) are the hot path and run
 entirely on the b200flow CUDA kernels (histogram build, Gini split scoring, batch predict).
+MultilayerPerceptronClassifier runs on the fused fp64 tensor-core loss/gradient and forward kernels (b200flow/mlp.py,
+csrc/mlp.cu, DESIGN.md §5d); its model is the same bits for any number of ranks.
 LogisticRegression and NaiveBayes (kdd99.py:57,67; cicids17.py:61,71) are OUT of the kernel scope (SURVEY.md
 §8f rank 4): torch fp64 implementations of MLlib's statistics / objective (b200flow/linear.py), checked against a numpy
 restatement and scikit-learn in tests/test_linear_models.py.
@@ -14,6 +16,7 @@ import torch
 from b200flow import dist as bdist
 from b200flow import forest as fr
 from b200flow import linear as _linear
+from b200flow import mlp as _mlp
 
 from . import Estimator, Model
 from ..sql import ColumnData
@@ -379,4 +382,94 @@ class NaiveBayesModel(_ProbModel):
 
     def _transform(self, df):
         raw = _linear.nb_raw(self._fit_result, df._cols[self.getOrDefault("featuresCol")].data)
+        return self._emit(df, raw, torch.softmax(raw, 1))
+
+
+# ------------------------------------------------------------------------------- multilayer perceptron (CUDA)
+class _MLPParams:
+    _defaults = dict(_ProbModel._defaults, layers=None, maxIter=100, tol=1e-6, blockSize=128, solver="l-bfgs", stepSize=0.03,
+                     seed=None, initialWeights=None)
+
+
+class MultilayerPerceptronClassifier(Estimator, _MLPParams):
+    """Spark's feed-forward classifier: sigmoid hidden layers, softmax output, trained in fp64 by L-BFGS or gradient
+    descent on the device (b200flow/mlp.py).  blockSize is validated but does not change the result (DESIGN.md §5d)."""
+
+    def __init__(self, featuresCol=None, labelCol=None, predictionCol=None, maxIter=None, tol=None, seed=None, layers=None,
+                 blockSize=None, stepSize=None, solver=None, initialWeights=None, probabilityCol=None, rawPredictionCol=None):
+        kw = dict(locals()); kw.pop("self"); kw.pop("__class__", None)
+        super().__init__(**kw)
+
+    def _check(self):
+        """Spark's param validators."""
+        g = self.getOrDefault
+        layers = g("layers")
+        if layers is None:
+            raise IllegalArgumentException("MultilayerPerceptronClassifier needs the layers param")
+        if len(layers) < 2 or any(int(v) != v or int(v) <= 0 for v in layers):
+            raise IllegalArgumentException("layers must have at least 2 entries, all integers > 0, got %r" % (list(layers),))
+        if int(layers[-1]) < 2:
+            raise IllegalArgumentException("the output layer needs at least 2 classes, got %r" % (layers[-1],))
+        it, bs = g("maxIter"), g("blockSize")
+        if int(it) != it or int(it) < 0:
+            raise IllegalArgumentException("maxIter must be an integer >= 0, got %r" % (it,))
+        if int(bs) != bs or int(bs) <= 0:
+            raise IllegalArgumentException("blockSize must be an integer > 0, got %r" % (bs,))
+        for name in ("stepSize", "tol"):
+            if not float(g(name)) > 0:
+                raise IllegalArgumentException("%s must be > 0, got %r" % (name, g(name)))
+        if g("solver") not in ("l-bfgs", "gd"):
+            raise IllegalArgumentException("solver must be 'l-bfgs' or 'gd', got %r" % (g("solver"),))
+        return [int(v) for v in layers]
+
+    def _fit(self, df):
+        layers = self._check()
+        g = self.getOrDefault
+        x, y, _, _ = _features_and_labels(df, self)
+        seed = _default_seed(self) if g("seed") is None else int(g("seed"))
+        iw = g("initialWeights")
+        if iw is not None and hasattr(iw, "toArray"):
+            iw = iw.toArray()
+        try:
+            fit = _mlp.mlp_fit(x, y, layers, solver=g("solver"), max_iter=int(g("maxIter")), tol=float(g("tol")),
+                               step_size=float(g("stepSize")), seed=seed, initial_weights=iw, group=bdist.group())
+        except ValueError as e:        # includes b200flow's UnsupportedParamError
+            raise IllegalArgumentException(str(e))
+        m = MultilayerPerceptronClassificationModel(layers, fit)
+        m._paramMap = {k: v for k, v in self._paramMap.items() if k in m._all_defaults()}
+        m._paramMap["layers"] = list(layers)
+        return m
+
+
+class MultilayerPerceptronClassificationModel(_ProbModel, _MLPParams):
+    def __init__(self, layers, fit):
+        super().__init__()
+        self._layers, self._weights = list(layers), fit.weights
+        self.summary = _TrainingSummary(fit.objective_history, fit.iterations)
+
+    @property
+    def layers(self):
+        return list(self._layers)
+
+    @property
+    def weights(self):
+        from .linalg import DenseVector
+        return DenseVector(self._weights.cpu().numpy())
+
+    @property
+    def numFeatures(self):
+        return self._layers[0]
+
+    @property
+    def numClasses(self):
+        return self._layers[-1]
+
+    def _transform(self, df):
+        fcol = self.getOrDefault("featuresCol")
+        if fcol not in df._cols or df._cols[fcol].kind != "vector":
+            raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+        try:
+            raw = _mlp.mlp_raw(self._weights, self._layers, df._cols[fcol].data)
+        except ValueError as e:
+            raise IllegalArgumentException(str(e))
         return self._emit(df, raw, torch.softmax(raw, 1))
