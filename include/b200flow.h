@@ -458,6 +458,37 @@ int b200flow_mlp_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, int64
 int b200flow_mlp_forward(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, const int32_t* layers, int32_t n_layers,
                          const double* weights, double* raw, void* stream);
 
+/* ------------------------------------------------------- gradient-boosted trees ---
+ * GBTClassifier (binary, LogLoss), DESIGN.md §5e.  The regression trees reuse the forest's level loop: feature_subsets,
+ * partition_level, next_segments, grow_level (with C = 6: a node's int64 stats {Σw, Σw·q, Σw·q2} travel as six opaque
+ * uint32 words in pool_counts) and predict (C = 1 over the payloads).  Residuals are on a fixed-point grid: rq int64
+ * [n][2] = {q, q2}, q = rint(r 2^S), q2 = rint((q 2^-S)^2 2^S2), S = 60 - ceil(log2 max(n_global, 2)), S2 = S - 2, so every
+ * histogram sum is an exact integer below 2^62.  rq must be 16-byte aligned.
+ * b200flow_gbt_hist_level: hist int64 [n_slots][m][n_bins][3] (caller zeroes) += {w, w·q, w·q2} of every entry of the slot
+ * at the bin of each subset feature; entries, segments and the chunk table as for b200flow_hist_level. */
+int b200flow_gbt_hist_level(const uint8_t* tp, int32_t tp_stride, const void* ent, const int64_t* rq, int32_t n_slots,
+                            const int64_t* seg_begin, const int64_t* seg_end, const int64_t* chunk_off, int64_t n_chunks,
+                            int32_t chunk_rows, const uint16_t* subset, int32_t m, int32_t n_bins, int64_t* hist, void* stream);
+/* Variance split scoring, one CTA per slot: split[s] as score_level writes it (categorical features are ordered by centroid
+ * sum/count; a child is a leaf at level + 1 == max_depth or when its variance is below 2^-52), and the int64 stats [3] of
+ * the node and of both children (zero when there is no split). */
+int b200flow_gbt_score_level(const int64_t* hist, int32_t n_slots, const uint16_t* subset, int32_t m, int32_t n_bins,
+                             const int32_t* feat_bins, const int32_t* feat_kind, int32_t S, int32_t S2, int32_t level,
+                             int32_t max_depth, int32_t min_instances, double min_info_gain, b200flow_split* split,
+                             int64_t* node_stats, int64_t* left_stats, int64_t* right_stats, void* stream);
+/* payload[i] = tree_weight[node_tree[i]] * ((Σw·q 2^-S) / Σw) for the n_nodes pool nodes (stats int64 [n_nodes][3]) */
+int b200flow_gbt_leaf_values(int64_t n_nodes, const int64_t* stats, const int32_t* node_tree, const double* tree_weight,
+                             int32_t S, double* payload, void* stream);
+/* per binned record (label at byte F, 0 or 1; y = 2 label - 1): tree < 0 sets margin = +0.0 and rq to y's grid values;
+ * tree >= 0 walks that tree (root = pool node `tree`), margin += payload of its leaf, rq = grid of 4y / (1 + exp(2y margin))
+ * (csrc/portable_exp.h; a NaN residual becomes 0). */
+int b200flow_gbt_update(const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows, const b200flow_node* nodes,
+                        const uint64_t* node_mask, const double* payload, int32_t tree, int32_t S, int32_t S2, double* margin,
+                        int64_t* rq, void* stream);
+/* GBTClassificationModel output from the margins: raw [n][2] = {-F, F}, prob [n][2] = {1 / (1 + exp(2F)), 1 - that},
+ * pred = F > 0; raw / prob / pred may be NULL. */
+int b200flow_gbt_output(const double* margin, int64_t n_rows, double* raw, double* prob, double* pred, void* stream);
+
 /* -------------------------------------------------- either side of the path ---
  * DataFrame.randomSplit (kdd99.py:52, cicids17.py:56): split id per row from a uniform keyed
  * by (seed, global row): first k with u < cum_bounds[k] (n_splits <= 32).  out uint8[n]. */

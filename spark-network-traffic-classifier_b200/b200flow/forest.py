@@ -465,6 +465,90 @@ def _gather_sample(sample, n_s, cap, F, group):
     return out.view(-1), tot, new_cap
 
 
+class _TrainingRows:
+    """The front half of RandomForest.run, shared by the forest and the GBT trainers: the global row count, the metadata,
+    findSplits (R4), binning (R5) and the de-duplication of the binned rows.  The constructor only enqueues device work;
+    read() then fetches the bad-cell counts, the bin count, the sample count and the unique-record count in ONE host read, so
+    the caller can prepare what does not depend on them in between, while the GPU works through the queue."""
+
+    def __init__(self, src, num_classes, arity, max_bins, num_trees, strategy, seed, row_offset, group):
+        from . import dist as bdist
+        dev = src.device
+        n, F, C, T = src.n, src.F, num_classes, num_trees
+        n_global = n
+        if group is not None:
+            t = torch.tensor([n], dtype=torch.int64, device=dev)
+            bdist.all_reduce_(t, group)
+            n_global = int(t.item())
+        mpb, kind, m = build_metadata(n_global, F, C, arity, max_bins, T, strategy)
+        arity = np.asarray(arity, np.int32)
+        arity_dev = _i32(arity, dev)
+
+        # ---- R4 findSplits: Bernoulli row sample keyed by global row, sort + stride walk on device
+        has_cont = bool((arity == 0).any())
+        frac = min(1.0, max(mpb * mpb, 10000) / float(max(n_global, 1))) if has_cont else 1.0
+        keep = int(frac * 4294967296.0)
+        expect = n if frac >= 1.0 else int(n * frac + 6.0 * math.sqrt(max(n * frac, 1.0)) + 64)
+        cap = 1
+        while cap < max(min(expect, n), 2):
+            cap <<= 1
+        sample = torch.empty(F * cap, dtype=torch.float64, device=dev)
+        n_s_dev = torch.zeros(1, dtype=torch.int32, device=dev)
+        thresholds = torch.zeros((F, mpb - 1), dtype=torch.float64, device=dev)
+        n_thr = torch.zeros(F, dtype=torch.int32, device=dev)
+        if has_cont:
+            src.sample(seed, keep, row_offset, sample, cap, n_s_dev)
+            if group is not None:
+                n_s = int(n_s_dev.item())
+                if n_s > cap:
+                    raise B200FlowError("findSplits sample overflow (%d > %d)" % (n_s, cap))
+                sample, n_s, cap = _gather_sample(sample, n_s, cap, F, group)
+                call("b200flow_find_splits", ptr(sample), cap, n_s, F, ptr(arity_dev), mpb, ptr(thresholds), ptr(n_thr), None)
+            else:       # single GPU: the sample count stays on the device (checked with the other counts below: one host sync)
+                call("b200flow_find_splits", ptr(sample), cap, cap, F, ptr(arity_dev), mpb, ptr(thresholds), ptr(n_thr), ptr(n_s_dev))
+        del sample
+
+        # ---- R5 binning (dense matrix: bin_rows; raw records: the fused encode -> bins kernel)
+        bad = torch.zeros(2, dtype=torch.int32, device=dev)
+        tp, _ = src.bin(thresholds, n_thr, arity_dev, mpb, bad)
+        feat_bins = torch.where(arity_dev > 0, arity_dev, n_thr + 1).to(torch.int32).contiguous()
+        feat_kind = _i32(kind, dev)
+        # ---- de-duplicate the binned rows: the level loop runs on UNIQUE TreePoint records carrying summed bag weights.
+        # Everything is enqueued first; ONE host read then fetches the bad-cell counts, the bin count, the sample count and U.
+        dedup = n > 0 and DEDUP
+        if dedup:
+            tp, uid, u_dev = dedup_rows(tp, F + 1, sync=False)
+        else:
+            uid, u_dev = None, torch.full((1,), n, dtype=torch.int64, device=dev)
+        self.src, self.group, self.n, self.F, self.n_global = src, group, n, F, n_global
+        self.mpb, self.kind, self.m, self.arity, self.arity_dev = mpb, kind, m, arity, arity_dev
+        self.has_cont, self.cap, self.n_s_dev, self.thresholds, self.n_thr = has_cont, cap, n_s_dev, thresholds, n_thr
+        self.bad, self.tp, self.feat_bins, self.feat_kind = bad, tp, feat_bins, feat_kind
+        self.dedup, self.uid, self.u_dev = dedup, uid, u_dev
+
+    def read(self):
+        """-> self with n_bins (the widest feature's bin count), U (unique records) and tp trimmed to them; head = the host copy
+        of [bad cells, NaN cells, n_bins, sample count, U, feat_bins...]."""
+        bad, feat_bins, n_s_dev, u_dev, tp, F = self.bad, self.feat_bins, self.n_s_dev, self.u_dev, self.tp, self.F
+        has_cont, group, cap, dedup, dev = self.has_cont, self.group, self.cap, self.dedup, self.src.device
+        stride = tp_stride(F)
+        head = torch.cat([bad.to(torch.int64), feat_bins.max().reshape(1).to(torch.int64), n_s_dev.to(torch.int64), u_dev,
+                          feat_bins.to(torch.int64)]).cpu()
+        if int(head[1]) != 0:
+            raise InvalidRowsError("%d NaN/null cells or unseen labels in the training rows" % int(head[1]))
+        if int(head[0]) != 0:
+            raise ValueError("categorical feature value outside [0, arity) or non-integral in %d cells" % int(head[0]))
+        if has_cont and group is None and int(head[3]) > cap:
+            raise B200FlowError("findSplits sample overflow (%d > %d)" % (int(head[3]), cap))
+        n_bins, U = int(head[2]), int(head[4])
+        if dedup:
+            tp = tp[:U]
+        if tp.shape[0] == 0:                                  # a rank without rows still walks the level loop (its collectives): give the
+            tp = torch.zeros((1, stride), dtype=torch.uint8, device=dev)   # kernels a real pointer (data_ptr() of an empty tensor is NULL)
+        self.head, self.n_bins, self.U, self.tp = head, n_bins, U, tp
+        return self
+
+
 def fit_forest(x, labels, num_classes, arity, params, row_offset=0, group=None):
     """RandomForest.run (R4-R8) on a dense CUDA feature matrix x [n, F] (f32/f64) and int32 labels [n].
 
@@ -498,53 +582,11 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
         raise ValueError("numClasses must be in [1, 256] (labels are stored as one byte), got %d" % C)
     T = int(p.num_trees)
     seed = int(p.seed) & 0xFFFFFFFFFFFFFFFF
-    n_global = n
-    if group is not None:
-        t = torch.tensor([n], dtype=torch.int64, device=dev)
-        bdist.all_reduce_(t, group)
-        n_global = int(t.item())
-    mpb, kind, m = build_metadata(n_global, F, C, arity, p.max_bins, T, p.feature_subset_strategy)
-    arity = np.asarray(arity, np.int32)
-    arity_dev = _i32(arity, dev)
-
-    # ---- R4 findSplits: Bernoulli row sample keyed by global row, sort + stride walk on device
-    has_cont = bool((arity == 0).any())
-    frac = min(1.0, max(mpb * mpb, 10000) / float(max(n_global, 1))) if has_cont else 1.0
-    keep = int(frac * 4294967296.0)
-    expect = n if frac >= 1.0 else int(n * frac + 6.0 * math.sqrt(max(n * frac, 1.0)) + 64)
-    cap = 1
-    while cap < max(min(expect, n), 2):
-        cap <<= 1
-    sample = torch.empty(F * cap, dtype=torch.float64, device=dev)
-    n_s_dev = torch.zeros(1, dtype=torch.int32, device=dev)
-    thresholds = torch.zeros((F, mpb - 1), dtype=torch.float64, device=dev)
-    n_thr = torch.zeros(F, dtype=torch.int32, device=dev)
-    if has_cont:
-        src.sample(seed, keep, row_offset, sample, cap, n_s_dev)
-        if group is not None:
-            n_s = int(n_s_dev.item())
-            if n_s > cap:
-                raise B200FlowError("findSplits sample overflow (%d > %d)" % (n_s, cap))
-            sample, n_s, cap = _gather_sample(sample, n_s, cap, F, group)
-            call("b200flow_find_splits", ptr(sample), cap, n_s, F, ptr(arity_dev), mpb, ptr(thresholds), ptr(n_thr), None)
-        else:       # single GPU: the sample count stays on the device (checked with the other counts below: one host sync)
-            call("b200flow_find_splits", ptr(sample), cap, cap, F, ptr(arity_dev), mpb, ptr(thresholds), ptr(n_thr), ptr(n_s_dev))
-    del sample
-
-    # ---- R5 binning (dense matrix: bin_rows; raw records: the fused encode -> bins kernel)
+    rows = _TrainingRows(src, C, arity, p.max_bins, T, p.feature_subset_strategy, seed, row_offset, group)
+    mpb, kind, m, arity = rows.mpb, rows.kind, rows.m, rows.arity
+    thresholds, n_thr, feat_bins, feat_kind, uid, dedup = rows.thresholds, rows.n_thr, rows.feat_bins, rows.feat_kind, rows.uid, rows.dedup
     stride = tp_stride(F)
-    bad = torch.zeros(2, dtype=torch.int32, device=dev)
-    tp, _ = src.bin(thresholds, n_thr, arity_dev, mpb, bad)
-    feat_bins = torch.where(arity_dev > 0, arity_dev, n_thr + 1).to(torch.int32).contiguous()
-    feat_kind = _i32(kind, dev)
-    # ---- de-duplicate the binned rows: the level loop runs on UNIQUE TreePoint records carrying summed bag weights.
-    # Everything is enqueued first; ONE host read then fetches the bad-cell counts, the bin count, the sample count and U.
     total = torch.zeros(1, dtype=torch.int64, device=dev)
-    dedup = n > 0 and DEDUP
-    if dedup:
-        tp, uid, u_dev = dedup_rows(tp, F + 1, sync=False)
-    else:
-        uid, u_dev = None, torch.full((1,), n, dtype=torch.int64, device=dev)
     # host-side preparation that does not depend on the counts runs BEFORE the read, while the GPU works through the queue
     bagging = p.bootstrap and T > 1
     cdf_host = np.ascontiguousarray(poisson_cdf_table(p.subsampling_rate)) if bagging else None
@@ -579,19 +621,9 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
             node_mask = ext(node_mask, (4,))
         cap_nodes = new_cap
 
-    head = torch.cat([bad.to(torch.int64), feat_bins.max().reshape(1).to(torch.int64), n_s_dev.to(torch.int64), u_dev,
-                      feat_bins.to(torch.int64)]).cpu()
-    if int(head[1]) != 0:
-        raise InvalidRowsError("%d NaN/null cells or unseen labels in the training rows" % int(head[1]))
-    if int(head[0]) != 0:
-        raise ValueError("categorical feature value outside [0, arity) or non-integral in %d cells" % int(head[0]))
-    if has_cont and group is None and int(head[3]) > cap:
-        raise B200FlowError("findSplits sample overflow (%d > %d)" % (int(head[3]), cap))
-    n_bins, U = int(head[2]), int(head[4])
-    if dedup:
-        tp = tp[:U]
-    if tp.shape[0] == 0:                                  # a rank without rows still walks the level loop (its collectives): give the
-        tp = torch.zeros((1, stride), dtype=torch.uint8, device=dev)   # kernels a real pointer (data_ptr() of an empty tensor is NULL)
+    rows.read()
+    n_bins, U, tp, head = rows.n_bins, rows.U, rows.tp, rows.head
+    del rows
     # launch shape of the fused kernel: entries per routing chunk and subset features per pass (wide nodes — many classes,
     # or a DecisionTree's all-feature histograms — are accumulated in several feature passes, the first of which routes)
     desc_host, rec_bytes = _lib.packed_layout(head[5:5 + F].numpy(), C) if FUSED else (None, 0)

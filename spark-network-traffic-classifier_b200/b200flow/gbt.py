@@ -1,0 +1,312 @@
+"""GBTClassifier (binary, LogLoss) on libb200flow.so: GradientBoostedTrees.boost with one regression tree per iteration
+(DESIGN.md §5e).
+
+Host logic only.  findSplits, binning and the de-duplication of the binned rows are the forest's (forest._TrainingRows,
+once per fit); every tree runs the forest's level loop with the variance kernels of csrc/gbt.cu.  Residuals sit on a
+fixed-point grid, so the level histograms are exact int64 sums: with rows sharded over ranks the one all-reduce per level
+is exact and the model is the same bits for any number of ranks.
+"""
+import math
+from dataclasses import dataclass
+
+import numpy as np
+import torch
+
+from . import _lib
+from . import forest as fr
+from ._lib import NODE_DTYPE, B200FlowError, call, ptr
+
+PROFILE = None                     # set to a dict to collect per-phase CUDA-event timings (tools/bench_gbt.py)
+
+
+def _timed(name, fn, *args):
+    if PROFILE is None:
+        return call(fn, *args)
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    call(fn, *args)
+    e1.record()
+    PROFILE.setdefault(name, []).append((e0, e1))
+
+
+@dataclass
+class GBTParams:
+    """Spark 3 GBTClassifier Param defaults."""
+    max_iter: int = 20
+    step_size: float = 0.1
+    max_depth: int = 5
+    max_bins: int = 32
+    min_instances_per_node: int = 1
+    min_info_gain: float = 0.0
+    subsampling_rate: float = 1.0
+    feature_subset_strategy: str = "all"
+    seed: int = 0
+
+
+def grid_shift(n_global):
+    """(S, S2) of the residual grid: q = rint(r 2^S), q2 = rint(r̂^2 2^S2); |r| <= 4 keeps every sum over n rows below 2^62."""
+    lg = int(math.ceil(math.log2(max(int(n_global), 2))))
+    return 60 - lg, 58 - lg
+
+
+def subsample_cdf(rate):
+    """the one-threshold inverse CDF that makes b200flow_bag_weights draw Bernoulli(rate) weights in {0, 1}"""
+    cdf = np.full(32, 0xFFFFFFFF, np.uint32)
+    cdf[0] = int(math.floor((1.0 - rate) * 4294967296.0))
+    return cdf
+
+
+class GBTModel:
+    """Device-resident boosted trees: one node pool (roots = nodes 0..T-1), payload[node] = tree weight x leaf value."""
+
+    def __init__(self, forest, tree_weights, stats, S):
+        self.forest = forest                            # ForestModel with C = 1 over the payloads: binning and the tree walk
+        self.T, self.F = forest.T, forest.F
+        self.tree_weights = list(tree_weights)
+        self.stats, self.S = stats, S                   # int64 [pool][3] {Σw, Σw·q, Σw·q2}
+
+    @property
+    def n_nodes(self):
+        return self.forest.n_nodes
+
+    def margin(self, x):
+        """Σ_t payload of the leaf each row reaches, in tree order from +0.0 (GBTClassificationModel.margin)."""
+        raw, _, _ = self.forest.predict(x, want_raw=True, want_prob=False)
+        return raw.view(-1)
+
+    def _output(self, margin):
+        n = margin.shape[0]
+        dev = margin.device
+        raw = torch.empty((n, 2), dtype=torch.float64, device=dev)
+        prob = torch.empty((n, 2), dtype=torch.float64, device=dev)
+        pred = torch.empty(n, dtype=torch.float64, device=dev)
+        call("b200flow_gbt_output", ptr(margin.contiguous()), n, ptr(raw), ptr(prob), ptr(pred))
+        return raw, prob, pred
+
+    def predict(self, x):
+        """-> (rawPrediction [n, 2], probability [n, 2], prediction [n]) on a dense feature matrix."""
+        return self._output(self.margin(x))
+
+    def predict_records(self, rec, plan, round_f32=False, on_invalid="ignore"):
+        """the same from raw flow records + the encode plan of the feature vector (fused encode -> bins)"""
+        raw, _, _, _ = self.forest.predict_records(rec, plan, want_raw=True, want_prob=False, round_f32=round_f32,
+                                                   on_invalid=on_invalid)
+        return self._output(raw.view(-1))
+
+    def export(self):
+        """canonical host copy ordered by (tree, node id): the forest export's structure + payload, gain and int64 stats"""
+        fo = self.forest
+        n = fo.n_nodes
+        nodes = fo.nodes[:n].cpu().numpy().view(NODE_DTYPE).reshape(-1)
+        tree = fo.node_tree[:n].cpu().numpy()
+        order = np.lexsort((nodes["nid"], tree))
+        mask = (fo.node_mask[:n].cpu().numpy().view(np.uint64) if fo.node_mask is not None else np.zeros((n, 4), np.uint64))
+        is_leaf = (nodes["feat"] < 0).astype(np.int32)
+        kind = np.where(is_leaf == 1, 0, nodes["kind_bin"] >> 16).astype(np.int32)
+        bin_thr = np.where(is_leaf == 1, 0, nodes["kind_bin"] & 0xffff).astype(np.int32)
+        mask = np.where(is_leaf[:, None] == 1, 0, mask).astype(np.uint64)
+        return dict(tree=tree[order], nid=nodes["nid"][order], feat=np.where(is_leaf == 1, -1, nodes["feat"])[order],
+                    kind=kind[order], bin_thr=bin_thr[order], is_leaf=is_leaf[order], mask=mask[order],
+                    gain=fo.node_gain[:n].cpu().numpy()[order], payload=fo.leaf_prob[:n, 0].cpu().numpy()[order],
+                    stats=self.stats[:n].cpu().numpy()[order])
+
+    def feature_importances(self):
+        """featureImportances with perTreeNormalization = false (SPARK-26721): Σ gain · count over the internal nodes of all
+        trees, normalised once."""
+        ex = self.export()
+        v = np.zeros(self.F)
+        sel = ex["is_leaf"] == 0
+        np.add.at(v, ex["feat"][sel], ex["gain"][sel] * ex["stats"][sel, 0].astype(np.float64))
+        return v / v.sum() if v.sum() > 0 else v
+
+
+def fit_gbt(x, labels, arity, params, row_offset=0, group=None):
+    """GradientBoostedTrees.boost on a dense CUDA feature matrix x [n, F] (f32/f64) and labels [n] in {0, 1}.  arity as
+    for fit_forest; with `group`, x / labels are this rank's row shard starting at global row `row_offset`."""
+    return _fit(fr._DenseSource(x, labels), arity, params, row_offset, group)
+
+
+def fit_gbt_records(rec, plan, arity, params, row_offset=0, group=None, round_f32=False):
+    """the same on raw flow records [n, row_bytes] + the encode plan of their feature vector (plan.label = a label column
+    with at most two values)"""
+    if plan.label is None:
+        raise ValueError("fit_gbt_records: the encode plan has no label column (EncodePlan.set_label)")
+    return _fit(fr._RecordSource(rec, plan, round_f32), arity, params, row_offset, group)
+
+
+def _fit(src, arity, params, row_offset=0, group=None):
+    from . import dist as bdist
+    _lib.require_cuda()
+    p = params
+    if not (0 <= p.max_depth <= 30):
+        raise ValueError("maxDepth must be in [0, 30], got %d" % p.max_depth)
+    if int(p.max_iter) < 1:
+        raise ValueError("maxIter must be >= 1, got %d" % p.max_iter)
+    if not (0.0 < p.step_size <= 1.0):
+        raise ValueError("stepSize must be in (0, 1], got %r" % p.step_size)
+    if not (0.0 < p.subsampling_rate <= 1.0):
+        raise ValueError("subsamplingRate must be in (0, 1], got %r" % p.subsampling_rate)
+    dev = src.device
+    n, F = src.n, src.F
+    T = int(p.max_iter)
+    seed = int(p.seed) & 0xFFFFFFFFFFFFFFFF
+    strategy = "all" if str(p.feature_subset_strategy) == "auto" else p.feature_subset_strategy
+    rows = fr._TrainingRows(src, 2, arity, p.max_bins, 1, strategy, seed, row_offset, group).read()
+    tp, uid, U, m, n_bins = rows.tp, rows.uid, rows.U, rows.m, rows.n_bins
+    feat_bins, feat_kind, stride = rows.feat_bins, rows.feat_kind, fr.tp_stride(F)
+    S, S2 = grid_shift(rows.n_global)
+    # labels must be 0 or 1 on EVERY rank: the flag is summed over the ranks first, so that all of them raise together
+    bad = (tp[:U, F] > 1).any().reshape(1).to(torch.int64) if U > 0 else torch.zeros(1, dtype=torch.int64, device=dev)
+    if group is not None:
+        bdist.all_reduce_(bad, group)
+    if int(bad.item()):
+        raise ValueError("GBTClassifier currently only supports binary classification: a label is not 0 or 1")
+
+    # subsampling weights W[iteration][unique record] (Bernoulli, tree index = iteration); without subsampling every
+    # iteration sees each unique record with its multiplicity
+    sub = p.subsampling_rate < 1.0
+    TW = T if sub else 1
+    W = torch.zeros(max(TW * U, 1), dtype=torch.int32, device=dev)
+    if n > 0:
+        cdf_host = subsample_cdf(p.subsampling_rate) if sub else None
+        call("b200flow_bag_weights", seed, TW, int(row_offset), n, ptr(_lib.h2d(cdf_host.view(np.int32), dev)) if sub else None,
+             cdf_host.ctypes.data if sub else None, ptr(uid), None, U, ptr(W))
+    del uid
+
+    # node pool: roots 0..T-1; a node's stats are 3 int64 = the 6 opaque words grow_level copies per node
+    cap_nodes = max(1024, T * min(1 << (p.max_depth + 1), 64))
+    nodes = torch.zeros((cap_nodes, 16), dtype=torch.uint8, device=dev)
+    node_mask = torch.zeros((cap_nodes, 4), dtype=torch.int64, device=dev) if bool((rows.kind > 0).any()) else None
+    stats = torch.zeros((cap_nodes, 3), dtype=torch.int64, device=dev)
+    node_tree = torch.zeros(cap_nodes, dtype=torch.int32, device=dev)
+    node_gain = torch.zeros(cap_nodes, dtype=torch.float64, device=dev)
+    root = np.zeros(T, NODE_DTYPE); root["feat"] = -1; root["left"] = -1; root["nid"] = 1
+    nodes[:T] = _lib.h2d(root.view(np.uint8).reshape(T, 16), dev)
+    node_tree[:T] = torch.arange(T, dtype=torch.int32, device=dev)
+    pool_size = T
+
+    def grow_pool(need):
+        nonlocal nodes, node_mask, stats, node_tree, node_gain, cap_nodes
+        if need <= cap_nodes:
+            return
+        new_cap = cap_nodes
+        while new_cap < need:
+            new_cap *= 2
+        def ext(t):
+            nt = torch.zeros((new_cap,) + tuple(t.shape[1:]), dtype=t.dtype, device=dev)
+            nt[:cap_nodes] = t
+            return nt
+        nodes, stats, node_tree, node_gain = ext(nodes), ext(stats), ext(node_tree), ext(node_gain)
+        if node_mask is not None:
+            node_mask = ext(node_mask)
+        cap_nodes = new_cap
+
+    weights = [1.0] + [float(p.step_size)] * (T - 1)
+    tree_weight = _lib.h2d(np.asarray(weights, np.float64), dev)
+    payload = torch.zeros(cap_nodes, dtype=torch.float64, device=dev)
+    margin = torch.zeros(max(U, 1), dtype=torch.float64, device=dev)
+    rq = torch.zeros((max(U, 1), 2), dtype=torch.int64, device=dev)
+    call("b200flow_gbt_update", ptr(tp), stride, F, U, None, None, None, -1, S, S2, ptr(margin), ptr(rq))
+
+    nb = (U + 1023) // 1024
+    blk_cnt = torch.zeros(max(nb, 1), dtype=torch.int32, device=dev)
+    blk_off = torch.zeros(nb + 1, dtype=torch.int64, device=dev)
+    total = torch.zeros(1, dtype=torch.int64, device=dev)
+    ent = torch.empty((max(U, 1), 2), dtype=torch.int32, device=dev)
+    ent2 = torch.empty_like(ent)
+    CH = fr.CHUNK_ROWS
+    stats_t = dict(levels=0, slots=0, rows=n, unique_rows=U, S=S)
+
+    def chunk_table(lens):
+        """(device chunk offsets, their host copy) of the slots' entry ranges"""
+        nch = ((lens + (CH - 1)) // CH).to(torch.int32).contiguous()
+        off = torch.empty(nch.shape[0] + 1, dtype=torch.int64, device=dev)
+        call("b200flow_exclusive_scan_i32_to_i64", ptr(nch), nch.shape[0], ptr(off), ptr(total))
+        return off, off.cpu()
+
+    per_slot = m * n_bins * 3
+    group_slots = max(1, fr.HIST_BUDGET_BYTES // (per_slot * 8))
+
+    counters = torch.zeros(8 + 2 * 64 + 1024, dtype=torch.int64, device=dev)
+    for t in range(T):
+        # ---- this iteration's entries {unique record, weight}: the non-zero weights, in unique-id order
+        Wt = W[(t if sub else 0) * U:(t if sub else 0) * U + max(U, 1)]
+        if U > 0:
+            call("b200flow_bag_count", ptr(Wt), 1, U, ptr(blk_cnt))
+        call("b200flow_exclusive_scan_i32_to_i64", ptr(blk_cnt), nb, ptr(blk_off), ptr(total))
+        if U > 0:
+            call("b200flow_bag_fill", ptr(Wt), 1, U, ptr(blk_off), ptr(ent))
+        seg_begin = torch.zeros(1, dtype=torch.int64, device=dev)
+        seg_end = total.clone()
+        slot_tree = torch.full((1,), t, dtype=torch.int32, device=dev)
+        slot_nid = torch.ones(1, dtype=torch.int32, device=dev)
+        slot_node = torch.full((1,), t, dtype=torch.int32, device=dev)
+        counters[0] = pool_size
+        n_slots, level = 1, 0
+        while n_slots > 0:
+            grow_pool(pool_size + 2 * n_slots)
+            if counters.numel() < 8 + 2 * ((n_slots + 255) // 256):
+                counters = torch.cat([counters, torch.zeros(2 * n_slots, dtype=torch.int64, device=dev)])
+            subset = torch.empty((n_slots, m), dtype=torch.int16, device=dev)
+            call("b200flow_feature_subsets", seed, n_slots, ptr(slot_tree), ptr(slot_nid), F, m, ptr(subset))
+            chunk_off, off_h = chunk_table(seg_end - seg_begin)
+            n_chunks = int(off_h[-1])
+            split = torch.empty((n_slots, 64), dtype=torch.uint8, device=dev)
+            st = torch.empty((3, n_slots, 3), dtype=torch.int64, device=dev)   # node, left, right
+            for g0 in range(0, n_slots, group_slots):      # slot groups keep one level's histograms within HIST_BUDGET_BYTES
+                g1 = min(n_slots, g0 + group_slots)
+                hist = torch.zeros((g1 - g0) * per_slot, dtype=torch.int64, device=dev)
+                gch = int(off_h[g1] - off_h[g0])
+                if gch > 0:
+                    coff = (chunk_off[g0:g1 + 1] - chunk_off[g0]).contiguous()
+                    _timed("gbt_hist_level", "b200flow_gbt_hist_level", ptr(tp), stride, ptr(ent), ptr(rq), g1 - g0,
+                           ptr(seg_begin[g0:g1]), ptr(seg_end[g0:g1]), ptr(coff), gch, CH, ptr(subset[g0:g1]), m, n_bins, ptr(hist))
+                if group is not None:                   # the one data-path collective: exact int64 sums
+                    bdist.all_reduce_(hist, group)
+                _timed("gbt_score_level", "b200flow_gbt_score_level", ptr(hist), g1 - g0, ptr(subset[g0:g1]), m, n_bins,
+                       ptr(feat_bins), ptr(feat_kind), S, S2, level, p.max_depth, int(p.min_instances_per_node),
+                       float(p.min_info_gain), ptr(split[g0:g1]), ptr(st[0, g0:g1]), ptr(st[1, g0:g1]), ptr(st[2, g0:g1]))
+                del hist
+            next_tree = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
+            next_nid = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
+            next_node = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
+            next_parent = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
+            _timed("grow_level", "b200flow_grow_level", n_slots, ptr(slot_tree), ptr(slot_nid), ptr(slot_node), ptr(split), ptr(st[0]),
+                   ptr(st[1]), ptr(st[2]), 6, ptr(nodes), ptr(node_mask), ptr(stats), ptr(node_tree), cap_nodes, ptr(next_tree),
+                   ptr(next_nid), ptr(next_node), ptr(next_parent), None, ptr(counters))
+            node_gain[slot_node.long()] = split.view(torch.float64)[:, 2]
+            cnt = counters[:3].cpu()
+            if int(cnt[2]) != 0:
+                raise B200FlowError("node pool overflow (capacity %d)" % cap_nodes)
+            pool_size, n_next = int(cnt[0]), int(cnt[1])
+            stats_t["levels"] += 1; stats_t["slots"] += n_slots
+            if n_next == 0:
+                break
+            cursors = torch.zeros(2 * n_slots, dtype=torch.int32, device=dev)
+            if n_chunks > 0:
+                _timed("partition_level", "b200flow_partition_level", ptr(tp), stride, ptr(ent), ptr(ent2), n_slots, ptr(seg_begin),
+                       ptr(seg_end), ptr(chunk_off), n_chunks, CH, ptr(split), ptr(cursors))
+            next_begin = torch.empty(n_next, dtype=torch.int64, device=dev)
+            next_end = torch.empty(n_next, dtype=torch.int64, device=dev)
+            call("b200flow_next_segments", n_next, None, ptr(next_parent), ptr(seg_begin), ptr(seg_end), ptr(cursors), ptr(next_begin),
+                 ptr(next_end))
+            ent, ent2 = ent2, ent
+            slot_tree, slot_nid, slot_node = next_tree[:n_next], next_nid[:n_next], next_node[:n_next]
+            seg_begin, seg_end = next_begin, next_end
+            n_slots = n_next
+            level += 1
+        # ---- leaf values of the pool so far, then F and the next residuals of every unique record
+        if payload.shape[0] < cap_nodes:
+            payload = torch.zeros(cap_nodes, dtype=torch.float64, device=dev)
+        call("b200flow_gbt_leaf_values", pool_size, ptr(stats), ptr(node_tree), ptr(tree_weight), S, ptr(payload))
+        _timed("gbt_update", "b200flow_gbt_update", ptr(tp), stride, F, U, ptr(nodes), ptr(node_mask), ptr(payload), t, S, S2,
+               ptr(margin), ptr(rq))
+
+    forest = fr.ForestModel(T, 1, F, rows.arity, rows.mpb, rows.thresholds, rows.n_thr, nodes, node_mask, None, node_tree,
+                            payload[:pool_size].reshape(pool_size, 1).contiguous(), node_gain, pool_size, dt_mode=False)
+    model = GBTModel(forest, weights, stats, S)
+    model.train_stats = stats_t
+    model.train_margin = margin[:U]                      # F of every unique training record (rows: train_margin[train_uid])
+    model.train_uid = rows.uid
+    model.feat_kind, model.feat_bins, model.n_bins, model.m = rows.kind, feat_bins, n_bins, m
+    return model

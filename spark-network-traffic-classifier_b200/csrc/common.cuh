@@ -176,6 +176,13 @@ template <> __device__ __forceinline__ double load_as_double<double>(const void*
     return __ldg((const double*)base + idx);
 }
 
+// chunk id -> (slot, chunk-in-slot) by binary search over the exclusive scan chunk_off[n_slots+1]
+__device__ __forceinline__ int find_slot(const int64_t* __restrict__ chunk_off, int n_slots, int64_t c) {
+    int lo = 0, hi = n_slots;                          // last s with chunk_off[s] <= c
+    while (hi - lo > 1) { int mid = (lo + hi) >> 1; if (__ldg(chunk_off + mid) <= c) lo = mid; else hi = mid; }
+    return lo;
+}
+
 inline int grid_for(int64_t work_items, int per_block, int max_blocks) {
     int64_t b = (work_items + per_block - 1) / per_block;
     if (b < 1) b = 1;

@@ -53,13 +53,6 @@ __global__ void __launch_bounds__(128) feature_subsets_kernel(uint64_t seed, int
     for (int i = 0; i < m; ++i) out[i] = pick[i];
 }
 
-// chunk id -> (slot, chunk-in-slot) by binary search over the exclusive scan chunk_off[n_slots+1]
-__device__ __forceinline__ int find_slot(const int64_t* __restrict__ chunk_off, int n_slots, int64_t c) {
-    int lo = 0, hi = n_slots;                          // last s with chunk_off[s] <= c
-    while (hi - lo > 1) { int mid = (lo + hi) >> 1; if (__ldg(chunk_off + mid) <= c) lo = mid; else hi = mid; }
-    return lo;
-}
-
 // ------------------------------------------------------------------ R7 histogram build (HOT LOOP A)
 __global__ void __launch_bounds__(256) hist_level_kernel(const uint8_t* __restrict__ tp, int stride, int F,
                                                          const b2f_entry* __restrict__ ent, int n_slots, const int64_t* __restrict__ seg_begin,

@@ -2,6 +2,8 @@
 
 RandomForestClassifier / DecisionTreeClassifier (kdd99.py:61,64; cicids17.py:65,68) are the hot path and run
 entirely on the b200flow CUDA kernels (histogram build, Gini split scoring, batch predict).
+GBTClassifier (binary) runs on the variance-histogram level loop of csrc/gbt.cu (b200flow/gbt.py, DESIGN.md §5e); its
+model is the same bits for any number of ranks.
 MultilayerPerceptronClassifier runs on the fused fp64 tensor-core loss/gradient and forward kernels (b200flow/mlp.py,
 csrc/mlp.cu, DESIGN.md §5d); its model is the same bits for any number of ranks.
 LogisticRegression and NaiveBayes (kdd99.py:57,67; cicids17.py:61,71) are OUT of the kernel scope (SURVEY.md
@@ -473,3 +475,168 @@ class MultilayerPerceptronClassificationModel(_ProbModel, _MLPParams):
         except ValueError as e:
             raise IllegalArgumentException(str(e))
         return self._emit(df, raw, torch.softmax(raw, 1))
+
+
+# ------------------------------------------------------------------------------- gradient-boosted trees (CUDA)
+class _GBTParams(_TreeParams):
+    _defaults = {"impurity": "variance", "maxIter": 20, "stepSize": 0.1, "subsamplingRate": 1.0, "featureSubsetStrategy": "all",
+                 "lossType": "logistic", "validationTol": 0.01, "validationIndicatorCol": None, "weightCol": None,
+                 "minWeightFractionPerNode": 0.0, "leafCol": ""}
+
+
+class GBTClassifier(Estimator, _GBTParams):
+    """Spark 3's GBTClassifier: binary LogLoss boosting of regression trees (variance impurity), trained on the device with
+    exact fixed-point histograms (b200flow/gbt.py, csrc/gbt.cu, DESIGN.md §5e); the model is the same bits for any number
+    of ranks."""
+
+    def __init__(self, featuresCol=None, labelCol=None, predictionCol=None, maxDepth=None, maxBins=None, minInstancesPerNode=None,
+                 minInfoGain=None, maxMemoryInMB=None, cacheNodeIds=None, checkpointInterval=None, lossType=None, maxIter=None,
+                 stepSize=None, seed=None, subsamplingRate=None, impurity=None, featureSubsetStrategy=None, validationTol=None,
+                 validationIndicatorCol=None, leafCol=None, minWeightFractionPerNode=None, weightCol=None, probabilityCol=None,
+                 rawPredictionCol=None):
+        kw = dict(locals()); kw.pop("self"); kw.pop("__class__", None)
+        super().__init__(**kw)
+
+    def _params(self):
+        """Spark's param validators, and the params the device trainer does not implement."""
+        from b200flow import gbt as _gbt
+        g = self.getOrDefault
+        if str(g("lossType")).lower() != "logistic":
+            raise IllegalArgumentException("GBTClassifier lossType must be 'logistic', got %r" % (g("lossType"),))
+        if str(g("impurity")).lower() != "variance":
+            raise IllegalArgumentException("GBTClassifier trains regression trees: impurity must be 'variance', got %r" % (g("impurity"),))
+        if g("validationIndicatorCol"):
+            raise IllegalArgumentException("validationIndicatorCol (early stopping) is not supported by the b200flow GBT trainer")
+        if g("weightCol"):
+            raise IllegalArgumentException("weightCol is not supported by the b200flow GBT trainer")
+        if float(g("minWeightFractionPerNode")) != 0.0:
+            raise IllegalArgumentException("minWeightFractionPerNode must be 0.0 on the b200flow GBT trainer")
+        it, step, rate = g("maxIter"), float(g("stepSize")), float(g("subsamplingRate"))
+        if int(it) != it or int(it) < 1:
+            raise IllegalArgumentException("maxIter must be an integer >= 1, got %r" % (it,))
+        if not 0.0 < step <= 1.0:
+            raise IllegalArgumentException("stepSize must be in (0, 1], got %r" % (step,))
+        if not 0.0 < rate <= 1.0:
+            raise IllegalArgumentException("subsamplingRate must be in (0, 1], got %r" % (rate,))
+        if int(g("maxBins")) < 2 or int(g("minInstancesPerNode")) < 1 or float(g("minInfoGain")) < 0.0 or int(g("maxDepth")) < 0:
+            raise IllegalArgumentException("maxBins >= 2, minInstancesPerNode >= 1, minInfoGain >= 0 and maxDepth >= 0 are required")
+        seed = g("seed")
+        return _gbt.GBTParams(max_iter=int(it), step_size=step, max_depth=int(g("maxDepth")), max_bins=int(g("maxBins")),
+                              min_instances_per_node=int(g("minInstancesPerNode")), min_info_gain=float(g("minInfoGain")),
+                              subsampling_rate=rate, feature_subset_strategy=str(g("featureSubsetStrategy")),
+                              seed=_default_seed(self) if seed is None else int(seed))
+
+    def _fit(self, df):
+        from b200flow import gbt as _gbt
+        from .feature import SparkException
+        p = self._params()
+        binary_only = "GBTClassifier currently only supports binary classification, but %d classes were found"
+        fused = _records_fit_inputs(df, self)
+        try:
+            grp = bdist.group()
+            if fused is not None:                           # lazy VectorAssembler output: bin straight from the raw records
+                rec, plan, C, attrs = fused
+                if C > 2:
+                    raise IllegalArgumentException(binary_only % C)
+                off, _ = bdist.global_offset(rec.shape[0], rec.device, grp)
+                model = _gbt.fit_gbt_records(rec, plan, _arity_from_attrs(attrs, plan.n_out), p, row_offset=off, group=grp)
+            else:
+                x, y, C, attrs = _features_and_labels(df, self)
+                if C > 2:
+                    raise IllegalArgumentException(binary_only % C)
+                off, _ = bdist.global_offset(x.shape[0], x.device, grp)
+                model = _gbt.fit_gbt(x, y.to(torch.int32), _arity_from_attrs(attrs, x.shape[1]), p, row_offset=off, group=grp)
+        except fr.InvalidRowsError as e:
+            raise SparkException("Encountered NaN/null while assembling a row with handleInvalid = \"error\" (%s)" % e)
+        except ValueError as e:        # includes b200flow's UnsupportedParamError; CUDA failures propagate as they are
+            raise IllegalArgumentException(str(e))
+        m = GBTClassificationModel(model)
+        m._paramMap = {k: v for k, v in self._paramMap.items() if k in m._all_defaults()}
+        return m
+
+
+class GBTClassificationModel(Model, _GBTParams):
+    def __init__(self, gbt):
+        super().__init__()
+        self._gbt = gbt
+
+    @property
+    def numClasses(self):
+        return 2
+
+    @property
+    def numFeatures(self):
+        return self._gbt.F
+
+    @property
+    def getNumTrees(self):
+        return self._gbt.T
+
+    @property
+    def treeWeights(self):
+        return list(self._gbt.tree_weights)
+
+    @property
+    def totalNumNodes(self):
+        return self._gbt.n_nodes
+
+    @property
+    def featureImportances(self):
+        from .linalg import DenseVector
+        return DenseVector(self._gbt.feature_importances())
+
+    def _transform(self, df):
+        fcol = self.getOrDefault("featuresCol")
+        if fcol not in df._cols or df._cols[fcol].kind != "vector":
+            raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+        plan = _lazy_plan(df, fcol)
+        if plan is not None and plan.n_out == self._gbt.F:      # lazy features: fused encode -> bins -> tree walk
+            from .feature import SparkException
+            try:
+                raw, prob, pred = self._gbt.predict_records(df._rec, plan, on_invalid="error" if plan.check_nan else "ignore")
+            except fr.InvalidRowsError as e:
+                raise SparkException("Encountered NaN/null while assembling a row with handleInvalid = \"error\" (%s)" % e)
+        else:
+            raw, prob, pred = self._gbt.predict(df._cols[fcol].data)
+        cols = dict(df._cols)
+        for name, val, kind in ((self.getOrDefault("rawPredictionCol"), raw, "vector"),
+                                (self.getOrDefault("probabilityCol"), prob, "vector"),
+                                (self.getOrDefault("predictionCol"), pred, "numeric")):
+            if name:
+                if name in cols:
+                    raise IllegalArgumentException("Output column %s already exists." % name)
+                cols[name] = ColumnData(kind, val, "f64")
+        return df._with(cols=cols)
+
+    @property
+    def toDebugString(self):
+        ex = self._gbt.export()
+        thr = self._gbt.forest.thresholds.cpu().numpy()
+        parts = ["GBTClassificationModel with %d trees" % self._gbt.T]
+        for t in range(self._gbt.T):
+            sel = np.nonzero(ex["tree"] == t)[0]
+            idx = {int(ex["nid"][i]): i for i in sel}
+            parts.append("  Tree %d (weight %r):" % (t, self._gbt.tree_weights[t]))
+
+            def rec(nid, depth):
+                i = idx[nid]
+                pad = "  " + " " * (depth + 1)
+                if ex["is_leaf"][i]:
+                    st = ex["stats"][i]
+                    parts.append("%sPredict: %r" % (pad, float(st[1]) * 2.0 ** -self._gbt.S / float(st[0])))
+                    return
+                f = int(ex["feat"][i])
+                if ex["kind"][i] == 0:
+                    v = repr(float(thr[f, int(ex["bin_thr"][i])]))
+                    parts.append("%sIf (feature %d <= %s)" % (pad, f, v)); rec(nid * 2, depth + 1)
+                    parts.append("%sElse (feature %d > %s)" % (pad, f, v)); rec(nid * 2 + 1, depth + 1)
+                else:
+                    cats = [c for c in range(256) if (int(ex["mask"][i][c >> 6]) >> (c & 63)) & 1]
+                    s = "{%s}" % ",".join("%.1f" % c for c in cats)
+                    parts.append("%sIf (feature %d in %s)" % (pad, f, s)); rec(nid * 2, depth + 1)
+                    parts.append("%sElse (feature %d not in %s)" % (pad, f, s)); rec(nid * 2 + 1, depth + 1)
+            rec(1, 0)
+        return "\n".join(parts) + "\n"
+
+    def __repr__(self):
+        return "GBTClassificationModel with %d trees" % self._gbt.T
