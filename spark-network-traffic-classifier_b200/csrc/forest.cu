@@ -150,7 +150,7 @@ __global__ void __launch_bounds__(kScoreThreads) score_level_kernel(
     const int tid = threadIdx.x, w = warp_id(), lane = lane_id(), nw = kScoreThreads / 32;
     const int nbC = n_bins * C;
     // layout: tot[C] | bestL[C] | per-warp {cen[n_bins] f64, raw[nbC] u32} (8-byte multiples) | cum[batch][nbC] | order[batch][n_bins]
-    //         | cand[batch][n_bins] u8
+    //         | cand[batch][n_bins] u8 (continuous and ordered features; an unordered feature's candidates are all its subsets)
     uint32_t* tot = (uint32_t*)sm_raw;
     uint32_t* bestL = tot + C;
     const size_t per_warp = ((size_t)n_bins * 8 + (size_t)nbC * 4 + 7) & ~(size_t)7;
@@ -226,19 +226,26 @@ __global__ void __launch_bounds__(kScoreThreads) score_level_kernel(
                     tot[k] = a;
                 }
             }
-            uint8_t* cand = cand_all + (size_t)jj * n_bins;
-            const int ns = kind == 2 ? (1 << (nb - 1)) - 1 : nb - 1;
+            // the candidate row holds at most nb - 1 <= n_bins - 1 splits of a continuous / ordered feature.  An unordered
+            // feature keeps all of its 2^(nb-1) - 1 subsets, which can outnumber n_bins (nb = 5 categories, n_bins = 5): its
+            // list is implicitly 0, 1, ..., ns - 1 and is never written to the row
             int n_cand = 0;
-            for (int sp0 = 0; sp0 < ns; sp0 += 32) {
-                const int sp = sp0 + lane;
-                bool keep = sp < ns;
-                if (keep && kind != 2 && sp > 0) {
-                    keep = false;
-                    for (int k = 0; k < C; ++k) keep |= cum[sp * C + k] != cum[(sp - 1) * C + k];
+            if (kind == 2) {
+                n_cand = (1 << (nb - 1)) - 1;
+            } else {
+                uint8_t* cand = cand_all + (size_t)jj * n_bins;
+                const int ns = nb - 1;
+                for (int sp0 = 0; sp0 < ns; sp0 += 32) {
+                    const int sp = sp0 + lane;
+                    bool keep = sp < ns;
+                    if (keep && sp > 0) {
+                        keep = false;
+                        for (int k = 0; k < C; ++k) keep |= cum[sp * C + k] != cum[(sp - 1) * C + k];
+                    }
+                    const uint32_t mk = __ballot_sync(0xffffffffu, keep);
+                    if (keep) cand[n_cand + __popc(mk & ((1u << lane) - 1u))] = (uint8_t)sp;
+                    n_cand += __popc(mk);
                 }
-                const uint32_t mk = __ballot_sync(0xffffffffu, keep);
-                if (keep) cand[n_cand + __popc(mk & ((1u << lane) - 1u))] = (uint8_t)sp;
-                n_cand += __popc(mk);
             }
             if (lane == 0) sh_ncand[jj] = n_cand;
         }
@@ -255,7 +262,7 @@ __global__ void __launch_bounds__(kScoreThreads) score_level_kernel(
         for (int it = tid; it < n_items; it += kScoreThreads) {
             int jj = 0, o = 0;
             while (it >= o + sh_ncand[jj]) { o += sh_ncand[jj]; ++jj; }
-            const int sp = cand_all[(size_t)jj * n_bins + (it - o)];
+            const int sp = sh_kind[jj] == 2 ? it - o : cand_all[(size_t)jj * n_bins + (it - o)];
             const uint32_t* cum = cum_all + (size_t)jj * nbC;
             double g;
             if (sh_kind[jj] != 2) {
