@@ -469,6 +469,12 @@ int b200flow_mlp_forward(const void* x, int32_t x_dtype, int64_t n_rows, int64_t
 int b200flow_gbt_hist_level(const uint8_t* tp, int32_t tp_stride, const void* ent, const int64_t* rq, int32_t n_slots,
                             const int64_t* seg_begin, const int64_t* seg_end, const int64_t* chunk_off, int64_t n_chunks,
                             int32_t chunk_rows, const uint16_t* subset, int32_t m, int32_t n_bins, int64_t* hist, void* stream);
+/* OneVsRest(GBTClassifier), DESIGN.md §5f: b200flow_gbt_hist_level over the slots of K classes' trees at once.  rq is
+ * int64 [K][class_rows][2] and slot s reads {q, q2} of its records from block slot_class[s]; tp and the entries are shared. */
+int b200flow_gbt_hist_level_classes(const uint8_t* tp, int32_t tp_stride, const void* ent, const int64_t* rq, int64_t class_rows,
+                                    const int32_t* slot_class, int32_t n_slots, const int64_t* seg_begin, const int64_t* seg_end,
+                                    const int64_t* chunk_off, int64_t n_chunks, int32_t chunk_rows, const uint16_t* subset,
+                                    int32_t m, int32_t n_bins, int64_t* hist, void* stream);
 /* Variance split scoring, one CTA per slot: split[s] as score_level writes it (categorical features are ordered by centroid
  * sum/count; a child is a leaf at level + 1 == max_depth or when its variance is below 2^-52), and the int64 stats [3] of
  * the node and of both children (zero when there is no split). */
@@ -485,6 +491,12 @@ int b200flow_gbt_leaf_values(int64_t n_nodes, const int64_t* stats, const int32_
 int b200flow_gbt_update(const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows, const b200flow_node* nodes,
                         const uint64_t* node_mask, const double* payload, int32_t tree, int32_t S, int32_t S2, double* margin,
                         int64_t* rq, void* stream);
+/* b200flow_gbt_update for n_classes relabelled problems at once (OneVsRest): margin f64 [K][n_rows], rq int64 [K][n_rows][2];
+ * class k's label is (label byte == k) and its tree of iteration `tree` is rooted at pool node k n_iter + tree.  tree < 0
+ * initialises every class. */
+int b200flow_gbt_update_classes(const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows, int32_t n_classes,
+                                const b200flow_node* nodes, const uint64_t* node_mask, const double* payload, int32_t tree,
+                                int32_t n_iter, int32_t S, int32_t S2, double* margin, int64_t* rq, void* stream);
 /* GBTClassificationModel output from the margins: raw [n][2] = {-F, F}, prob [n][2] = {1 / (1 + exp(2F)), 1 - that},
  * pred = F > 0; raw / prob / pred may be NULL. */
 int b200flow_gbt_output(const double* margin, int64_t n_rows, double* raw, double* prob, double* pred, void* stream);

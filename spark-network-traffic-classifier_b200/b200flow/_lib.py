@@ -81,9 +81,11 @@ _SIGNATURES = {
     "b200flow_mlp_loss_grad": [_P, _I32, _I64, _I64, _P, _P, _I32, _P, _I64, _P, _P],
     "b200flow_mlp_forward": [_P, _I32, _I64, _I64, _P, _I32, _P, _P, _P],
     "b200flow_gbt_hist_level": [_P, _I32, _P, _P, _I32, _P, _P, _P, _I64, _I32, _P, _I32, _I32, _P, _P],
+    "b200flow_gbt_hist_level_classes": [_P, _I32, _P, _P, _I64, _P, _I32, _P, _P, _P, _I64, _I32, _P, _I32, _I32, _P, _P],
     "b200flow_gbt_score_level": [_P, _I32, _P, _I32, _I32, _P, _P, _I32, _I32, _I32, _I32, _I32, _F64, _P, _P, _P, _P, _P],
     "b200flow_gbt_leaf_values": [_I64, _P, _P, _P, _I32, _P, _P],
     "b200flow_gbt_update": [_P, _I32, _I32, _I64, _P, _P, _P, _I32, _I32, _I32, _P, _P, _P],
+    "b200flow_gbt_update_classes": [_P, _I32, _I32, _I64, _I32, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P],
     "b200flow_gbt_output": [_P, _I64, _P, _P, _P, _P],
     "b200flow_random_split": [_U64, _I64, _I64, _P, _I32, _P, _P],
     "b200flow_compact_rows": [_P, _I64, _I32, _P, _I32, _P, _P, _P, _P],

@@ -5,6 +5,9 @@ Host logic only.  findSplits, binning and the de-duplication of the binned rows 
 once per fit); every tree runs the forest's level loop with the variance kernels of csrc/gbt.cu.  Residuals sit on a
 fixed-point grid, so the level histograms are exact int64 sums: with rows sharded over ranks the one all-reduce per level
 is exact and the model is the same bits for any number of ranks.
+
+fit_gbt_ovr trains OneVsRest(GBTClassifier)'s K binary problems (label == k) in one level loop, K trees side by side per
+iteration (DESIGN.md §5f); every class's model is the same bits as fit_gbt on the relabelled rows.
 """
 import math
 from dataclasses import dataclass
@@ -134,7 +137,46 @@ def fit_gbt_records(rec, plan, arity, params, row_offset=0, group=None, round_f3
     return _fit(fr._RecordSource(rec, plan, round_f32), arity, params, row_offset, group)
 
 
-def _fit(src, arity, params, row_offset=0, group=None):
+def fit_gbt_ovr(x, labels, K, arity, params, row_offset=0, group=None):
+    """OneVsRest(GBTClassifier) on a dense CUDA feature matrix: the K problems (labels == k) for k < K, with labels [n] in
+    [0, K), K <= 256, trained together.  -> OvRGBTModel whose models[k] equals fit_gbt(x, labels == k, ...) bit for bit."""
+    return _fit(fr._DenseSource(x, labels), arity, params, row_offset, group, n_classes=K)
+
+
+def fit_gbt_ovr_records(rec, plan, K, arity, params, row_offset=0, group=None, round_f32=False):
+    """the same on raw flow records [n, row_bytes] + the encode plan of their feature vector (plan.label = the label column)"""
+    if plan.label is None:
+        raise ValueError("fit_gbt_ovr_records: the encode plan has no label column (EncodePlan.set_label)")
+    return _fit(fr._RecordSource(rec, plan, round_f32), arity, params, row_offset, group, n_classes=K)
+
+
+class OvRGBTModel:
+    """OneVsRest over K binary GBT models trained together.  models[k] is class k's GBTModel on its own node pool; `forest`
+    is the combined pool (K·T trees, tree k·T + t = class k's tree t) with C = K, whose leaf_prob[node] is one-hot on the class
+    of the node's tree and carries the node's payload.  One b200flow_predict over it gives every class's margin — class k's
+    column adds its own payloads and +0.0 for the other classes' trees, in tree order from +0.0, so it has the bits of
+    models[k].margin — and the first argmax under Spark's `>` rule."""
+
+    def __init__(self, models, forest):
+        self.models, self.forest = list(models), forest
+        self.K, self.T, self.F = len(self.models), self.models[0].T, forest.F
+
+    def predict(self, x):
+        """-> (rawPrediction [n, K] = each class's margin, prediction [n]) on a dense feature matrix."""
+        raw, _, pred = self.forest.predict(x, want_raw=True, want_prob=False)
+        return raw, pred
+
+    def predict_records(self, rec, plan, round_f32=False, on_invalid="ignore"):
+        """the same from raw flow records + the encode plan of the feature vector (fused encode -> bins)"""
+        raw, _, pred, _ = self.forest.predict_records(rec, plan, want_raw=True, want_prob=False, round_f32=round_f32,
+                                                      on_invalid=on_invalid)
+        return raw, pred
+
+
+def _fit(src, arity, params, row_offset=0, group=None, n_classes=None):
+    """the boosting loop.  n_classes None: the binary problem of the label byte.  n_classes = K: the K problems (label == k)
+    side by side — the pool holds K·T trees, class-major (tree k·T + t), margin and rq are [K][U], every iteration's entries
+    are repeated in K segments (one per class root) and one level loop grows all K trees."""
     from . import dist as bdist
     _lib.require_cuda()
     p = params
@@ -146,20 +188,30 @@ def _fit(src, arity, params, row_offset=0, group=None):
         raise ValueError("stepSize must be in (0, 1], got %r" % p.step_size)
     if not (0.0 < p.subsampling_rate <= 1.0):
         raise ValueError("subsamplingRate must be in (0, 1], got %r" % p.subsampling_rate)
+    ovr = n_classes is not None
+    K = int(n_classes) if ovr else 1
+    if not (1 <= K <= 256):
+        raise ValueError("OneVsRest on the GBT trainer needs 1 <= numClasses <= 256 (labels are stored as one byte), got %d" % K)
     dev = src.device
     n, F = src.n, src.F
     T = int(p.max_iter)
     seed = int(p.seed) & 0xFFFFFFFFFFFFFFFF
     strategy = "all" if str(p.feature_subset_strategy) == "auto" else p.feature_subset_strategy
+    # num_classes = 2 only shapes the metadata, so the bins are the binary fit's; de-duplication keys on (bins, label byte), and
+    # with K classes those records refine each relabelled problem's records: the trees see the same integer histogram sums
     rows = fr._TrainingRows(src, 2, arity, p.max_bins, 1, strategy, seed, row_offset, group).read()
     tp, uid, U, m, n_bins = rows.tp, rows.uid, rows.U, rows.m, rows.n_bins
     feat_bins, feat_kind, stride = rows.feat_bins, rows.feat_kind, fr.tp_stride(F)
     S, S2 = grid_shift(rows.n_global)
-    # labels must be 0 or 1 on EVERY rank: the flag is summed over the ranks first, so that all of them raise together
-    bad = (tp[:U, F] > 1).any().reshape(1).to(torch.int64) if U > 0 else torch.zeros(1, dtype=torch.int64, device=dev)
+    # labels must be 0 or 1 (OneVsRest: below K) on EVERY rank: the flag is summed over the ranks first, so that all of them
+    # raise together
+    top = K - 1 if ovr else 1
+    bad = (tp[:U, F] > top).any().reshape(1).to(torch.int64) if U > 0 else torch.zeros(1, dtype=torch.int64, device=dev)
     if group is not None:
         bdist.all_reduce_(bad, group)
     if int(bad.item()):
+        if ovr:
+            raise ValueError("OneVsRest: a label is not in [0, %d)" % K)
         raise ValueError("GBTClassifier currently only supports binary classification: a label is not 0 or 1")
 
     # subsampling weights W[iteration][unique record] (Bernoulli, tree index = iteration); without subsampling every
@@ -173,17 +225,18 @@ def _fit(src, arity, params, row_offset=0, group=None):
              cdf_host.ctypes.data if sub else None, ptr(uid), None, U, ptr(W))
     del uid
 
-    # node pool: roots 0..T-1; a node's stats are 3 int64 = the 6 opaque words grow_level copies per node
-    cap_nodes = max(1024, T * min(1 << (p.max_depth + 1), 64))
+    # node pool: roots 0..K·T-1; a node's stats are 3 int64 = the 6 opaque words grow_level copies per node
+    TK = K * T
+    cap_nodes = max(1024, TK * min(1 << (p.max_depth + 1), 64))
     nodes = torch.zeros((cap_nodes, 16), dtype=torch.uint8, device=dev)
     node_mask = torch.zeros((cap_nodes, 4), dtype=torch.int64, device=dev) if bool((rows.kind > 0).any()) else None
     stats = torch.zeros((cap_nodes, 3), dtype=torch.int64, device=dev)
     node_tree = torch.zeros(cap_nodes, dtype=torch.int32, device=dev)
     node_gain = torch.zeros(cap_nodes, dtype=torch.float64, device=dev)
-    root = np.zeros(T, NODE_DTYPE); root["feat"] = -1; root["left"] = -1; root["nid"] = 1
-    nodes[:T] = _lib.h2d(root.view(np.uint8).reshape(T, 16), dev)
-    node_tree[:T] = torch.arange(T, dtype=torch.int32, device=dev)
-    pool_size = T
+    root = np.zeros(TK, NODE_DTYPE); root["feat"] = -1; root["left"] = -1; root["nid"] = 1
+    nodes[:TK] = _lib.h2d(root.view(np.uint8).reshape(TK, 16), dev)
+    node_tree[:TK] = torch.arange(TK, dtype=torch.int32, device=dev)
+    pool_size = TK
 
     def grow_pool(need):
         nonlocal nodes, node_mask, stats, node_tree, node_gain, cap_nodes
@@ -202,20 +255,26 @@ def _fit(src, arity, params, row_offset=0, group=None):
         cap_nodes = new_cap
 
     weights = [1.0] + [float(p.step_size)] * (T - 1)
-    tree_weight = _lib.h2d(np.asarray(weights, np.float64), dev)
+    tree_weight = _lib.h2d(np.asarray(weights * K, np.float64), dev)
     payload = torch.zeros(cap_nodes, dtype=torch.float64, device=dev)
-    margin = torch.zeros(max(U, 1), dtype=torch.float64, device=dev)
-    rq = torch.zeros((max(U, 1), 2), dtype=torch.int64, device=dev)
-    call("b200flow_gbt_update", ptr(tp), stride, F, U, None, None, None, -1, S, S2, ptr(margin), ptr(rq))
+    margin = torch.zeros(max(K * U, 1), dtype=torch.float64, device=dev)          # [K][U]
+    rq = torch.zeros((max(K * U, 1), 2), dtype=torch.int64, device=dev)           # [K][U][2]: class blocks stay 16-byte aligned
+    if ovr:
+        call("b200flow_gbt_update_classes", ptr(tp), stride, F, U, K, None, None, None, -1, T, S, S2, ptr(margin), ptr(rq))
+    else:
+        call("b200flow_gbt_update", ptr(tp), stride, F, U, None, None, None, -1, S, S2, ptr(margin), ptr(rq))
 
     nb = (U + 1023) // 1024
     blk_cnt = torch.zeros(max(nb, 1), dtype=torch.int32, device=dev)
     blk_off = torch.zeros(nb + 1, dtype=torch.int64, device=dev)
     total = torch.zeros(1, dtype=torch.int64, device=dev)
-    ent = torch.empty((max(U, 1), 2), dtype=torch.int32, device=dev)
+    ent = torch.empty((max(K * U, 1), 2), dtype=torch.int32, device=dev)        # class k's segment starts at k·U
     ent2 = torch.empty_like(ent)
     CH = fr.CHUNK_ROWS
     stats_t = dict(levels=0, slots=0, rows=n, unique_rows=U, S=S)
+    if ovr:
+        cls_base = torch.arange(K, dtype=torch.int64, device=dev) * U
+        cls_root = torch.arange(K, dtype=torch.int32, device=dev) * T
 
     def chunk_table(lens):
         """(device chunk offsets, their host copy) of the slots' entry ranges"""
@@ -236,19 +295,31 @@ def _fit(src, arity, params, row_offset=0, group=None):
         call("b200flow_exclusive_scan_i32_to_i64", ptr(blk_cnt), nb, ptr(blk_off), ptr(total))
         if U > 0:
             call("b200flow_bag_fill", ptr(Wt), 1, U, ptr(blk_off), ptr(ent))
-        seg_begin = torch.zeros(1, dtype=torch.int64, device=dev)
-        seg_end = total.clone()
-        slot_tree = torch.full((1,), t, dtype=torch.int32, device=dev)
-        slot_nid = torch.ones(1, dtype=torch.int32, device=dev)
-        slot_node = torch.full((1,), t, dtype=torch.int32, device=dev)
+        if ovr:             # the same entries for every class: one segment per class root k·T + t
+            if K > 1 and U > 0:
+                ent[:K * U].view(K, U, 2)[1:] = ent[:U]
+            seg_begin = cls_base.clone()
+            seg_end = cls_base + total
+            slot_tree = cls_root + t
+            slot_nid = torch.ones(K, dtype=torch.int32, device=dev)
+            slot_node = slot_tree.clone()
+        else:
+            seg_begin = torch.zeros(1, dtype=torch.int64, device=dev)
+            seg_end = total.clone()
+            slot_tree = torch.full((1,), t, dtype=torch.int32, device=dev)
+            slot_nid = torch.ones(1, dtype=torch.int32, device=dev)
+            slot_node = torch.full((1,), t, dtype=torch.int32, device=dev)
         counters[0] = pool_size
-        n_slots, level = 1, 0
+        n_slots, level = K, 0
         while n_slots > 0:
             grow_pool(pool_size + 2 * n_slots)
             if counters.numel() < 8 + 2 * ((n_slots + 255) // 256):
                 counters = torch.cat([counters, torch.zeros(2 * n_slots, dtype=torch.int64, device=dev)])
             subset = torch.empty((n_slots, m), dtype=torch.int16, device=dev)
-            call("b200flow_feature_subsets", seed, n_slots, ptr(slot_tree), ptr(slot_nid), F, m, ptr(subset))
+            # the feature subsets are keyed by the iteration, as in the K separate fits: class k's tree t draws tree t's
+            slot_iter = torch.remainder(slot_tree, T) if ovr else slot_tree
+            call("b200flow_feature_subsets", seed, n_slots, ptr(slot_iter), ptr(slot_nid), F, m, ptr(subset))
+            slot_class = torch.div(slot_tree, T, rounding_mode="floor") if ovr else None
             chunk_off, off_h = chunk_table(seg_end - seg_begin)
             n_chunks = int(off_h[-1])
             split = torch.empty((n_slots, 64), dtype=torch.uint8, device=dev)
@@ -259,8 +330,14 @@ def _fit(src, arity, params, row_offset=0, group=None):
                 gch = int(off_h[g1] - off_h[g0])
                 if gch > 0:
                     coff = (chunk_off[g0:g1 + 1] - chunk_off[g0]).contiguous()
-                    _timed("gbt_hist_level", "b200flow_gbt_hist_level", ptr(tp), stride, ptr(ent), ptr(rq), g1 - g0,
-                           ptr(seg_begin[g0:g1]), ptr(seg_end[g0:g1]), ptr(coff), gch, CH, ptr(subset[g0:g1]), m, n_bins, ptr(hist))
+                    if ovr:
+                        _timed("gbt_hist_level", "b200flow_gbt_hist_level_classes", ptr(tp), stride, ptr(ent), ptr(rq), U,
+                               ptr(slot_class[g0:g1]), g1 - g0, ptr(seg_begin[g0:g1]), ptr(seg_end[g0:g1]), ptr(coff), gch, CH,
+                               ptr(subset[g0:g1]), m, n_bins, ptr(hist))
+                    else:
+                        _timed("gbt_hist_level", "b200flow_gbt_hist_level", ptr(tp), stride, ptr(ent), ptr(rq), g1 - g0,
+                               ptr(seg_begin[g0:g1]), ptr(seg_end[g0:g1]), ptr(coff), gch, CH, ptr(subset[g0:g1]), m, n_bins,
+                               ptr(hist))
                 if group is not None:                   # the one data-path collective: exact int64 sums
                     bdist.all_reduce_(hist, group)
                 _timed("gbt_score_level", "b200flow_gbt_score_level", ptr(hist), g1 - g0, ptr(subset[g0:g1]), m, n_bins,
@@ -299,9 +376,16 @@ def _fit(src, arity, params, row_offset=0, group=None):
         if payload.shape[0] < cap_nodes:
             payload = torch.zeros(cap_nodes, dtype=torch.float64, device=dev)
         call("b200flow_gbt_leaf_values", pool_size, ptr(stats), ptr(node_tree), ptr(tree_weight), S, ptr(payload))
-        _timed("gbt_update", "b200flow_gbt_update", ptr(tp), stride, F, U, ptr(nodes), ptr(node_mask), ptr(payload), t, S, S2,
-               ptr(margin), ptr(rq))
+        if ovr:
+            _timed("gbt_update", "b200flow_gbt_update_classes", ptr(tp), stride, F, U, K, ptr(nodes), ptr(node_mask), ptr(payload),
+                   t, T, S, S2, ptr(margin), ptr(rq))
+        else:
+            _timed("gbt_update", "b200flow_gbt_update", ptr(tp), stride, F, U, ptr(nodes), ptr(node_mask), ptr(payload), t, S, S2,
+                   ptr(margin), ptr(rq))
 
+    if ovr:
+        return _ovr_model(rows, K, T, weights, S, stats_t, nodes, node_mask, stats, node_tree, node_gain, payload, pool_size,
+                          margin, U)
     forest = fr.ForestModel(T, 1, F, rows.arity, rows.mpb, rows.thresholds, rows.n_thr, nodes, node_mask, None, node_tree,
                             payload[:pool_size].reshape(pool_size, 1).contiguous(), node_gain, pool_size, dt_mode=False)
     model = GBTModel(forest, weights, stats, S)
@@ -309,4 +393,44 @@ def _fit(src, arity, params, row_offset=0, group=None):
     model.train_margin = margin[:U]                      # F of every unique training record (rows: train_margin[train_uid])
     model.train_uid = rows.uid
     model.feat_kind, model.feat_bins, model.n_bins, model.m = rows.kind, feat_bins, n_bins, m
+    return model
+
+
+def _ovr_model(rows, K, T, weights, S, stats_t, nodes, node_mask, stats, node_tree, node_gain, payload, pool_size, margin, U):
+    """the K·T-tree pool -> OvRGBTModel: each class's nodes compacted into their own pool (pool order kept, so its roots
+    k·T..k·T+T-1 become 0..T-1 and sibling pairs stay adjacent; left indices remapped), and the combined C = K forest."""
+    dev = nodes.device
+    F = rows.F
+    n = pool_size
+    tree = node_tree[:n]
+    cls = torch.div(tree, T, rounding_mode="floor").long()
+    sels = [torch.nonzero(cls == k).view(-1) for k in range(K)]
+    rank = torch.empty(n, dtype=torch.int64, device=dev)         # every node's index within its class, in pool order
+    for sel in sels:
+        rank[sel] = torch.arange(sel.numel(), dtype=torch.int64, device=dev)
+    nd32 = nodes[:n].view(torch.int32).view(n, 4)
+    left = nd32[:, 2].long()
+    new_left = torch.where(left >= 0, rank[left.clamp(min=0)], left).to(torch.int32)
+    models = []
+    for k, sel in enumerate(sels):
+        nk = sel.numel()
+        nk32 = nd32[sel].clone()
+        nk32[:, 2] = new_left[sel]
+        nodes_k = nk32.contiguous().view(torch.uint8).view(nk, 16)
+        mask_k = node_mask[sel].contiguous() if node_mask is not None else None
+        tree_k = (tree[sel] - k * T).contiguous()
+        forest_k = fr.ForestModel(T, 1, F, rows.arity, rows.mpb, rows.thresholds, rows.n_thr, nodes_k, mask_k, None, tree_k,
+                                  payload[sel].reshape(nk, 1).contiguous(), node_gain[sel].contiguous(), nk, dt_mode=False)
+        mk = GBTModel(forest_k, weights, stats[sel].contiguous(), S)
+        mk.train_margin = margin[k * U:(k + 1) * U]
+        mk.train_uid = rows.uid
+        mk.feat_kind, mk.feat_bins, mk.n_bins, mk.m = rows.kind, rows.feat_bins, rows.n_bins, rows.m
+        models.append(mk)
+    leaf = torch.zeros((max(n, 1), K), dtype=torch.float64, device=dev)
+    if n > 0:
+        leaf[torch.arange(n, device=dev), cls] = payload[:n]
+    forest = fr.ForestModel(K * T, K, F, rows.arity, rows.mpb, rows.thresholds, rows.n_thr, nodes, node_mask, None, node_tree,
+                            leaf, node_gain, n, dt_mode=False)
+    model = OvRGBTModel(models, forest)
+    model.train_stats = stats_t
     return model

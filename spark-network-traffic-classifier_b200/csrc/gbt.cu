@@ -6,7 +6,8 @@
 // the all-reduce over ranks, the shared- and global-memory atomics and the order of the entries cannot change a bit.
 // The tree structure reuses the forest's: b200flow_split records, b200flow_partition_level, b200flow_next_segments,
 // b200flow_grow_level (the three int64 stats travel as 6 opaque words per node) and b200flow_predict (C = 1 over the
-// payloads).  Compiled with -fmad=false: every fp64 expression below is restated operation for operation by the test oracle.
+// payloads).  OneVsRest(GBTClassifier) grows the K binary problems' trees side by side (DESIGN.md §5f): the _classes entry
+// points read each slot's residuals from its class's block and update every (class, record) pair.  Compiled with -fmad=false: every fp64 expression below is restated operation for operation by the test oracle.
 #include <float.h>
 
 #include "common.cuh"
@@ -23,14 +24,20 @@ constexpr double kGbtEpsilon = 2.220446049250313e-16; // MLUtils.EPSILON (2^-52)
 // One CTA per chunk of one slot's entries (the chunk table of hist_level).  Each entry's record, q and q2 are gathered once
 // per feature pass, and every subset feature of the pass adds {w, w·q, w·q2} to the slot's shared-memory histogram with
 // 64-bit shared atomics; the histogram is flushed with sparse global REDs.  Wide nodes go in feature passes of m_pass.
+// kClasses (OneVsRest, DESIGN.md §5f): the residuals are rq [K][class_rows] and slot s reads the block of its class
+// slot_class[s]; the records and entries are the ones all classes share.  The binary instantiation ignores both arguments,
+// which come last so that its parameter layout and SASS are those of the kernel before classes existed.
+template <bool kClasses>
 __global__ void __launch_bounds__(kGbtHistThreads, 2) gbt_hist_level_kernel(
     const uint8_t* __restrict__ tp, int stride, const b2f_entry* __restrict__ ent, const longlong2* __restrict__ rq, int n_slots,
     const int64_t* __restrict__ seg_begin, const int64_t* __restrict__ seg_end, const int64_t* __restrict__ chunk_off,
-    int chunk_rows, const uint16_t* __restrict__ subset, int m, int n_bins, int m_pass, unsigned long long* hist) {
+    int chunk_rows, const uint16_t* __restrict__ subset, int m, int n_bins, int m_pass, unsigned long long* hist,
+    const int32_t* __restrict__ slot_class, int64_t class_rows) {
     extern __shared__ unsigned long long sh_h[];        // [m_pass][n_bins][3]
     __shared__ int sh_feat[256];
     const int64_t c = blockIdx.x;
     const int s = find_slot(chunk_off, n_slots, c);
+    if (kClasses) rq += (int64_t)slot_class[s] * class_rows;
     const int64_t b = seg_begin[s] + (c - chunk_off[s]) * chunk_rows;
     const int64_t e = min(seg_end[s], b + chunk_rows);
     const int nb3 = n_bins * 3;
@@ -211,22 +218,19 @@ __device__ __forceinline__ longlong2 gbt_grid(double r, int S, int S2) {
     return make_longlong2(q, __double2ll_rn(rh * rh * pexp_pow2(S2)));
 }
 
-// tree < 0: F = +0.0 and the targets of tree 0 (r = y itself).  tree >= 0: walk tree `tree` (root = pool node `tree`),
+// root < 0: F = +0.0 and the targets of tree 0 (r = y itself).  root >= 0: walk the tree whose root is pool node `root`,
 // F += its payload, then r = -LogLoss.gradient = 4y / (1 + exp(2yF)), y = 2 label - 1.  A NaN margin (only reachable through
 // an empty tree, whose leaf value is 0/0) gives r = 0, so that q stays defined.
-__global__ void gbt_update_kernel(const uint8_t* __restrict__ tp, int stride, int F, int64_t n, const int4* __restrict__ nodes,
-                                  const unsigned long long* __restrict__ node_mask, const double* __restrict__ payload, int tree,
-                                  int S, int S2, double* margin, longlong2* rq) {
-    const int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (u >= n) return;
-    const uint8_t* rec = tp + u * stride;
-    const double y = rec[F] ? 1.0 : -1.0;
-    if (tree < 0) {
-        margin[u] = 0.0;
-        rq[u] = gbt_grid(y, S, S2);
+__device__ __forceinline__ void gbt_update_record(const uint8_t* rec, double y, const int4* __restrict__ nodes,
+                                                  const unsigned long long* __restrict__ node_mask,
+                                                  const double* __restrict__ payload, int root, int S, int S2, double* margin,
+                                                  longlong2* rq) {
+    if (root < 0) {
+        *margin = 0.0;
+        *rq = gbt_grid(y, S, S2);
         return;
     }
-    int idx = tree;
+    int idx = root;
     int4 nd = __ldg(nodes + idx);
     while (nd.x >= 0) {
         const int bin = rec[nd.x];
@@ -234,11 +238,34 @@ __global__ void gbt_update_kernel(const uint8_t* __restrict__ tp, int stride, in
         idx = nd.z + right;
         nd = __ldg(nodes + idx);
     }
-    const double Fm = margin[u] + payload[idx];
-    margin[u] = Fm;
+    const double Fm = *margin + payload[idx];
+    *margin = Fm;
     double r = 4.0 * y / (1.0 + portable_exp(2.0 * y * Fm));
     if (r != r) r = 0.0;
-    rq[u] = gbt_grid(r, S, S2);
+    *rq = gbt_grid(r, S, S2);
+}
+
+__global__ void gbt_update_kernel(const uint8_t* __restrict__ tp, int stride, int F, int64_t n, const int4* __restrict__ nodes,
+                                  const unsigned long long* __restrict__ node_mask, const double* __restrict__ payload, int tree,
+                                  int S, int S2, double* margin, longlong2* rq) {
+    const int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (u >= n) return;
+    const uint8_t* rec = tp + u * stride;
+    gbt_update_record(rec, rec[F] ? 1.0 : -1.0, nodes, node_mask, payload, tree, S, S2, margin + u, rq + u);
+}
+
+// OneVsRest: thread i = (class k, record u), k = i / n.  Class k's tree of iteration `tree` is pool node k T + tree, its
+// label is (label == k), and margin / rq are [K][n]: the operations of gbt_update_kernel on the relabelled record.
+__global__ void gbt_update_classes_kernel(const uint8_t* __restrict__ tp, int stride, int F, int64_t n, int K,
+                                          const int4* __restrict__ nodes, const unsigned long long* __restrict__ node_mask,
+                                          const double* __restrict__ payload, int tree, int T, int S, int S2, double* margin,
+                                          longlong2* rq) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n * K) return;
+    const int k = (int)(i / n);
+    const uint8_t* rec = tp + (i - (int64_t)k * n) * stride;
+    gbt_update_record(rec, rec[F] == k ? 1.0 : -1.0, nodes, node_mask, payload, tree < 0 ? -1 : k * T + tree, S, S2, margin + i,
+                      rq + i);
 }
 
 // GBTClassificationModel output: raw = [-F, F], probability[0] = 1 / (1 + exp(-2 raw[0])), probability[1] = 1 - that,
@@ -259,25 +286,44 @@ static GbtScale gbt_scale(int S, int S2) { GbtScale sc; sc.s1 = ldexp(1.0, -S); 
 
 using namespace b200flow;
 
-extern "C" int b200flow_gbt_hist_level(const uint8_t* tp, int32_t tp_stride, const void* ent, const int64_t* rq, int32_t n_slots,
-                                       const int64_t* seg_begin, const int64_t* seg_end, const int64_t* chunk_off, int64_t n_chunks,
-                                       int32_t chunk_rows, const uint16_t* subset, int32_t m, int32_t n_bins, int64_t* hist,
-                                       void* stream) {
-    B2F_REQUIRE(tp && ent && rq && seg_begin && seg_end && chunk_off && subset && hist, "gbt_hist_level: null pointer");
-    B2F_REQUIRE(m > 0 && m <= 256 && n_bins > 0 && n_bins <= 256 && chunk_rows > 0, "gbt_hist_level: bad shape");
-    B2F_REQUIRE(((uintptr_t)rq & 15) == 0, "gbt_hist_level: rq must be 16-byte aligned");
+template <bool kClasses>
+static int gbt_hist_level_launch(const char* name, const uint8_t* tp, int32_t tp_stride, const void* ent, const int64_t* rq,
+                                 const int32_t* slot_class, int64_t class_rows, int32_t n_slots, const int64_t* seg_begin,
+                                 const int64_t* seg_end, const int64_t* chunk_off, int64_t n_chunks, int32_t chunk_rows,
+                                 const uint16_t* subset, int32_t m, int32_t n_bins, int64_t* hist, void* stream) {
+    B2F_REQUIRE(tp && ent && rq && seg_begin && seg_end && chunk_off && subset && hist, "%s: null pointer", name);
+    B2F_REQUIRE(m > 0 && m <= 256 && n_bins > 0 && n_bins <= 256 && chunk_rows > 0, "%s: bad shape", name);
+    B2F_REQUIRE(((uintptr_t)rq & 15) == 0, "%s: rq must be 16-byte aligned", name);
     const size_t per_feat = (size_t)n_bins * 24;
     int m_pass = (int)(kGbtHistSmem / per_feat);
     if (m_pass > m) m_pass = m;
     const size_t smem = per_feat * m_pass;
     if (n_slots <= 0 || n_chunks <= 0) return B200FLOW_OK;
-    B2F_REQUIRE(n_chunks < ((int64_t)1 << 31), "gbt_hist_level: too many chunks");
-    cudaError_t e = cudaFuncSetAttribute(gbt_hist_level_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) { (void)cudaGetLastError(); set_error("gbt_hist_level: %s", cudaGetErrorString(e)); return B200FLOW_ERR_CUDA; }
-    gbt_hist_level_kernel<<<(unsigned)n_chunks, kGbtHistThreads, smem, (cudaStream_t)stream>>>(
+    B2F_REQUIRE(n_chunks < ((int64_t)1 << 31), "%s: too many chunks", name);
+    cudaError_t e = cudaFuncSetAttribute(gbt_hist_level_kernel<kClasses>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { (void)cudaGetLastError(); set_error("%s: %s", name, cudaGetErrorString(e)); return B200FLOW_ERR_CUDA; }
+    gbt_hist_level_kernel<kClasses><<<(unsigned)n_chunks, kGbtHistThreads, smem, (cudaStream_t)stream>>>(
         tp, tp_stride, (const b2f_entry*)ent, (const longlong2*)rq, n_slots, seg_begin, seg_end, chunk_off, chunk_rows, subset, m,
-        n_bins, m_pass, (unsigned long long*)hist);
-    return check_launch("gbt_hist_level");
+        n_bins, m_pass, (unsigned long long*)hist, slot_class, class_rows);
+    return check_launch(name);
+}
+
+extern "C" int b200flow_gbt_hist_level(const uint8_t* tp, int32_t tp_stride, const void* ent, const int64_t* rq, int32_t n_slots,
+                                       const int64_t* seg_begin, const int64_t* seg_end, const int64_t* chunk_off, int64_t n_chunks,
+                                       int32_t chunk_rows, const uint16_t* subset, int32_t m, int32_t n_bins, int64_t* hist,
+                                       void* stream) {
+    return gbt_hist_level_launch<false>("gbt_hist_level", tp, tp_stride, ent, rq, nullptr, 0, n_slots, seg_begin, seg_end,
+                                        chunk_off, n_chunks, chunk_rows, subset, m, n_bins, hist, stream);
+}
+
+extern "C" int b200flow_gbt_hist_level_classes(const uint8_t* tp, int32_t tp_stride, const void* ent, const int64_t* rq,
+                                               int64_t class_rows, const int32_t* slot_class, int32_t n_slots,
+                                               const int64_t* seg_begin, const int64_t* seg_end, const int64_t* chunk_off,
+                                               int64_t n_chunks, int32_t chunk_rows, const uint16_t* subset, int32_t m,
+                                               int32_t n_bins, int64_t* hist, void* stream) {
+    B2F_REQUIRE(slot_class && class_rows >= 0, "gbt_hist_level_classes: bad class table");
+    return gbt_hist_level_launch<true>("gbt_hist_level_classes", tp, tp_stride, ent, rq, slot_class, class_rows, n_slots,
+                                       seg_begin, seg_end, chunk_off, n_chunks, chunk_rows, subset, m, n_bins, hist, stream);
 }
 
 extern "C" int b200flow_gbt_score_level(const int64_t* hist, int32_t n_slots, const uint16_t* subset, int32_t m, int32_t n_bins,
@@ -314,6 +360,21 @@ extern "C" int b200flow_gbt_update(const uint8_t* tp, int32_t tp_stride, int32_t
     gbt_update_kernel<<<(unsigned)((n_rows + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
         tp, tp_stride, F, n_rows, (const int4*)nodes, (const unsigned long long*)node_mask, payload, tree, S, S2, margin, (longlong2*)rq);
     return check_launch("gbt_update");
+}
+
+extern "C" int b200flow_gbt_update_classes(const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows, int32_t n_classes,
+                                           const b200flow_node* nodes, const uint64_t* node_mask, const double* payload,
+                                           int32_t tree, int32_t n_iter, int32_t S, int32_t S2, double* margin, int64_t* rq,
+                                           void* stream) {
+    B2F_REQUIRE(tp && margin && rq && (tree < 0 || (nodes && payload)), "gbt_update_classes: null pointer");
+    B2F_REQUIRE(n_classes >= 1 && n_classes <= 256 && (tree < 0 || tree < n_iter), "gbt_update_classes: bad shape");
+    B2F_REQUIRE(((uintptr_t)rq & 15) == 0, "gbt_update_classes: rq must be 16-byte aligned");
+    if (n_rows <= 0) return B200FLOW_OK;
+    const int64_t total = n_rows * n_classes;
+    gbt_update_classes_kernel<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        tp, tp_stride, F, n_rows, n_classes, (const int4*)nodes, (const unsigned long long*)node_mask, payload, tree, n_iter, S, S2,
+        margin, (longlong2*)rq);
+    return check_launch("gbt_update_classes");
 }
 
 extern "C" int b200flow_gbt_output(const double* margin, int64_t n_rows, double* raw, double* prob, double* pred, void* stream) {

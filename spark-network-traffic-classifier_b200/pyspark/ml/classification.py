@@ -6,6 +6,8 @@ GBTClassifier (binary) runs on the variance-histogram level loop of csrc/gbt.cu 
 model is the same bits for any number of ranks.
 MultilayerPerceptronClassifier runs on the fused fp64 tensor-core loss/gradient and forward kernels (b200flow/mlp.py,
 csrc/mlp.cu, DESIGN.md §5d); its model is the same bits for any number of ranks.
+OneVsRest reduces a K-class problem to K binary ones; OneVsRest(GBTClassifier) trains the K boosted models together in one
+level loop on the device (b200flow.gbt.fit_gbt_ovr, DESIGN.md §5f), each the same bits as its standalone fit.
 LogisticRegression and NaiveBayes (kdd99.py:57,67; cicids17.py:61,71) are OUT of the kernel scope (SURVEY.md
 §8f rank 4): torch fp64 implementations of MLlib's statistics / objective (b200flow/linear.py), checked against a numpy
 restatement and scikit-learn in tests/test_linear_models.py.
@@ -20,7 +22,8 @@ from b200flow import forest as fr
 from b200flow import linear as _linear
 from b200flow import mlp as _mlp
 
-from . import Estimator, Model
+from . import Estimator, Model, Pipeline
+from .param import Param
 from ..sql import ColumnData
 from .feature import IllegalArgumentException, _materialize
 
@@ -640,3 +643,209 @@ class GBTClassificationModel(Model, _GBTParams):
 
     def __repr__(self):
         return "GBTClassificationModel with %d trees" % self._gbt.T
+
+
+# ------------------------------------------------------------------------------- one-vs-rest
+def _first_argmax(raw):
+    """Spark's Vector.argmax per row of raw [n, K]: start at index 0 and move only on a strict `>`.  So a tie keeps the first
+    index, -0.0 does not beat +0.0, and a NaN is never chosen unless it sits at index 0 (where nothing beats it); torch.argmax
+    treats NaN as the maximum instead."""
+    n, K = raw.shape
+    arg = torch.zeros(n, dtype=torch.float64, device=raw.device)
+    if K == 0:
+        return arg
+    best = raw[:, 0]
+    for k in range(1, K):
+        v = raw[:, k]
+        gt = v > best
+        best = torch.where(gt, v, best)
+        arg = torch.where(gt, torch.full_like(arg, float(k)), arg)
+    return arg
+
+
+def _ovr_num_classes(df, lcol):
+    """MetadataUtils.getNumClasses of the label column, else max label + 1 (over every rank) [recalled]; invalid labels raise
+    as in _features_and_labels."""
+    lab_meta = df._cols[lcol].meta.get("ml_attr", {})
+    if lab_meta.get("type") == "nominal":
+        return len(lab_meta["vals"])
+    y = df._column_tensor(lcol).to(torch.float64)
+    bad = ((y < 0) | (y != torch.floor(y))).any().reshape(1).to(torch.float64)
+    mx = (y.max() if y.numel() else torch.full((), -1.0, dtype=torch.float64, device=y.device)).reshape(1)
+    grp = bdist.group()
+    if grp is not None:
+        import torch.distributed as dist
+        bdist.all_reduce_(bad, grp, op=dist.ReduceOp.MAX)
+        bdist.all_reduce_(mx, grp, op=dist.ReduceOp.MAX)
+    if bool(bad.item()):
+        raise IllegalArgumentException("Classifier was given dataset with invalid label. Labels must be integers in [0, numClasses).")
+    return int(mx.item()) + 1
+
+
+class _OneVsRestParams:
+    _defaults = {"classifier": None, "featuresCol": "features", "labelCol": "label", "predictionCol": "prediction",
+                 "rawPredictionCol": "rawPrediction", "weightCol": None, "parallelism": 1}
+
+
+class OneVsRest(Estimator, _OneVsRestParams):
+    """Spark 3's OneVsRest [recalled]: one binary model per class k, fitted on the label (label == k ? 1.0 : 0.0), which
+    carries two-value nominal metadata; the prediction is the first argmax of the models' rawPrediction[1].  A GBTClassifier
+    with at most 256 classes (the label byte of a binned record) is trained as ONE class-batched boosting run on the device
+    (DESIGN.md §5f), whose K models equal the K separate fits bit for bit; every other classifier, and more classes, take the
+    generic loop.  parallelism is validated but only orders host work, so it does not change the result (DESIGN.md §6)."""
+    GBT_MAX_CLASSES = 256
+
+    def __init__(self, featuresCol=None, labelCol=None, predictionCol=None, rawPredictionCol=None, classifier=None,
+                 weightCol=None, parallelism=None):
+        kw = dict(locals()); kw.pop("self"); kw.pop("__class__", None)
+        super().__init__(**kw)
+
+    def copy(self, extra=None):
+        """as in pyspark, the param map also reaches the classifier (fit(df, {gbt.maxDepth: 3}), ParamGridBuilder grids)."""
+        c = super().copy(extra)
+        staged = {k: v for k, v in (extra or {}).items() if isinstance(k, Param)}
+        if staged and c.getOrDefault("classifier") is not None:
+            c._paramMap["classifier"] = c.getOrDefault("classifier").copy(staged)
+        return c
+
+    def _check(self):
+        g = self.getOrDefault
+        clf = g("classifier")
+        if clf is None:
+            raise IllegalArgumentException("OneVsRest needs the classifier param")
+        if not isinstance(clf, Estimator) or isinstance(clf, (OneVsRest, Pipeline)):
+            raise IllegalArgumentException("OneVsRest classifier must be a classifier Estimator, got %s" % type(clf).__name__)
+        if g("weightCol"):
+            raise IllegalArgumentException("weightCol is not supported by OneVsRest in this shim")
+        par = g("parallelism")
+        if isinstance(par, bool) or int(par) != par or int(par) < 1:
+            raise IllegalArgumentException("parallelism must be an integer >= 1, got %r" % (par,))
+        return clf
+
+    def _binary_copy(self, clf, label_col):
+        """the classifier as OneVsRest fits it for one class: its labelCol the relabelled column, its featuresCol and
+        predictionCol the OneVsRest's [recalled]"""
+        g = self.getOrDefault
+        return clf.copy({"labelCol": label_col, "featuresCol": g("featuresCol"), "predictionCol": g("predictionCol")})
+
+    def _fit(self, df):
+        clf = self._check()
+        fcol, lcol = self.getOrDefault("featuresCol"), self.getOrDefault("labelCol")
+        for c in (fcol, lcol):
+            if c not in df._cols:
+                raise IllegalArgumentException("Field \"%s\" does not exist." % c)
+        if df._cols[fcol].kind != "vector":
+            raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+        K = _ovr_num_classes(df, lcol)
+        if K < 1:
+            raise IllegalArgumentException("OneVsRest needs at least one class, the label column has none")
+        tmp = _ovr_temp_name(df, "ovr_binary_label")
+        if type(clf) is GBTClassifier and K <= self.GBT_MAX_CLASSES:
+            models, joint = self._fit_gbt(clf, df, K, tmp)
+        else:
+            models, joint = self._fit_generic(clf, df, K, tmp), None
+        m = OneVsRestModel(models, joint)
+        m._paramMap = {k: v for k, v in self._paramMap.items() if k in m._all_defaults()}
+        return m
+
+    def _fit_generic(self, clf, df, K, tmp):
+        """K fits of the classifier, one per relabelled frame"""
+        y = df._column_tensor(self.getOrDefault("labelCol"))
+        out = []
+        for k in range(K):
+            cols = dict(df._cols)
+            cols[tmp] = ColumnData("numeric", (y == k).to(torch.float64), "f64", _BINARY_LABEL_META)
+            out.append(self._binary_copy(clf, tmp).fit(df._with(cols=cols)))
+        return out
+
+    def _fit_gbt(self, clf, df, K, tmp):
+        """the class-batched device trainer -> (K GBTClassificationModels, the joint model)"""
+        from b200flow import gbt as _gbt
+        from .feature import SparkException
+        binary = self._binary_copy(clf, tmp)
+        p = binary._params()
+        fcol, lcol = self.getOrDefault("featuresCol"), self.getOrDefault("labelCol")
+        fused = _records_fit_inputs(df, clf.copy({"featuresCol": fcol, "labelCol": lcol}))
+        try:
+            grp = bdist.group()
+            if fused is not None:                           # lazy VectorAssembler output: bin straight from the raw records
+                rec, plan, _, attrs = fused
+                off, _ = bdist.global_offset(rec.shape[0], rec.device, grp)
+                joint = _gbt.fit_gbt_ovr_records(rec, plan, K, _arity_from_attrs(attrs, plan.n_out), p, row_offset=off, group=grp)
+            else:
+                fc = df._cols[fcol]
+                x, y = fc.data, df._column_tensor(lcol)
+                off, _ = bdist.global_offset(x.shape[0], x.device, grp)
+                joint = _gbt.fit_gbt_ovr(x, y.to(torch.int32), K, _arity_from_attrs(fc.meta.get("attrs"), x.shape[1]), p,
+                                         row_offset=off, group=grp)
+        except fr.InvalidRowsError as e:
+            raise SparkException("Encountered NaN/null while assembling a row with handleInvalid = \"error\" (%s)" % e)
+        except ValueError as e:        # includes b200flow's UnsupportedParamError; CUDA failures propagate as they are
+            raise IllegalArgumentException(str(e))
+        models = []
+        for sub in joint.models:
+            m = GBTClassificationModel(sub)
+            m._paramMap = {k: v for k, v in binary._paramMap.items() if k in m._all_defaults()}
+            models.append(m)
+        return models, joint
+
+
+_BINARY_LABEL_META = {"ml_attr": {"type": "nominal", "vals": ["0.0", "1.0"]}}
+
+
+def _ovr_temp_name(df, base):
+    name = base
+    while name in df._cols:
+        name = "_" + name
+    return name
+
+
+class OneVsRestModel(Model, _OneVsRestParams):
+    """models[k]: class k's binary model.  rawPrediction = each model's rawPrediction[1], prediction = the first argmax
+    (_first_argmax); no probability column [recalled]."""
+
+    def __init__(self, models, joint=None):
+        super().__init__()
+        self.models = list(models)
+        self._joint = joint                   # b200flow.gbt.OvRGBTModel of a class-batched GBT fit, else None
+
+    @property
+    def numClasses(self):
+        return len(self.models)
+
+    def _transform(self, df):
+        fcol = self.getOrDefault("featuresCol")
+        if fcol not in df._cols or df._cols[fcol].kind != "vector":
+            raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+        rcol, pcol = self.getOrDefault("rawPredictionCol"), self.getOrDefault("predictionCol")
+        for name in (rcol, pcol):
+            if name and name in df._cols:
+                raise IllegalArgumentException("Output column %s already exists." % name)
+        if self._joint is not None:
+            raw, pred = self._joint_predict(df, fcol)
+        else:
+            tmp = _ovr_temp_name(df, "ovr_raw")
+            cols = []
+            for m in self.models:
+                out = m.copy({"rawPredictionCol": tmp, "predictionCol": "", "probabilityCol": ""}).transform(df)
+                cols.append(out._column_tensor(tmp)[:, 1].to(torch.float64))
+            raw = torch.stack(cols, 1) if cols else torch.zeros((df.count(), 0), dtype=torch.float64, device=df._device())
+            pred = _first_argmax(raw)
+        cols = dict(df._cols)
+        if rcol:
+            cols[rcol] = ColumnData("vector", raw, "f64")
+        if pcol:
+            cols[pcol] = ColumnData("numeric", pred, "f64")
+        return df._with(cols=cols)
+
+    def _joint_predict(self, df, fcol):
+        """one tree walk over the K·T trees (b200flow_predict with C = K): the margins and the `>` argmax in one kernel"""
+        j = self._joint
+        plan = _lazy_plan(df, fcol)
+        if plan is not None and plan.n_out == j.F:          # lazy features: fused encode -> bins -> tree walk
+            from .feature import SparkException
+            try:
+                return j.predict_records(df._rec, plan, on_invalid="error" if plan.check_nan else "ignore")
+            except fr.InvalidRowsError as e:
+                raise SparkException("Encountered NaN/null while assembling a row with handleInvalid = \"error\" (%s)" % e)
+        return j.predict(df._cols[fcol].data)
