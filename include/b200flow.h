@@ -458,6 +458,23 @@ int b200flow_mlp_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, int64
 int b200flow_mlp_forward(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, const int32_t* layers, int32_t n_layers,
                          const double* weights, double* raw, void* stream);
 
+/* ------------------------------------------------------------ mixture models ---
+ * GaussianMixture (full covariance), DESIGN.md §5g.  Features x [n_rows][ld] f64, rows [0, n_rows) are global rows
+ * row_offset + i; 1 <= D <= 256, 1 <= k <= 64.  A partial row of chunk b (b counted from the first 4096-row chunk the rows
+ * touch, as for b200flow_group_sums) is [LL, then per component i: W_i, S_i [D], Q_i [D(D+1)/2]], width
+ * 1 + k (1 + D + D(D+1)/2); Q_i is packed upper, (a, b) with a <= b at a + b(b+1)/2.
+ * b200flow_gmm_estep: means [k][D], roots [k][D][D], log_consts [k] = log w_i + u_i.  Per row: q_i = sum over j in order of
+ * y_j^2, y = roots_i (x - means_i); s_i = log_consts_i - 0.5 q_i; t_i = logaddexp(log 2^-52, s_i); resp [n_rows][k] =
+ * exp(t_i - logsumexp(t)); pred [n_rows] = first argmax of resp; partials[b][0] = the sum of logsumexp(t) over the chunk's
+ * rows in row order from +0.0.  resp, pred and partials may each be NULL. */
+int b200flow_gmm_estep(const double* x, int64_t n_rows, int32_t D, int64_t ld, int32_t k, const double* means,
+                       const double* roots, const double* log_consts, int64_t row_offset, double* resp, int32_t* pred,
+                       double* partials, void* stream);
+/* b200flow_gmm_moments: the rest of each partial row from resp [n_rows][k]: W_i = sum r_i, S_i = sum r_i x,
+ * Q_i = sum r_i x x^T over the chunk's rows (fp64 tensor-core contractions in a fixed order; slot 0 is left alone). */
+int b200flow_gmm_moments(const double* x, int64_t n_rows, int32_t D, int64_t ld, int32_t k, const double* resp,
+                         int64_t row_offset, double* partials, void* stream);
+
 /* ------------------------------------------------------- gradient-boosted trees ---
  * GBTClassifier (binary, LogLoss), DESIGN.md §5e.  The regression trees reuse the forest's level loop: feature_subsets,
  * partition_level, next_segments, grow_level (with C = 6: a node's int64 stats {Σw, Σw·q, Σw·q2} travel as six opaque

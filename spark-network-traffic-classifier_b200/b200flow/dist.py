@@ -158,16 +158,19 @@ def chunk_tail(values, ids, sh):
     return t0, tail_v, tail_i
 
 
-def chunk_chain(partials, n_chunks, G, W, sh):
+def chunk_chain(partials, n_chunks, G, W, sh, more=()):
     """totals [G, W] f64: the running totals received from the previous rank (+0.0 on rank 0), plus this rank's
     partials [n_chunks, G, W] added in chunk order (b200flow_group_sums_chain), sent on to the next rank; the last rank's
-    totals are broadcast, so every rank returns the same bits."""
+    totals are broadcast, so every rank returns the same bits.  `more` yields further (partials, n_chunks) batches, the
+    chunks that follow in order; each is added before the next is drawn, so a rank need not hold all its partials at once."""
     totals = torch.zeros((G, W), dtype=torch.float64, device=partials.device)
     rank, grp = sh.rank, sh.grp
     world = len(sh.ns)
     if grp is not None and rank > 0:
         recv_(totals, rank - 1, grp)
     call("b200flow_group_sums_chain", ptr(partials), n_chunks, G, W, ptr(totals))
+    for p, n in more:
+        call("b200flow_group_sums_chain", ptr(p), n, G, W, ptr(totals))
     if grp is not None:
         if rank < world - 1:
             send(totals, rank + 1, grp)
