@@ -475,6 +475,20 @@ int b200flow_gmm_estep(const double* x, int64_t n_rows, int32_t D, int64_t ld, i
 int b200flow_gmm_moments(const double* x, int64_t n_rows, int32_t D, int64_t ld, int32_t k, const double* resp,
                          int64_t row_offset, double* partials, void* stream);
 
+/* ------------------------------------------------------ dimensionality reduction ---
+ * PCA and Pearson correlation, DESIGN.md §5h.  Features x [n_rows][ld] f64, 1 <= D <= 256.
+ * b200flow_centered_gram: rows [0, n_rows) are global rows row_offset + i.  partials [n_chunks][D(D+1)/2] (n_chunks =
+ * b200flow_group_sums_chunks(row_offset, n_rows)): for each 4096-row global chunk the rows touch, the packed upper triangle
+ * of (X - shift)^T (X - shift) over the chunk's present rows, (a, b) with a <= b at a + b(b+1)/2; shift [D] (NULL: zeros) is
+ * subtracted as the rows are staged.  fp64 tensor-core contractions over the rows in row order; a chunk's partial depends
+ * only on which of its rows are present. */
+int b200flow_centered_gram(const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* shift, int64_t row_offset,
+                           double* partials, void* stream);
+/* b200flow_pca_project: out [n_rows][k] = x pc, pc [D][k] row-major, 1 <= k <= 256; out[i][j] accumulates x[i][a] pc[a][j]
+ * over a in ascending order (fp64 tensor cores), so a row's output depends on that row and pc alone, not on its position. */
+int b200flow_pca_project(const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* pc, int32_t k, double* out,
+                         void* stream);
+
 /* ------------------------------------------------------- gradient-boosted trees ---
  * GBTClassifier (binary, LogLoss), DESIGN.md §5e.  The regression trees reuse the forest's level loop: feature_subsets,
  * partition_level, next_segments, grow_level (with C = 6: a node's int64 stats {Σw, Σw·q, Σw·q2} travel as six opaque

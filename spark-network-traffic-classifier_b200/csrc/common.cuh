@@ -168,6 +168,17 @@ __device__ __forceinline__ void st_stream_u4(void* p, uint4 v) {
     asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
 }
 
+// ------------------------------------------------------------------ fp64 tensor-core MMA (mma.sync m8n8k4 f64, SASS DMMA.8x8x4)
+// Fragments (PTX ISA): A holds (row lane>>2, k lane&3), B holds (k lane&3, col lane>>2), C/D hold (row lane>>2,
+// col 2(lane&3) + {0,1}).  c += a b, the four products of a (row, col) rounded once.
+__device__ __forceinline__ void dmma(double (&c)[2], double a, double b) {
+    asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
+        : "+d"(c[0]), "+d"(c[1])
+        : "d"(a), "d"(b));
+}
+// widths are zero-padded to multiples of the 8-wide fragments; the padding is exact zeros and adds nothing to a product
+__host__ __device__ inline int pad8(int v) { return (v + 7) / 8 * 8; }
+
 template <typename T> __device__ __forceinline__ double load_as_double(const void* base, int64_t idx);
 template <> __device__ __forceinline__ double load_as_double<float>(const void* base, int64_t idx) {
     return (double)__ldg((const float*)base + idx);

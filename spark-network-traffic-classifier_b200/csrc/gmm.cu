@@ -41,13 +41,6 @@ constexpr int kGmmSlab = 64;                      // rows of R per shared-memory
 constexpr int kGmmSlots = 32;                     // moment tiles per warp and pass
 constexpr int kGmmMaxD = 256, kGmmMaxK = 64;
 
-__device__ __forceinline__ void dmma(double (&c)[2], double a, double b) {
-    asm("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-        : "+d"(c[0]), "+d"(c[1])
-        : "d"(a), "d"(b));
-}
-
-__host__ __device__ inline int pad8(int v) { return (v + 7) / 8 * 8; }
 // 4 mod 8 doubles: fragment loads take the minimum 2 wavefronts; at least 36, so that 8 rows of a slab hold a warp's
 // [kGmmTile][8] block of y
 __host__ __device__ inline int estep_pitch(int D) { return (pad8(D) > 32 ? pad8(D) : 32) + 4; }

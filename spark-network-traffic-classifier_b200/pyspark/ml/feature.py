@@ -1,6 +1,6 @@
 """pyspark.ml.feature shim: StringIndexer, VectorAssembler (used by the reference scripts: kdd99.py:34-35,45-46;
 cicids17.py:41-46) and OneHotEncoder, StandardScaler (named by the north star) — all executed by the fused
-b200flow encode kernel.  Each output column remembers how it derives from the raw record fields
+b200flow encode kernel — and PCA on the PCA kernels (b200flow/pca.py).  Each output column remembers how it derives from the raw record fields
 (ColumnData.prov), so VectorAssembler / StandardScaler re-run ONE fused kernel over the raw AoS records
 instead of chaining per-stage passes (StringIndexer lookup + one-hot expand + scale + assemble).
 """
@@ -11,11 +11,13 @@ import torch
 
 from b200flow import dist as bdist
 from b200flow import encode as enc
+from b200flow import pca as _pca
 from b200flow._lib import SRC_F32, SRC_INDEX, SRC_ONEHOT, B200FlowError
 from b200flow.encode import EncodePlan, RecordSchema
 
 from . import Estimator, Model, Transformer
 from ..sql import ColumnData, DataFrame
+from .linalg import DenseMatrix, DenseVector
 
 
 class SparkException(Exception):
@@ -386,4 +388,57 @@ class StandardScalerModel(Model):
             plan = None
         cols = dict(df._cols)
         cols[out] = ColumnData("vector", vec, "f64", {"attrs": [{"type": "numeric"}] * D}, ("plan", plan) if plan else None)
+        return df._with(cols=cols)
+
+
+# ----------------------------------------------------------------------------------- PCA
+class PCA(Estimator):
+    """pyspark.ml.feature.PCA on the b200flow PCA kernels (b200flow/pca.py, DESIGN.md §5h).  The model is the same bits for
+    any number of ranks; each principal component's sign is fixed so that its entry of largest magnitude is positive."""
+    _defaults = {"k": None, "inputCol": None, "outputCol": None}
+
+    def __init__(self, k=None, inputCol=None, outputCol=None):
+        super().__init__(k=k, inputCol=inputCol, outputCol=outputCol)
+
+    def _fit(self, df):
+        name = self.getOrDefault("inputCol")
+        if name not in df._cols:
+            raise IllegalArgumentException("Field \"%s\" does not exist." % name)
+        try:
+            fit = _pca.pca_fit(_materialize(df, name), self.getOrDefault("k"), group=bdist.group())
+        except ValueError as e:        # includes b200flow's UnsupportedParamError
+            raise IllegalArgumentException(str(e))
+        m = PCAModel(fit)
+        m._paramMap = dict(self._paramMap)
+        return m
+
+
+class PCAModel(Model):
+    _defaults = dict(PCA._defaults)
+
+    def __init__(self, fit):
+        super().__init__()
+        self._fit_result = fit             # b200flow.pca.PCAFit
+
+    @property
+    def pc(self):
+        p = self._fit_result.pc
+        return DenseMatrix(p.shape[0], p.shape[1], p.T.ravel())
+
+    @property
+    def explainedVariance(self):
+        return DenseVector(self._fit_result.explained_variance.copy())
+
+    def _transform(self, df):
+        name, out = self.getOrDefault("inputCol"), self.getOrDefault("outputCol")
+        if out in df._cols:
+            raise IllegalArgumentException("Output column %s already exists." % out)
+        if name not in df._cols:
+            raise IllegalArgumentException("Field \"%s\" does not exist." % name)
+        try:
+            vec = _pca.pca_transform(_materialize(df, name), self._fit_result)
+        except ValueError as e:
+            raise IllegalArgumentException(str(e))
+        cols = dict(df._cols)
+        cols[out] = ColumnData("vector", vec, "f64", {"attrs": [{"type": "numeric"}] * vec.shape[1]}, None)
         return df._with(cols=cols)

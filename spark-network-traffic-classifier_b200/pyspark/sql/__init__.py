@@ -147,6 +147,10 @@ class LocalFrame:
         names = list(self._pdf.columns)
         return [Row([_py(v) for v in rec], names) for rec in self._pdf.itertuples(index=False, name=None)]
 
+    def head(self, n=None):
+        rows = LocalFrame(self._pdf.head(1 if n is None else n)).collect()
+        return (rows[0] if rows else None) if n is None else rows
+
     @property
     def rdd(self):
         return _RDD(self.collect())
