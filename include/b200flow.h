@@ -489,6 +489,37 @@ int b200flow_centered_gram(const double* x, int64_t n_rows, int32_t D, int64_t l
 int b200flow_pca_project(const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* pc, int32_t k, double* out,
                          void* stream);
 
+/* ------------------------------------------------------------ feature selection ---
+ * Chi-square, ANOVA and F-value tests and the selectors built on them, DESIGN.md §5i.  Values x [n_rows][ld] f64, finite
+ * (the caller checks), 1 <= W <= 256.
+ * b200flow_distinct_values: per column w, the set of value keys in an open-addressed table tables[w][32768] (device, the
+ * caller fills every slot with 0xFFFFFFFFFFFFFFFF, a NaN pattern that is never a key).  A key is the value's bits with -0.0
+ * mapped to +0.0.  counts int32 [W] (caller zeroes) += the keys this call inserted; overflow int32 [W] (caller zeroes) is set
+ * to 1 once counts[w] passes 10000, after which column w takes no more keys.  The table's contents are a set: which slot
+ * holds a key depends on the launch. */
+int b200flow_distinct_values(const double* x, int64_t n_rows, int32_t W, int64_t ld, uint64_t* tables, int32_t* counts,
+                             int32_t* overflow, void* stream);
+/* b200flow_dictionary_ids: ids[i] = the index of values[i * ld] in dict [L] (device, ascending, no duplicates, -0.0 equal to
+ * +0.0 as in any f64 comparison), -1 when it is absent.  1 <= L <= 10000. */
+int b200flow_dictionary_ids(const double* values, int64_t n_rows, int64_t ld, const double* dict, int32_t L, int32_t* ids,
+                            void* stream);
+/* b200flow_contingency_counts: counts int64 [n_values][L] (device, caller zeroes) += the rows with x[i][w] == dicts[v]
+ * and label_ids[i] == l at row v = dict_off[w] + index of the value in dicts[dict_off[w] .. dict_off[w + 1]) (each range
+ * ascending); dict_off int32 [W + 1] (device), n_values = dict_off[W] (host copy) <= 2^26 / L.  Rows whose value is absent
+ * or whose label id is outside [0, L) are not counted.  1 <= L <= 256.  Integer counts: exact for any launch. */
+int b200flow_contingency_counts(const double* x, int64_t n_rows, int32_t W, int64_t ld, const int32_t* label_ids, int32_t L,
+                                const double* dicts, const int32_t* dict_off, int64_t n_values, int64_t* counts, void* stream);
+/* b200flow_group_centered_moments: rows [0, n_rows) are global rows row_offset + i.  For each 4096-row global chunk they
+ * touch (n_chunks = b200flow_group_sums_chunks(row_offset, n_rows)), partials [n_chunks][G][W'] (device):
+ *   y NULL:  W' = W, [c][g][w] = sum over the chunk's rows with ids[i] == g of (x[i][w] - centers[g][w])^2;
+ *   y [n_rows] (then G == 1 and ids is ignored): W' = 2W + 1, [c][0][w] = sum (x[i][w] - centers[w])^2,
+ *            [c][0][W + w] = sum (x[i][w] - centers[w]) (y[i] - y_center), [c][0][2W] = sum (y[i] - y_center)^2.
+ * Each sum runs over the rows in row order from +0.0 without FMA, so a chunk's partial depends only on which of its rows
+ * are present.  ids NULL: every row is in group 0 (G == 1).  centers [G][W] (device).  1 <= G <= 256. */
+int b200flow_group_centered_moments(const double* x, int64_t n_rows, int32_t W, int64_t ld, const int32_t* ids, int32_t G,
+                                    const double* centers, const double* y, double y_center, int64_t row_offset,
+                                    double* partials, void* stream);
+
 /* ------------------------------------------------------- gradient-boosted trees ---
  * GBTClassifier (binary, LogLoss), DESIGN.md §5e.  The regression trees reuse the forest's level loop: feature_subsets,
  * partition_level, next_segments, grow_level (with C = 6: a node's int64 stats {Σw, Σw·q, Σw·q2} travel as six opaque

@@ -84,6 +84,10 @@ _SIGNATURES = {
     "b200flow_gmm_moments": [_P, _I64, _I32, _I64, _I32, _P, _I64, _P, _P],
     "b200flow_centered_gram": [_P, _I64, _I32, _I64, _P, _I64, _P, _P],
     "b200flow_pca_project": [_P, _I64, _I32, _I64, _P, _I32, _P, _P],
+    "b200flow_distinct_values": [_P, _I64, _I32, _I64, _P, _P, _P, _P],
+    "b200flow_dictionary_ids": [_P, _I64, _I64, _P, _I32, _P, _P],
+    "b200flow_contingency_counts": [_P, _I64, _I32, _I64, _P, _I32, _P, _P, _I64, _P, _P],
+    "b200flow_group_centered_moments": [_P, _I64, _I32, _I64, _P, _I32, _P, _P, _F64, _I64, _P, _P],
     "b200flow_gbt_hist_level": [_P, _I32, _P, _P, _I32, _P, _P, _P, _I64, _I32, _P, _I32, _I32, _P, _P],
     "b200flow_gbt_hist_level_classes": [_P, _I32, _P, _P, _I64, _P, _I32, _P, _P, _P, _I64, _I32, _P, _I32, _I32, _P, _P],
     "b200flow_gbt_score_level": [_P, _I32, _P, _I32, _I32, _P, _P, _I32, _I32, _I32, _I32, _I32, _F64, _P, _P, _P, _P, _P],

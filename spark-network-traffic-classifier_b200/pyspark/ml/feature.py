@@ -1,6 +1,7 @@
 """pyspark.ml.feature shim: StringIndexer, VectorAssembler (used by the reference scripts: kdd99.py:34-35,45-46;
 cicids17.py:41-46) and OneHotEncoder, StandardScaler (named by the north star) — all executed by the fused
-b200flow encode kernel — and PCA on the PCA kernels (b200flow/pca.py).  Each output column remembers how it derives from the raw record fields
+b200flow encode kernel — PCA on the PCA kernels (b200flow/pca.py), and the feature selectors (UnivariateFeatureSelector,
+ChiSqSelector, VarianceThresholdSelector) on the selection kernels (b200flow/selection.py).  Each output column remembers how it derives from the raw record fields
 (ColumnData.prov), so VectorAssembler / StandardScaler re-run ONE fused kernel over the raw AoS records
 instead of chaining per-stage passes (StringIndexer lookup + one-hot expand + scale + assemble).
 """
@@ -12,6 +13,7 @@ import torch
 from b200flow import dist as bdist
 from b200flow import encode as enc
 from b200flow import pca as _pca
+from b200flow import selection as _sel
 from b200flow._lib import SRC_F32, SRC_INDEX, SRC_ONEHOT, B200FlowError
 from b200flow.encode import EncodePlan, RecordSchema
 
@@ -45,6 +47,16 @@ def _materialize(df, name):
         return df._field_values(name).to(torch.float64).reshape(-1, 1).contiguous()
     d = c.data
     return (d.reshape(d.shape[0], -1) if d.dim() == 1 else d).to(torch.float64).contiguous()
+
+
+def _peek(df, name):
+    """like _materialize, but a lazy column's values are computed without being kept: the column stays lazy, so a tree
+    trainer downstream still bins straight from the raw records."""
+    c = df._cols[name]
+    if c.kind != "field" and c.lazy and c._maker is not None and df._rec is not None:
+        d = c._maker(df._rec)
+        return (d.reshape(d.shape[0], -1) if d.dim() == 1 else d).to(torch.float64).contiguous()
+    return _materialize(df, name)
 
 
 def _prefetch_category_counts(df, col):
@@ -442,3 +454,170 @@ class PCAModel(Model):
         cols = dict(df._cols)
         cols[out] = ColumnData("vector", vec, "f64", {"attrs": [{"type": "numeric"}] * vec.shape[1]}, None)
         return df._with(cols=cols)
+
+
+# ----------------------------------------------------------------------------------- feature selection
+_SELECTION_MODES = ("numTopFeatures", "percentile", "fpr", "fdr", "fwe")
+_DEFAULT_THRESHOLD = {"numTopFeatures": 50, "percentile": 0.1, "fpr": 0.05, "fdr": 0.05, "fwe": 0.05}
+
+
+def _check_selection(mode, threshold):
+    if mode not in _SELECTION_MODES:
+        raise IllegalArgumentException("selectionMode must be one of %s, got %r" % (list(_SELECTION_MODES), mode))
+    if mode == "numTopFeatures":
+        if not threshold >= 1:
+            raise IllegalArgumentException("numTopFeatures must be >= 1, got %r" % (threshold,))
+    elif not 0.0 <= threshold <= 1.0:
+        raise IllegalArgumentException("%s must be in [0, 1], got %r" % (mode, threshold))
+    return float(threshold)
+
+
+def _select_column(df, name, out, sel):
+    """df with column `out` = the slots `sel` (ascending) of the vector column `name`, keeping their per-slot attrs.  A
+    column with raw-record provenance stays a plan over the selected slots (lazy when the input is lazy), so a tree trainer
+    downstream still bins straight from the records; otherwise the encode kernel gathers the slots from the dense vector."""
+    if name not in df._cols:
+        raise IllegalArgumentException("Field \"%s\" does not exist." % name)
+    if out in df._cols:
+        raise IllegalArgumentException("Output column %s already exists." % out)
+    c = df._cols[name]
+    if c.kind != "vector":
+        raise IllegalArgumentException("Column %s must be of type vector" % name)
+    attrs_in = c.meta.get("attrs")
+    plan_in = c.prov[1] if c.prov is not None and c.prov[0] == "plan" and df._rec is not None else None
+    x = None if plan_in is not None else _materialize(df, name)         # the only read of a dense input
+    D = plan_in.n_out if plan_in is not None else x.shape[1]
+    if sel and sel[-1] >= D:
+        raise IllegalArgumentException("vector size %d does not hold the selected feature %d" % (D, sel[-1]))
+    attrs = [attrs_in[i] for i in sel] if attrs_in and len(attrs_in) == D else [{"type": "numeric"}] * len(sel)
+    cols = dict(df._cols)
+    if not sel:
+        cols[out] = ColumnData("vector", torch.empty((df._n, 0), dtype=torch.float64, device=df._device()), "f64",
+                               {"attrs": []}, None)
+    elif plan_in is not None:
+        plan = copy.copy(plan_in); plan.slots = [plan_in.slots[i] for i in sel]; plan.luts = list(plan_in.luts)
+        plan._dev = None
+        plan.label = None
+        vdtype = torch.float32 if c.dtype == "f32" else torch.float64
+        if c.lazy:
+            def mk(r, plan=plan, vdtype=vdtype):
+                feats, _, valid = plan.run(r, vdtype, want_valid=bool(plan.check_nan))
+                if plan.check_nan and r.shape[0] and int((valid == 0).sum().item()):
+                    raise SparkException("Encountered NaN/null while assembling a row with handleInvalid = \"error\". Consider "
+                                         "removing NaNs from dataset or using handleInvalid = \"keep\" or \"skip\".")
+                return feats
+            rec0 = df._rec
+            cols[out] = ColumnData("vector", None, c.dtype, {"attrs": attrs}, ("plan", plan), thunk=lambda: mk(rec0), maker=mk)
+        else:
+            vec, _, _ = plan.run(df._rec, vdtype, want_valid=False)
+            cols[out] = ColumnData("vector", vec, c.dtype, {"attrs": attrs}, ("plan", plan))
+    else:
+        plan = EncodePlan(_dense_schema(D))
+        for i in sel:
+            plan.add_numeric("v%d" % i)
+        vec, _, _ = plan.run(x.view(torch.uint8).reshape(x.shape[0], -1), torch.float64, want_valid=False)
+        cols[out] = ColumnData("vector", vec, "f64", {"attrs": attrs}, None)
+    return df._with(cols=cols)
+
+
+class _SelectorModel(Model):
+    """selectedFeatures (ascending indices); transform keeps those slots of featuresCol."""
+
+    def __init__(self, selectedFeatures):
+        super().__init__()
+        self.selectedFeatures = [int(j) for j in selectedFeatures]
+
+    def _transform(self, df):
+        out = self.getOrDefault("outputCol") or "%s__output" % self.uid
+        return _select_column(df, self.getOrDefault("featuresCol"), out, self.selectedFeatures)
+
+
+def _statistical_selection(est, df, test, mode, threshold):
+    from .stat import _run_test
+    res = _run_test(test, df, est.getOrDefault("featuresCol"), est.getOrDefault("labelCol"))
+    return _sel.select(res.p_values, mode, threshold)
+
+
+class UnivariateFeatureSelector(Estimator):
+    """pyspark.ml.feature.UnivariateFeatureSelector (Spark 3.1): chi-square (categorical features and label), ANOVA
+    (continuous features, categorical label) or F-value (continuous features and label) p-values, then one of five
+    selection rules (b200flow/selection.py, DESIGN.md §5i).  The model is the same for any number of ranks."""
+    _defaults = {"featuresCol": "features", "outputCol": None, "labelCol": "label", "featureType": None, "labelType": None,
+                 "selectionMode": "numTopFeatures", "selectionThreshold": None}
+
+    def __init__(self, featuresCol=None, outputCol=None, labelCol=None, selectionMode=None):
+        super().__init__(featuresCol=featuresCol, outputCol=outputCol, labelCol=labelCol, selectionMode=selectionMode)
+
+    def _fit(self, df):
+        ft, lt = self.getOrDefault("featureType"), self.getOrDefault("labelType")
+        for v, what in ((ft, "featureType"), (lt, "labelType")):
+            if v not in ("categorical", "continuous"):
+                raise IllegalArgumentException("%s must be 'categorical' or 'continuous', got %r" % (what, v))
+        test = {("categorical", "categorical"): _sel.chi_square_test, ("continuous", "categorical"): _sel.anova_test,
+                ("continuous", "continuous"): _sel.f_value_test}.get((ft, lt))
+        if test is None:
+            raise IllegalArgumentException("Unsupported combination: featureType=%s, labelType=%s" % (ft, lt))
+        mode = self.getOrDefault("selectionMode")
+        thr = self.getOrDefault("selectionThreshold")
+        thr = _check_selection(mode, _DEFAULT_THRESHOLD.get(mode, 0.0) if thr is None else thr)
+        m = UnivariateFeatureSelectorModel(_statistical_selection(self, df, test, mode, thr))
+        m._paramMap = dict(self._paramMap)
+        return m
+
+
+class UnivariateFeatureSelectorModel(_SelectorModel):
+    _defaults = dict(UnivariateFeatureSelector._defaults)
+
+
+class ChiSqSelector(Estimator):
+    """pyspark.ml.feature.ChiSqSelector: the chi-square test of every categorical feature against the label, then
+    selectorType's rule (numTopFeatures, percentile, fpr, fdr, fwe)."""
+    _defaults = {"numTopFeatures": 50, "featuresCol": "features", "outputCol": None, "labelCol": "label",
+                 "selectorType": "numTopFeatures", "percentile": 0.1, "fpr": 0.05, "fdr": 0.05, "fwe": 0.05}
+
+    def __init__(self, numTopFeatures=None, featuresCol=None, outputCol=None, labelCol=None, selectorType=None,
+                 percentile=None, fpr=None, fdr=None, fwe=None):
+        super().__init__(numTopFeatures=numTopFeatures, featuresCol=featuresCol, outputCol=outputCol, labelCol=labelCol,
+                         selectorType=selectorType, percentile=percentile, fpr=fpr, fdr=fdr, fwe=fwe)
+
+    def _fit(self, df):
+        mode = self.getOrDefault("selectorType")
+        if mode not in _SELECTION_MODES:
+            raise IllegalArgumentException("selectorType must be one of %s, got %r" % (list(_SELECTION_MODES), mode))
+        for k in _SELECTION_MODES:                       # every threshold is validated, as Spark's param validators do
+            _check_selection(k, self.getOrDefault(k))
+        thr = float(self.getOrDefault(mode))
+        m = ChiSqSelectorModel(_statistical_selection(self, df, _sel.chi_square_test, mode, thr))
+        m._paramMap = dict(self._paramMap)
+        return m
+
+
+class ChiSqSelectorModel(_SelectorModel):
+    _defaults = dict(ChiSqSelector._defaults)
+
+
+class VarianceThresholdSelector(Estimator):
+    """pyspark.ml.feature.VarianceThresholdSelector: keeps the features whose unbiased variance is > varianceThreshold."""
+    _defaults = {"featuresCol": "features", "outputCol": None, "varianceThreshold": 0.0}
+
+    def __init__(self, featuresCol=None, outputCol=None, varianceThreshold=None):
+        super().__init__(featuresCol=featuresCol, outputCol=outputCol, varianceThreshold=varianceThreshold)
+
+    def _fit(self, df):
+        t = self.getOrDefault("varianceThreshold")
+        if not t >= 0.0:
+            raise IllegalArgumentException("varianceThreshold must be >= 0, got %r" % (t,))
+        name = self.getOrDefault("featuresCol")
+        if name not in df._cols:
+            raise IllegalArgumentException("Field \"%s\" does not exist." % name)
+        try:
+            var = _sel.variances(_peek(df, name), group=bdist.group())
+        except ValueError as e:        # includes b200flow's UnsupportedParamError
+            raise IllegalArgumentException(str(e))
+        m = VarianceThresholdSelectorModel([j for j in range(len(var)) if var[j] > t])
+        m._paramMap = dict(self._paramMap)
+        return m
+
+
+class VarianceThresholdSelectorModel(_SelectorModel):
+    _defaults = dict(VarianceThresholdSelector._defaults)
