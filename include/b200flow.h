@@ -458,6 +458,28 @@ int b200flow_mlp_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, int64
 int b200flow_mlp_forward(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, const int32_t* layers, int32_t n_layers,
                          const double* weights, double* raw, void* stream);
 
+/* ------------------------------------------------------------ linear SVM ---
+ * LinearSVC and OneVsRest(LinearSVC), DESIGN.md §5j.  Features x [n_rows][ld] are f32 (x_dtype B200FLOW_F32) or f64
+ * (B200FLOW_F64), converted to f64 before any arithmetic; 1 <= D <= 255, K >= 1 class columns.  Column k's weights
+ * weights[k] = [beta_k (D), b_k] (device f64 [K][D + 1]) act on [xs, 1].  Classes are cut into blocks of at most 256
+ * columns whose gradient tiles fit in registers (8 * ceil(kb / 8) * ceil((D + 1) / 8) <= 256 * 8); a column's results do
+ * not depend on K, on the other columns or on its block.
+ * b200flow_svc_config (host-only): *block_classes = columns per block, *class_blocks = blocks, *smem_bytes = the kernels'
+ * dynamic shared memory; error beyond the limits. */
+int b200flow_svc_config(int32_t D, int64_t K, int32_t* block_classes, int32_t* class_blocks, int64_t* smem_bytes);
+/* partials [n_chunks][K][D + 2] (device; n_chunks = b200flow_group_sums_chunks(row_offset, n_rows)): for each 4096-row
+ * global chunk the rows [0, n_rows) (global rows row_offset + i) touch, and each column k, with xs_j = x_j * inv_std[j]
+ * (one rounding), y' = +1 if labels[i] == positives[k] (int32 [K], device) else -1 and m = [xs, 1] . weights[k] (fp64
+ * tensor cores, features in ascending order): slot 0 = the sum over the chunk's rows in row order from +0.0 of
+ * 1 - y' m where that is > 0, slots 1..D+1 = the sum of -y' [xs, 1] over the same rows (fp64 tensor cores over the rows
+ * in row order).  A chunk's partial depends only on which of its rows are present. */
+int b200flow_svc_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, int32_t D, const int32_t* labels,
+                           const int32_t* positives, int64_t K, const double* inv_std, const double* weights,
+                           int64_t row_offset, double* partials, void* stream);
+/* raw [n_rows][K] f64: raw[i][k] = [x_i, 1] . weights[k] (unscaled), with b200flow_svc_loss_grad's margin arithmetic. */
+int b200flow_svc_margins(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, int32_t D, int64_t K,
+                         const double* weights, double* raw, void* stream);
+
 /* ------------------------------------------------------------ mixture models ---
  * GaussianMixture (full covariance), DESIGN.md §5g.  Features x [n_rows][ld] f64, rows [0, n_rows) are global rows
  * row_offset + i; 1 <= D <= 256, 1 <= k <= 64.  A partial row of chunk b (b counted from the first 4096-row chunk the rows

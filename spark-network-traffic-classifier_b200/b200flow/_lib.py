@@ -80,6 +80,8 @@ _SIGNATURES = {
     "b200flow_silhouette_rows": [_P, _I64, _I32, _I64, _P, _P, _P, _P, _P, _I32, _P, _P],
     "b200flow_mlp_loss_grad": [_P, _I32, _I64, _I64, _P, _P, _I32, _P, _I64, _P, _P],
     "b200flow_mlp_forward": [_P, _I32, _I64, _I64, _P, _I32, _P, _P, _P],
+    "b200flow_svc_loss_grad": [_P, _I32, _I64, _I64, _I32, _P, _P, _I64, _P, _P, _I64, _P, _P],
+    "b200flow_svc_margins": [_P, _I32, _I64, _I64, _I32, _I64, _P, _P, _P],
     "b200flow_gmm_estep": [_P, _I64, _I32, _I64, _I32, _P, _P, _P, _I64, _P, _P, _P, _P],
     "b200flow_gmm_moments": [_P, _I64, _I32, _I64, _I32, _P, _I64, _P, _P],
     "b200flow_centered_gram": [_P, _I64, _I32, _I64, _P, _I64, _P, _P],
@@ -105,7 +107,8 @@ _SIGNATURES = {
 }
 EXPORTS = sorted(list(_SIGNATURES) + ["b200flow_last_error", "b200flow_version", "b200flow_route_hist_config",
                                        "b200flow_packed_layout", "b200flow_binary_counts_scratch",
-                                       "b200flow_group_sums_chunks", "b200flow_mlp_config"])
+                                       "b200flow_group_sums_chunks", "b200flow_mlp_config",
+                                       "b200flow_svc_config"])
 
 _lib = None
 launches = 0   # kernels of OURS launched so far (counted per C-ABI call); bench.py reads the delta over the timed region
@@ -137,6 +140,8 @@ def load():
         lib.b200flow_group_sums_chunks.restype = C.c_int
         lib.b200flow_mlp_config.argtypes = [_P, _I32, C.POINTER(_I64), C.POINTER(_I64)]
         lib.b200flow_mlp_config.restype = C.c_int
+        lib.b200flow_svc_config.argtypes = [_I32, _I64, C.POINTER(_I32), C.POINTER(_I32), C.POINTER(_I64)]
+        lib.b200flow_svc_config.restype = C.c_int
         _lib = lib
     return _lib
 
@@ -188,6 +193,16 @@ def mlp_config(layers):
     if lib.b200flow_mlp_config(la.ctypes.data, int(la.shape[0]), C.byref(P), C.byref(sm)) != 0:
         raise UnsupportedParamError("layers %s: %s" % (list(map(int, la)), lib.b200flow_last_error().decode()))
     return int(P.value), int(sm.value)
+
+
+def svc_config(D, K):
+    """(columns per class block, class blocks, shared-memory bytes) of the LinearSVC kernels (host-only call); raises
+    UnsupportedParamError beyond the kernels' limits."""
+    kb, nb, sm = _I32(0), _I32(0), _I64(0)
+    lib = load()
+    if lib.b200flow_svc_config(int(D), int(K), C.byref(kb), C.byref(nb), C.byref(sm)) != 0:
+        raise UnsupportedParamError("LinearSVC with %d features: %s" % (int(D), lib.b200flow_last_error().decode()))
+    return int(kb.value), int(nb.value), int(sm.value)
 
 
 def ptr(t):

@@ -106,16 +106,14 @@ def _pseudo_gradient(x, g, c):
     return torch.where(x > 0, right, torch.where(x < 0, left, at0))
 
 
-def lbfgs(smooth, v, max_iter, tol, history=10, l1=None):
-    """minimise smooth(v) -> (f, gradient) from v: L-BFGS with `history` corrections, backtracking (Armijo 1e-4, halving,
-    at most 40 trials), stopping after max_iter iterations or once the relative decrease (F - Fn) / max(|Fn|, |F|) falls
-    to tol after the first iteration.  l1 (one weight per variable) makes it OWL-QN for f + sum l1 |v|: the direction
-    is kept to the components that descend along the pseudo-gradient and the steps are projected onto the orthant; None
-    is plain L-BFGS (Breeze LBFGS, what Spark runs without an L1 term).  -> (v, objective history, iterations)."""
+def lbfgs_steps(v, max_iter, tol, history=10, l1=None):
+    """lbfgs as a generator: it yields every point at which it needs the smooth part, receives (f, gradient) for that point
+    through send(), and returns (v, objective history, iterations).  So several problems can advance in lockstep, their
+    evaluations batched by the caller, each taking exactly the steps of its own lbfgs run."""
     def full(v, f):
         return f if l1 is None else f + (l1 * v.abs()).sum()
 
-    f, g = smooth(v)
+    f, g = yield v
     F = float(full(v, f).item())
     hist = [F]
     S, Y, RHO = [], [], []
@@ -147,7 +145,7 @@ def lbfgs(smooth, v, max_iter, tol, history=10, l1=None):
             vn = v + step * d
             if l1 is not None:
                 vn = torch.where(vn * orth < 0, torch.zeros_like(vn), vn)  # projection onto the orthant
-            fn, gn = smooth(vn)
+            fn, gn = yield vn
             Fn = float(full(vn, fn).item())
             if Fn <= F + 1e-4 * float((pg @ (vn - v)).item()):
                 ok = True
@@ -169,6 +167,21 @@ def lbfgs(smooth, v, max_iter, tol, history=10, l1=None):
         if improved <= tol and it > 1:
             break
     return v, hist, it
+
+
+def lbfgs(smooth, v, max_iter, tol, history=10, l1=None):
+    """minimise smooth(v) -> (f, gradient) from v: L-BFGS with `history` corrections, backtracking (Armijo 1e-4, halving,
+    at most 40 trials), stopping after max_iter iterations or once the relative decrease (F - Fn) / max(|Fn|, |F|) falls
+    to tol after the first iteration.  l1 (one weight per variable) makes it OWL-QN for f + sum l1 |v|: the direction
+    is kept to the components that descend along the pseudo-gradient and the steps are projected onto the orthant; None
+    is plain L-BFGS (Breeze LBFGS, what Spark runs without an L1 term).  -> (v, objective history, iterations)."""
+    steps = lbfgs_steps(v, max_iter, tol, history, l1)
+    point = next(steps)
+    try:
+        while True:
+            point = steps.send(smooth(point))
+    except StopIteration as done:
+        return done.value
 
 
 def lr_fit(x, y, num_classes, max_iter=100, reg_param=0.0, elastic_net=0.0, tol=1e-6, fit_intercept=True, standardization=True,

@@ -8,6 +8,9 @@ MultilayerPerceptronClassifier runs on the fused fp64 tensor-core loss/gradient 
 csrc/mlp.cu, DESIGN.md §5d); its model is the same bits for any number of ranks.
 OneVsRest reduces a K-class problem to K binary ones; OneVsRest(GBTClassifier) trains the K boosted models together in one
 level loop on the device (b200flow.gbt.fit_gbt_ovr, DESIGN.md §5f), each the same bits as its standalone fit.
+LinearSVC runs on the fused fp64 tensor-core hinge kernel (b200flow/svc.py, csrc/svc.cu, DESIGN.md §5j);
+OneVsRest(LinearSVC) trains its K models together, one kernel pass per optimiser round, each the same bits as its standalone
+fit, and its transform computes the K margins in one launch.  Both are the same bits for any number of ranks.
 LogisticRegression and NaiveBayes (kdd99.py:57,67; cicids17.py:61,71) are OUT of the kernel scope (SURVEY.md
 §8f rank 4): torch fp64 implementations of MLlib's statistics / objective (b200flow/linear.py), checked against a numpy
 restatement and scikit-learn in tests/test_linear_models.py.
@@ -21,6 +24,7 @@ from b200flow import dist as bdist
 from b200flow import forest as fr
 from b200flow import linear as _linear
 from b200flow import mlp as _mlp
+from b200flow import svc as _svc
 
 from . import Estimator, Model, Pipeline
 from .param import Param
@@ -480,6 +484,126 @@ class MultilayerPerceptronClassificationModel(_ProbModel, _MLPParams):
         return self._emit(df, raw, torch.softmax(raw, 1))
 
 
+# ------------------------------------------------------------------------------- linear SVM (CUDA)
+class _LinearSVCParams:
+    _defaults = {"featuresCol": "features", "labelCol": "label", "predictionCol": "prediction",
+                 "rawPredictionCol": "rawPrediction", "maxIter": 100, "regParam": 0.0, "tol": 1e-6, "fitIntercept": True,
+                 "standardization": True, "threshold": 0.0, "aggregationDepth": 2, "maxBlockSizeInMB": 0.0,
+                 "weightCol": None}
+
+
+class LinearSVC(Estimator, _LinearSVCParams):
+    """Spark 3's binary LinearSVC [recalled]: the hinge loss plus an L2 penalty on standardised (not centred) features,
+    minimised by OWL-QN with a zero L1 weight, on the device (b200flow/svc.py).  aggregationDepth and maxBlockSizeInMB are
+    validated but do not change the result: the sums have one fixed order (DESIGN.md §5j)."""
+
+    def __init__(self, featuresCol=None, labelCol=None, predictionCol=None, maxIter=None, regParam=None, tol=None,
+                 rawPredictionCol=None, fitIntercept=None, standardization=None, threshold=None, weightCol=None,
+                 aggregationDepth=None, maxBlockSizeInMB=None):
+        kw = dict(locals()); kw.pop("self"); kw.pop("__class__", None)
+        super().__init__(**kw)
+
+    def _check(self):
+        """Spark's param validators, and the refusal of weightCol -> b200flow.svc.SVCParams."""
+        g = self.getOrDefault
+        it, depth = g("maxIter"), g("aggregationDepth")
+        if isinstance(it, bool) or int(it) != it or int(it) < 0:
+            raise IllegalArgumentException("maxIter must be an integer >= 0, got %r" % (it,))
+        if isinstance(depth, bool) or int(depth) != depth or int(depth) < 2:
+            raise IllegalArgumentException("aggregationDepth must be an integer >= 2, got %r" % (depth,))
+        for name in ("regParam", "tol", "maxBlockSizeInMB"):
+            if not float(g(name)) >= 0:
+                raise IllegalArgumentException("%s must be >= 0, got %r" % (name, g(name)))
+        if g("weightCol"):
+            raise IllegalArgumentException("weightCol is not supported by the b200flow LinearSVC (out of scope)")
+        return _svc.SVCParams(max_iter=int(it), reg_param=float(g("regParam")), tol=float(g("tol")),
+                              fit_intercept=bool(g("fitIntercept")), standardization=bool(g("standardization")))
+
+    def _fit(self, df):
+        params = self._check()
+        fcol, lcol = self.getOrDefault("featuresCol"), self.getOrDefault("labelCol")
+        for c in (fcol, lcol):
+            if c not in df._cols:
+                raise IllegalArgumentException("Field \"%s\" does not exist." % c)
+        if df._cols[fcol].kind != "vector":
+            raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+        # numClasses and the invalid-label check from values reduced over every rank, so that a rank whose shard is empty
+        # or lacks label 1 decides as the others do, and every rank raises or none does
+        C = _ovr_num_classes(df, lcol)
+        if C != 2:
+            raise IllegalArgumentException("LinearSVC only supports binary classification. %d classes detected in %s"
+                                           % (C, lcol))
+        try:
+            fit = _svc.svc_fit_classes(df._cols[fcol].data, df._column_tensor(lcol), [1], params, group=bdist.group())[0]
+        except ValueError as e:        # includes b200flow's UnsupportedParamError
+            raise IllegalArgumentException(str(e))
+        return _svc_model(fit, self._paramMap)
+
+
+def _svc_model(fit, param_map):
+    m = LinearSVCModel(fit)
+    m._paramMap = {k: v for k, v in param_map.items() if k in m._all_defaults()}
+    return m
+
+
+class LinearSVCModel(Model, _LinearSVCParams):
+    """coefficients (original feature scale), intercept; rawPrediction = [-m, m] with m = x . coefficients + intercept,
+    prediction = 1.0 iff m > threshold; no probability column [recalled]."""
+
+    def __init__(self, fit):
+        super().__init__()
+        self._fit_result = fit             # b200flow.svc.SVCFit
+        self.summary = _TrainingSummary(fit.objective_history, fit.iterations)
+
+    @property
+    def coefficients(self):
+        from .linalg import DenseVector
+        return DenseVector(self._fit_result.coef.copy())
+
+    @property
+    def intercept(self):
+        return self._fit_result.intercept
+
+    @property
+    def numClasses(self):
+        return 2
+
+    @property
+    def numFeatures(self):
+        return int(self._fit_result.coef.shape[0])
+
+    def _weights(self):
+        """[D + 1] f64 host: the coefficients, then the intercept"""
+        return np.concatenate([self._fit_result.coef, [self._fit_result.intercept]])
+
+    def _transform(self, df):
+        fcol = self.getOrDefault("featuresCol")
+        if fcol not in df._cols or df._cols[fcol].kind != "vector":
+            raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+        try:
+            m = _svc.svc_margins(df._cols[fcol].data, torch.from_numpy(self._weights()).reshape(1, -1))
+        except ValueError as e:
+            raise IllegalArgumentException(str(e))
+        cols = dict(df._cols)
+        rcol, pcol = self.getOrDefault("rawPredictionCol"), self.getOrDefault("predictionCol")
+        if rcol:
+            cols[rcol] = ColumnData("vector", torch.cat([-m, m], 1), "f64")
+        if pcol:
+            cols[pcol] = ColumnData("numeric", (m[:, 0] > float(self.getOrDefault("threshold"))).to(torch.float64), "f64")
+        return df._with(cols=cols)
+
+
+class _OvRSVCJoint:
+    """the K LinearSVC models of a OneVsRest fit as one weight matrix: the K margins of a row in one launch"""
+
+    def __init__(self, models):
+        self.weights = torch.from_numpy(np.stack([m._weights() for m in models]))     # [K, D + 1] f64 host
+
+    def predict(self, x):
+        raw = _svc.svc_margins(x, self.weights)
+        return raw, _first_argmax(raw)
+
+
 # ------------------------------------------------------------------------------- gradient-boosted trees (CUDA)
 class _GBTParams(_TreeParams):
     _defaults = {"impurity": "variance", "maxIter": 20, "stepSize": 0.1, "subsamplingRate": 1.0, "featureSubsetStrategy": "all",
@@ -691,8 +815,9 @@ class OneVsRest(Estimator, _OneVsRestParams):
     """Spark 3's OneVsRest [recalled]: one binary model per class k, fitted on the label (label == k ? 1.0 : 0.0), which
     carries two-value nominal metadata; the prediction is the first argmax of the models' rawPrediction[1].  A GBTClassifier
     with at most 256 classes (the label byte of a binned record) is trained as ONE class-batched boosting run on the device
-    (DESIGN.md §5f), whose K models equal the K separate fits bit for bit; every other classifier, and more classes, take the
-    generic loop.  parallelism is validated but only orders host work, so it does not change the result (DESIGN.md §6)."""
+    (DESIGN.md §5f), whose K models equal the K separate fits bit for bit; a LinearSVC trains its K models in lockstep on one
+    kernel pass per optimiser round (DESIGN.md §5j), each equal to its separate fit bit for bit; every other classifier, and
+    GBT with more classes, take the generic loop.  parallelism is validated but only orders host work, so it does not change the result (DESIGN.md §6)."""
     GBT_MAX_CLASSES = 256
 
     def __init__(self, featuresCol=None, labelCol=None, predictionCol=None, rawPredictionCol=None, classifier=None,
@@ -742,6 +867,8 @@ class OneVsRest(Estimator, _OneVsRestParams):
         tmp = _ovr_temp_name(df, "ovr_binary_label")
         if type(clf) is GBTClassifier and K <= self.GBT_MAX_CLASSES:
             models, joint = self._fit_gbt(clf, df, K, tmp)
+        elif type(clf) is LinearSVC:
+            models, joint = self._fit_svc(clf, df, K, tmp)
         else:
             models, joint = self._fit_generic(clf, df, K, tmp), None
         m = OneVsRestModel(models, joint)
@@ -789,6 +916,21 @@ class OneVsRest(Estimator, _OneVsRestParams):
             models.append(m)
         return models, joint
 
+    def _fit_svc(self, clf, df, K, tmp):
+        """the K LinearSVC fits in lockstep on the device (b200flow.svc.svc_fit_classes with positives 0..K-1) -> (K
+        LinearSVCModels, the joint model).  A class absent from the rows still gets its model, as its all-0 relabelled
+        column carries two-value metadata."""
+        binary = self._binary_copy(clf, tmp)
+        params = binary._check()
+        fcol = df._cols[self.getOrDefault("featuresCol")]
+        y = df._column_tensor(self.getOrDefault("labelCol"))
+        try:
+            fits = _svc.svc_fit_classes(fcol.data, y, range(K), params, group=bdist.group())
+        except ValueError as e:        # includes b200flow's UnsupportedParamError
+            raise IllegalArgumentException(str(e))
+        models = [_svc_model(f, binary._paramMap) for f in fits]
+        return models, _OvRSVCJoint(models)
+
 
 _BINARY_LABEL_META = {"ml_attr": {"type": "nominal", "vals": ["0.0", "1.0"]}}
 
@@ -807,7 +949,7 @@ class OneVsRestModel(Model, _OneVsRestParams):
     def __init__(self, models, joint=None):
         super().__init__()
         self.models = list(models)
-        self._joint = joint                   # b200flow.gbt.OvRGBTModel of a class-batched GBT fit, else None
+        self._joint = joint                   # b200flow.gbt.OvRGBTModel of a class-batched GBT fit, _OvRSVCJoint, or None
 
     @property
     def numClasses(self):
@@ -841,6 +983,11 @@ class OneVsRestModel(Model, _OneVsRestParams):
     def _joint_predict(self, df, fcol):
         """one tree walk over the K·T trees (b200flow_predict with C = K): the margins and the `>` argmax in one kernel"""
         j = self._joint
+        if isinstance(j, _OvRSVCJoint):
+            try:
+                return j.predict(df._cols[fcol].data)
+            except ValueError as e:
+                raise IllegalArgumentException(str(e))
         plan = _lazy_plan(df, fcol)
         if plan is not None and plan.n_out == j.F:          # lazy features: fused encode -> bins -> tree walk
             from .feature import SparkException
