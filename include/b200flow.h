@@ -480,6 +480,34 @@ int b200flow_svc_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, int64
 int b200flow_svc_margins(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, int32_t D, int64_t K,
                          const double* weights, double* raw, void* stream);
 
+/* ------------------------------------------------------------ factorization machines ---
+ * FMClassifier and OneVsRest(FMClassifier), DESIGN.md §5k.  Features x [n_rows][ld] are f32 (x_dtype B200FLOW_F32) or
+ * f64 (B200FLOW_F64), converted to f64 before any arithmetic; 1 <= D <= 255, factor_size F >= 1, K >= 1 class columns.
+ * Column k's weights weights[k] = [V_k (D x F, row-major), w_k (D), b_k] (device f64 [K][D (F + 1) + 1]).  With
+ * s_f = sum_i v_if x_i and q_f = sum_i x_i^2 v_if^2 (fp64 tensor cores, features in ascending order), the raw value is
+ * r = (b + x . w) + 1/2 (s_0^2 - q_0) + 1/2 (s_1^2 - q_1) + ...  Classes are cut into blocks whose gradient tiles fit in
+ * registers and whose products fit in shared memory; a column's results do not depend on K, on the other columns or on
+ * its block.  Every D <= 255 with F <= 32 fits.
+ * b200flow_fm_config (host-only): *block_classes = classes per block, *class_blocks = blocks, *smem_bytes = the kernels'
+ * dynamic shared memory; error beyond the limits. */
+int b200flow_fm_config(int32_t D, int32_t factor_size, int64_t K, int32_t* block_classes, int32_t* class_blocks,
+                       int64_t* smem_bytes);
+/* partials [n_chunks][K][D (F + 1) + D + 3] (device; n_chunks = b200flow_group_sums_chunks(row_offset, n_rows)): for each
+ * 4096-row global chunk the rows [0, n_rows) (global rows row_offset + i) touch, and each column k, over the chunk's rows
+ * in the mini-batch (all rows when mini_batch_fraction == 1, else those whose Philox draw, purpose FMMB, key seed
+ * batch_seed, counter (global row lo, hi, 0, 0), word 0, is < floor(fraction 2^32)), with y = 1 if labels[i] ==
+ * positives[k] (int32 [K], device) else 0 and g = 1 / (1 + exp(-r)) - y: slot 0 = the loss sum in row order from +0.0
+ * (log1pExp(-r) if y = 1, else log1pExp(r)), slot 1 = the row count, then sum g x_i s_f at 2 + i F + f, sum g x_i at
+ * 2 + D F + i, sum g at 2 + D F + D, and sum g x_i^2 at 3 + D F + D + i (fp64 tensor cores over the rows in row order).
+ * The factor gradient is the first block minus v_if times the last.  A chunk's partial depends only on which of its rows
+ * are present. */
+int b200flow_fm_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, int32_t D, int32_t factor_size,
+                          const int32_t* labels, const int32_t* positives, int64_t K, const double* weights,
+                          double mini_batch_fraction, uint64_t batch_seed, int64_t row_offset, double* partials, void* stream);
+/* raw [n_rows][K] f64: raw[i][k] = r of row i under weights[k], with b200flow_fm_loss_grad's arithmetic. */
+int b200flow_fm_raw(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, int32_t D, int32_t factor_size, int64_t K,
+                    const double* weights, double* raw, void* stream);
+
 /* ------------------------------------------------------------ mixture models ---
  * GaussianMixture (full covariance), DESIGN.md §5g.  Features x [n_rows][ld] f64, rows [0, n_rows) are global rows
  * row_offset + i; 1 <= D <= 256, 1 <= k <= 64.  A partial row of chunk b (b counted from the first 4096-row chunk the rows

@@ -82,6 +82,8 @@ _SIGNATURES = {
     "b200flow_mlp_forward": [_P, _I32, _I64, _I64, _P, _I32, _P, _P, _P],
     "b200flow_svc_loss_grad": [_P, _I32, _I64, _I64, _I32, _P, _P, _I64, _P, _P, _I64, _P, _P],
     "b200flow_svc_margins": [_P, _I32, _I64, _I64, _I32, _I64, _P, _P, _P],
+    "b200flow_fm_loss_grad": [_P, _I32, _I64, _I64, _I32, _I32, _P, _P, _I64, _P, _F64, _U64, _I64, _P, _P],
+    "b200flow_fm_raw": [_P, _I32, _I64, _I64, _I32, _I32, _I64, _P, _P, _P],
     "b200flow_gmm_estep": [_P, _I64, _I32, _I64, _I32, _P, _P, _P, _I64, _P, _P, _P, _P],
     "b200flow_gmm_moments": [_P, _I64, _I32, _I64, _I32, _P, _I64, _P, _P],
     "b200flow_centered_gram": [_P, _I64, _I32, _I64, _P, _I64, _P, _P],
@@ -108,7 +110,7 @@ _SIGNATURES = {
 EXPORTS = sorted(list(_SIGNATURES) + ["b200flow_last_error", "b200flow_version", "b200flow_route_hist_config",
                                        "b200flow_packed_layout", "b200flow_binary_counts_scratch",
                                        "b200flow_group_sums_chunks", "b200flow_mlp_config",
-                                       "b200flow_svc_config"])
+                                       "b200flow_svc_config", "b200flow_fm_config"])
 
 _lib = None
 launches = 0   # kernels of OURS launched so far (counted per C-ABI call); bench.py reads the delta over the timed region
@@ -142,6 +144,8 @@ def load():
         lib.b200flow_mlp_config.restype = C.c_int
         lib.b200flow_svc_config.argtypes = [_I32, _I64, C.POINTER(_I32), C.POINTER(_I32), C.POINTER(_I64)]
         lib.b200flow_svc_config.restype = C.c_int
+        lib.b200flow_fm_config.argtypes = [_I32, _I32, _I64, C.POINTER(_I32), C.POINTER(_I32), C.POINTER(_I64)]
+        lib.b200flow_fm_config.restype = C.c_int
         _lib = lib
     return _lib
 
@@ -202,6 +206,17 @@ def svc_config(D, K):
     lib = load()
     if lib.b200flow_svc_config(int(D), int(K), C.byref(kb), C.byref(nb), C.byref(sm)) != 0:
         raise UnsupportedParamError("LinearSVC with %d features: %s" % (int(D), lib.b200flow_last_error().decode()))
+    return int(kb.value), int(nb.value), int(sm.value)
+
+
+def fm_config(D, factor_size, K):
+    """(classes per class block, class blocks, shared-memory bytes) of the FMClassifier kernels (host-only call); raises
+    UnsupportedParamError beyond the kernels' limits."""
+    kb, nb, sm = _I32(0), _I32(0), _I64(0)
+    lib = load()
+    if lib.b200flow_fm_config(int(D), int(factor_size), int(K), C.byref(kb), C.byref(nb), C.byref(sm)) != 0:
+        raise UnsupportedParamError("FMClassifier with %d features and factorSize %d: %s"
+                                    % (int(D), int(factor_size), lib.b200flow_last_error().decode()))
     return int(kb.value), int(nb.value), int(sm.value)
 
 

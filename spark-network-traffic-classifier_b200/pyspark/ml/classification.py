@@ -11,6 +11,10 @@ level loop on the device (b200flow.gbt.fit_gbt_ovr, DESIGN.md §5f), each the sa
 LinearSVC runs on the fused fp64 tensor-core hinge kernel (b200flow/svc.py, csrc/svc.cu, DESIGN.md §5j);
 OneVsRest(LinearSVC) trains its K models together, one kernel pass per optimiser round, each the same bits as its standalone
 fit, and its transform computes the K margins in one launch.  Both are the same bits for any number of ranks.
+FMClassifier runs on the fused fp64 tensor-core factorization-machine kernel (b200flow/fm.py, csrc/fm.cu, DESIGN.md §5k);
+OneVsRest(FMClassifier) trains its K models together, one kernel pass per gradient-descent iteration, each the same bits
+as its standalone fit, and its transform computes the K raw values in one launch.  Both are the same bits for any number
+of ranks.
 LogisticRegression and NaiveBayes (kdd99.py:57,67; cicids17.py:61,71) are OUT of the kernel scope (SURVEY.md
 §8f rank 4): torch fp64 implementations of MLlib's statistics / objective (b200flow/linear.py), checked against a numpy
 restatement and scikit-learn in tests/test_linear_models.py.
@@ -22,6 +26,7 @@ import torch
 
 from b200flow import dist as bdist
 from b200flow import forest as fr
+from b200flow import fm as _fm
 from b200flow import linear as _linear
 from b200flow import mlp as _mlp
 from b200flow import svc as _svc
@@ -604,6 +609,147 @@ class _OvRSVCJoint:
         return raw, _first_argmax(raw)
 
 
+# ------------------------------------------------------------------------------- factorization machines (CUDA)
+class _FMParams:
+    _defaults = dict(_ProbModel._defaults, factorSize=8, fitIntercept=True, fitLinear=True, regParam=0.0,
+                     miniBatchFraction=1.0, initStd=0.01, maxIter=100, stepSize=1.0, tol=1e-6, solver="adamW",
+                     thresholds=None, seed=None, weightCol=None)
+
+
+class FMClassifier(Estimator, _FMParams):
+    """Spark 3's binary FMClassifier [recalled]: a factorization machine with the logistic loss, trained by mllib's
+    mini-batch gradient descent with the adamW or gd updater, on the device (b200flow/fm.py, csrc/fm.cu, DESIGN.md §5k).
+    Features are not standardised."""
+
+    def __init__(self, featuresCol=None, labelCol=None, predictionCol=None, probabilityCol=None, rawPredictionCol=None,
+                 factorSize=None, fitIntercept=None, fitLinear=None, regParam=None, miniBatchFraction=None, initStd=None,
+                 maxIter=None, stepSize=None, tol=None, solver=None, thresholds=None, seed=None, weightCol=None):
+        kw = dict(locals()); kw.pop("self"); kw.pop("__class__", None)
+        super().__init__(**kw)
+
+    def _check(self):
+        """Spark's param validators, and the refusals of weightCol and thresholds -> b200flow.fm.FMParams."""
+        g = self.getOrDefault
+        fs, it = g("factorSize"), g("maxIter")
+        if isinstance(fs, bool) or int(fs) != fs or int(fs) < 1:
+            raise IllegalArgumentException("factorSize must be an integer >= 1, got %r" % (fs,))
+        if isinstance(it, bool) or int(it) != it or int(it) < 0:
+            raise IllegalArgumentException("maxIter must be an integer >= 0, got %r" % (it,))
+        for name in ("regParam", "initStd", "tol"):
+            if not float(g(name)) >= 0:
+                raise IllegalArgumentException("%s must be >= 0, got %r" % (name, g(name)))
+        if not float(g("stepSize")) > 0:
+            raise IllegalArgumentException("stepSize must be > 0, got %r" % (g("stepSize"),))
+        if not 0.0 < float(g("miniBatchFraction")) <= 1.0:
+            raise IllegalArgumentException("miniBatchFraction must be in (0, 1], got %r" % (g("miniBatchFraction"),))
+        if g("solver") not in _fm.SOLVERS:
+            raise IllegalArgumentException("solver must be 'gd' or 'adamW', got %r" % (g("solver"),))
+        if g("weightCol"):
+            raise IllegalArgumentException("weightCol is not supported by the b200flow FMClassifier (out of scope)")
+        if g("thresholds") is not None:
+            raise IllegalArgumentException("thresholds is not supported by the b200flow FMClassifier")
+        seed = g("seed")
+        return _fm.FMParams(factor_size=int(fs), fit_intercept=bool(g("fitIntercept")), fit_linear=bool(g("fitLinear")),
+                            reg_param=float(g("regParam")), mini_batch_fraction=float(g("miniBatchFraction")),
+                            init_std=float(g("initStd")), max_iter=int(it), step_size=float(g("stepSize")),
+                            tol=float(g("tol")), solver=g("solver"), seed=_default_seed(self) if seed is None else int(seed))
+
+    def _fit(self, df):
+        params = self._check()
+        fcol, lcol = self.getOrDefault("featuresCol"), self.getOrDefault("labelCol")
+        for c in (fcol, lcol):
+            if c not in df._cols:
+                raise IllegalArgumentException("Field \"%s\" does not exist." % c)
+        if df._cols[fcol].kind != "vector":
+            raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+        # numClasses from values reduced over every rank, as LinearSVC
+        C = _ovr_num_classes(df, lcol)
+        if C != 2:
+            raise IllegalArgumentException("FMClassifier only supports binary classification. %d classes detected in %s"
+                                           % (C, lcol))
+        try:
+            fit = _fm.fm_fit_classes(df._cols[fcol].data, df._column_tensor(lcol), [1], params, group=bdist.group())[0]
+        except ValueError as e:        # includes b200flow's UnsupportedParamError
+            raise IllegalArgumentException(str(e))
+        return _fm_model(fit, self._paramMap)
+
+
+def _fm_model(fit, param_map):
+    m = FMClassificationModel(fit)
+    m._paramMap = {k: v for k, v in param_map.items() if k in m._all_defaults()}
+    return m
+
+
+class FMClassificationModel(_ProbModel, _FMParams):
+    """intercept, linear (DenseVector [D]), factors (DenseMatrix D x k); rawPrediction = [-r, r], probability =
+    [1 - sigmoid(r), sigmoid(r)], prediction = the first argmax of rawPrediction (1.0 iff r > 0) [recalled]."""
+
+    def __init__(self, fit):
+        super().__init__()
+        self._fit_result = fit             # b200flow.fm.FMFit
+        # Spark's TrainingSummary: totalIterations = objectiveHistory.length - 1
+        self.summary = _TrainingSummary(fit.objective_history, max(len(fit.objective_history) - 1, 0))
+
+    @property
+    def intercept(self):
+        return self._fit_result.intercept
+
+    @property
+    def linear(self):
+        from .linalg import DenseVector
+        return DenseVector(self._fit_result.linear.copy())
+
+    @property
+    def factors(self):
+        from .linalg import DenseMatrix
+        f = self._fit_result.factors
+        return DenseMatrix(f.shape[0], f.shape[1], f.T.reshape(-1))
+
+    @property
+    def numClasses(self):
+        return 2
+
+    @property
+    def numFeatures(self):
+        return int(self._fit_result.factors.shape[0])
+
+    def _weights(self):
+        """[D (k + 1) + 1] f64 host: [V (row-major) | w | b], fm_raw's layout"""
+        f = self._fit_result
+        return np.concatenate([f.factors.reshape(-1), f.linear, [f.intercept]])
+
+    def _transform(self, df):
+        fcol = self.getOrDefault("featuresCol")
+        if fcol not in df._cols or df._cols[fcol].kind != "vector":
+            raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+        try:
+            r = _fm.fm_raw(df._cols[fcol].data, torch.from_numpy(self._weights()).reshape(1, -1),
+                           self._fit_result.factors.shape[1])
+        except ValueError as e:
+            raise IllegalArgumentException(str(e))
+        raw = torch.cat([-r, r], 1)
+        p1 = 1.0 / (1.0 + torch.exp(-r))
+        cols = dict(df._cols)
+        for name, val, kind in ((self.getOrDefault("rawPredictionCol"), raw, "vector"),
+                                (self.getOrDefault("probabilityCol"), torch.cat([1.0 - p1, p1], 1), "vector"),
+                                (self.getOrDefault("predictionCol"), _first_argmax(raw), "numeric")):
+            if name:
+                cols[name] = ColumnData(kind, val, "f64")
+        return df._with(cols=cols)
+
+
+class _OvRFMJoint:
+    """the K FMClassifier models of a OneVsRest fit as one weight matrix: the K raw values of a row in one launch"""
+
+    def __init__(self, models):
+        self.factor_size = models[0]._fit_result.factors.shape[1]
+        self.weights = torch.from_numpy(np.stack([m._weights() for m in models]))     # [K, D (k + 1) + 1] f64 host
+
+    def predict(self, x):
+        raw = _fm.fm_raw(x, self.weights, self.factor_size)
+        return raw, _first_argmax(raw)
+
+
 # ------------------------------------------------------------------------------- gradient-boosted trees (CUDA)
 class _GBTParams(_TreeParams):
     _defaults = {"impurity": "variance", "maxIter": 20, "stepSize": 0.1, "subsamplingRate": 1.0, "featureSubsetStrategy": "all",
@@ -816,7 +962,9 @@ class OneVsRest(Estimator, _OneVsRestParams):
     carries two-value nominal metadata; the prediction is the first argmax of the models' rawPrediction[1].  A GBTClassifier
     with at most 256 classes (the label byte of a binned record) is trained as ONE class-batched boosting run on the device
     (DESIGN.md §5f), whose K models equal the K separate fits bit for bit; a LinearSVC trains its K models in lockstep on one
-    kernel pass per optimiser round (DESIGN.md §5j), each equal to its separate fit bit for bit; every other classifier, and
+    kernel pass per optimiser round (DESIGN.md §5j), each equal to its separate fit bit for bit; an FMClassifier trains its K
+    models in lockstep on one kernel pass per gradient-descent iteration (DESIGN.md §5k), each equal to its separate fit bit
+    for bit; every other classifier, and
     GBT with more classes, take the generic loop.  parallelism is validated but only orders host work, so it does not change the result (DESIGN.md §6)."""
     GBT_MAX_CLASSES = 256
 
@@ -869,6 +1017,8 @@ class OneVsRest(Estimator, _OneVsRestParams):
             models, joint = self._fit_gbt(clf, df, K, tmp)
         elif type(clf) is LinearSVC:
             models, joint = self._fit_svc(clf, df, K, tmp)
+        elif type(clf) is FMClassifier:
+            models, joint = self._fit_fm(clf, df, K, tmp)
         else:
             models, joint = self._fit_generic(clf, df, K, tmp), None
         m = OneVsRestModel(models, joint)
@@ -931,6 +1081,20 @@ class OneVsRest(Estimator, _OneVsRestParams):
         models = [_svc_model(f, binary._paramMap) for f in fits]
         return models, _OvRSVCJoint(models)
 
+    def _fit_fm(self, clf, df, K, tmp):
+        """the K FMClassifier fits in lockstep on the device (b200flow.fm.fm_fit_classes with positives 0..K-1) -> (K
+        FMClassificationModels, the joint model).  A class absent from the rows still gets its model."""
+        binary = self._binary_copy(clf, tmp)
+        params = binary._check()
+        fcol = df._cols[self.getOrDefault("featuresCol")]
+        y = df._column_tensor(self.getOrDefault("labelCol"))
+        try:
+            fits = _fm.fm_fit_classes(fcol.data, y, range(K), params, group=bdist.group())
+        except ValueError as e:        # includes b200flow's UnsupportedParamError
+            raise IllegalArgumentException(str(e))
+        models = [_fm_model(f, binary._paramMap) for f in fits]
+        return models, _OvRFMJoint(models)
+
 
 _BINARY_LABEL_META = {"ml_attr": {"type": "nominal", "vals": ["0.0", "1.0"]}}
 
@@ -949,7 +1113,7 @@ class OneVsRestModel(Model, _OneVsRestParams):
     def __init__(self, models, joint=None):
         super().__init__()
         self.models = list(models)
-        self._joint = joint                   # b200flow.gbt.OvRGBTModel of a class-batched GBT fit, _OvRSVCJoint, or None
+        self._joint = joint                   # b200flow.gbt.OvRGBTModel of a class-batched GBT fit, _OvRSVCJoint, _OvRFMJoint or None
 
     @property
     def numClasses(self):
@@ -983,7 +1147,7 @@ class OneVsRestModel(Model, _OneVsRestParams):
     def _joint_predict(self, df, fcol):
         """one tree walk over the K·T trees (b200flow_predict with C = K): the margins and the `>` argmax in one kernel"""
         j = self._joint
-        if isinstance(j, _OvRSVCJoint):
+        if isinstance(j, (_OvRSVCJoint, _OvRFMJoint)):
             try:
                 return j.predict(df._cols[fcol].data)
             except ValueError as e:
