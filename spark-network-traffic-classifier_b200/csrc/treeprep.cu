@@ -395,10 +395,14 @@ constexpr int kBagBlockRows = 1024;
 // the tree quads (one Philox call per row yields the weights of a quad's 4 trees; the duplicate-group search is per row, not per tree).  Lanes whose rows belong to the same duplicate
 // group are merged first (match.any on the unique id + three ballots for the weights 1..3), so a hot group — the smurf
 // flood is a third of KDD99 — costs one global RED per warp and tree instead of one per row.
-struct CdfHead { uint32_t c[6]; };       // first thresholds of the inverse CDF, passed by value (uniform registers)
+// First thresholds of the inverse CDF, passed by value (uniform registers).  n = how many of them are not saturated
+// (0xFFFFFFFF): a saturated threshold is unreachable, yet r = 0xFFFFFFFF passes `r >= c[k]`, so the count is clamped to n.
+// Small subsampling rates saturate inside the head (Poisson 0.07: c[5]; GBT's Bernoulli CDF: c[1..]).
+struct CdfHead { uint32_t c[6]; uint32_t n; };
 
 __device__ __forceinline__ uint32_t poisson_weight_fast(uint32_t r, const CdfHead& h, const uint32_t* cdf_sh) {
     uint32_t k = (r >= h.c[0]) + (r >= h.c[1]) + (r >= h.c[2]) + (r >= h.c[3]) + (r >= h.c[4]) + (r >= h.c[5]);   // increasing thresholds
+    k = min(k, h.n);
     if (k == 6) while (k < 32 && cdf_sh[k] != 0xFFFFFFFFu && r >= cdf_sh[k]) ++k;                                 // P(w >= 6) = 6e-4 at lambda = 1
     return k;
 }
@@ -667,7 +671,11 @@ extern "C" int b200flow_bag_weights(uint64_t seed, int32_t T, int64_t row_offset
     B2F_REQUIRE(W && T > 0 && T <= 65535 * 4 && n_unique > 0, "bag_weights: bad arguments");
     B2F_REQUIRE((poisson_cdf == nullptr) == (poisson_cdf_host == nullptr), "bag_weights: pass the CDF table both as device and host pointer");
     CdfHead head;
-    for (int k = 0; k < 6; ++k) head.c[k] = poisson_cdf_host ? poisson_cdf_host[k] : 0xFFFFFFFFu;
+    head.n = 0;
+    for (int k = 0; k < 6; ++k) {
+        head.c[k] = poisson_cdf_host ? poisson_cdf_host[k] : 0xFFFFFFFFu;
+        if (head.c[k] != 0xFFFFFFFFu && head.n == (uint32_t)k) ++head.n;        // leading non-saturated thresholds
+    }
     const int64_t nb = (n_rows + kBagBlockRows - 1) / kBagBlockRows;
     bag_weights_kernel<<<(unsigned)nb, 256, 0, (cudaStream_t)stream>>>(seed, T, row_offset, n_rows, poisson_cdf, head, uid, perm, n_unique, W);
     return check_launch("bag_weights");
