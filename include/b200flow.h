@@ -613,6 +613,34 @@ int b200flow_gbt_update_classes(const uint8_t* tp, int32_t tp_stride, int32_t F,
  * pred = F > 0; raw / prob / pred may be NULL. */
 int b200flow_gbt_output(const double* margin, int64_t n_rows, double* raw, double* prob, double* pred, void* stream);
 
+/* -------------------------------------------------- regression (csrc/regression.cu, DESIGN.md §5l) ---
+ * Labels y' = y 2^-E on the grid of the variance-tree kernels above: q = rint(y' 2^S), q2 = rint((q 2^-S)^2 2^S2); the
+ * level loop passes S - E and S2 - 2E to b200flow_gbt_score_level, so gains and leaf values come out in label units. */
+/* out int64[2] (caller zeroes): [0] += labels that are NaN or ±inf, [1] = max |y| over the finite labels (as its bits);
+ * tp != NULL: the 8 bytes of y[i] are written to bytes [offset, offset + 8) of record i (tp_stride bytes each) */
+int b200flow_reg_labels(const double* y, int64_t n_rows, uint8_t* tp, int32_t tp_stride, int32_t offset, int64_t* out,
+                        void* stream);
+/* totals int64[n_trees] (caller zeroes) += Σ_u W[t][u] over the bag weights W int32 [n_trees][n_unique] */
+int b200flow_reg_tree_weights(const int32_t* W, int32_t n_trees, int64_t n_unique, int64_t* totals, void* stream);
+/* rq int64 [n_rows][2] (16-byte aligned) = {q, q2} of each record's label: read from its bytes [offset, offset + 8) when tp
+ * != NULL, else y[u]; 0 < S, S2 <= 62 */
+int b200flow_reg_grid(const uint8_t* tp, int32_t tp_stride, int32_t offset, const double* y, int64_t n_rows, int32_t E,
+                      int32_t S, int32_t S2, int64_t* rq, void* stream);
+/* table f64 [n_nodes][width]: [0] = (Σw·q 2^-S) / Σw of each node's stats int64 [n_nodes][3]; width 2 adds [1] = the
+ * node's variance (Σw·q2 2^-S2 - (Σw·q 2^-S)^2 / Σw) / Σw, 0 for an empty node */
+int b200flow_reg_leaf_table(int64_t n_nodes, const int64_t* stats, int32_t S, int32_t S2, double* table, int32_t width,
+                            void* stream);
+/* out[i] = in[i] / d for n_rows doubles, IEEE-rounded (in == out allowed): the forest's prediction, Σ over trees / T */
+int b200flow_reg_divide(const double* in, int64_t n_rows, double d, double* out, void* stream);
+/* RegressionEvaluator terms of each row: mode 0 {y, y^2, (y - p)^2, |y - p|}, mode 1 {(y - mean)^2, (p - mean)^2}.
+ * out int64[5] (caller zeroes): [0] += rows with a non-finite label, prediction or term, [1 + k] = max |term k| (bits). */
+int b200flow_reg_eval_max(const double* label, const double* pred, int64_t n_rows, int32_t mode, double mean, int64_t* out,
+                          void* stream);
+/* limbs int64 [4][4] (caller zeroes): limbs[k][j] += Σ_rows limb j of rint(term k 2^sh_k) as a two's-complement 128-bit
+ * integer (32-bit limbs, the top one signed); rows counted by b200flow_reg_eval_max are skipped.  n_rows < 2^31. */
+int b200flow_reg_eval_sums(const double* label, const double* pred, int64_t n_rows, int32_t mode, double mean, int32_t sh0,
+                           int32_t sh1, int32_t sh2, int32_t sh3, int64_t* limbs, void* stream);
+
 /* -------------------------------------------------- either side of the path ---
  * DataFrame.randomSplit (kdd99.py:52, cicids17.py:56): split id per row from a uniform keyed
  * by (seed, global row): first k with u < cum_bounds[k] (n_splits <= 32).  out uint8[n]. */

@@ -99,6 +99,13 @@ _SIGNATURES = {
     "b200flow_gbt_update": [_P, _I32, _I32, _I64, _P, _P, _P, _I32, _I32, _I32, _P, _P, _P],
     "b200flow_gbt_update_classes": [_P, _I32, _I32, _I64, _I32, _P, _P, _P, _I32, _I32, _I32, _I32, _P, _P, _P],
     "b200flow_gbt_output": [_P, _I64, _P, _P, _P, _P],
+    "b200flow_reg_labels": [_P, _I64, _P, _I32, _I32, _P, _P],
+    "b200flow_reg_tree_weights": [_P, _I32, _I64, _P, _P],
+    "b200flow_reg_grid": [_P, _I32, _I32, _P, _I64, _I32, _I32, _I32, _P, _P],
+    "b200flow_reg_leaf_table": [_I64, _P, _I32, _I32, _P, _I32, _P],
+    "b200flow_reg_divide": [_P, _I64, _F64, _P, _P],
+    "b200flow_reg_eval_max": [_P, _P, _I64, _I32, _F64, _P, _P],
+    "b200flow_reg_eval_sums": [_P, _P, _I64, _I32, _F64, _I32, _I32, _I32, _I32, _P, _P],
     "b200flow_random_split": [_U64, _I64, _I64, _P, _I32, _P, _P],
     "b200flow_compact_rows": [_P, _I64, _I32, _P, _I32, _P, _P, _P, _P],
     "b200flow_csv_count_lines": [_P, _I64, _P, _P, _P],

@@ -471,7 +471,10 @@ class _TrainingRows:
     read() then fetches the bad-cell counts, the bin count, the sample count and the unique-record count in ONE host read, so
     the caller can prepare what does not depend on them in between, while the GPU works through the queue."""
 
-    def __init__(self, src, num_classes, arity, max_bins, num_trees, strategy, seed, row_offset, group):
+    def __init__(self, src, num_classes, arity, max_bins, num_trees, strategy, seed, row_offset, group, key_bytes=None,
+                 dedup=None):
+        """key_bytes: the record bytes de-duplication compares (default F + 1: bins and label byte); dedup=False keeps the
+        binned rows as they are (default: DEDUP)"""
         from . import dist as bdist
         dev = src.device
         n, F, C, T = src.n, src.F, num_classes, num_trees
@@ -515,9 +518,9 @@ class _TrainingRows:
         feat_kind = _i32(kind, dev)
         # ---- de-duplicate the binned rows: the level loop runs on UNIQUE TreePoint records carrying summed bag weights.
         # Everything is enqueued first; ONE host read then fetches the bad-cell counts, the bin count, the sample count and U.
-        dedup = n > 0 and DEDUP
+        dedup = n > 0 and (DEDUP if dedup is None else bool(dedup))
         if dedup:
-            tp, uid, u_dev = dedup_rows(tp, F + 1, sync=False)
+            tp, uid, u_dev = dedup_rows(tp, F + 1 if key_bytes is None else key_bytes, sync=False)
         else:
             uid, u_dev = None, torch.full((1,), n, dtype=torch.int64, device=dev)
         self.src, self.group, self.n, self.F, self.n_global = src, group, n, F, n_global

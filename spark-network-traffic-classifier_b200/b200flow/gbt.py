@@ -59,6 +59,24 @@ def subsample_cdf(rate):
     return cdf
 
 
+def export_pool(fo, stats):
+    """canonical host copy of a variance-tree pool (ForestModel fo whose leaf_prob[:, 0] is the payload, stats int64 [pool][3])
+    ordered by (tree, node id)"""
+    n = fo.n_nodes
+    nodes = fo.nodes[:n].cpu().numpy().view(NODE_DTYPE).reshape(-1)
+    tree = fo.node_tree[:n].cpu().numpy()
+    order = np.lexsort((nodes["nid"], tree))
+    mask = (fo.node_mask[:n].cpu().numpy().view(np.uint64) if fo.node_mask is not None else np.zeros((n, 4), np.uint64))
+    is_leaf = (nodes["feat"] < 0).astype(np.int32)
+    kind = np.where(is_leaf == 1, 0, nodes["kind_bin"] >> 16).astype(np.int32)
+    bin_thr = np.where(is_leaf == 1, 0, nodes["kind_bin"] & 0xffff).astype(np.int32)
+    mask = np.where(is_leaf[:, None] == 1, 0, mask).astype(np.uint64)
+    return dict(tree=tree[order], nid=nodes["nid"][order], feat=np.where(is_leaf == 1, -1, nodes["feat"])[order],
+                kind=kind[order], bin_thr=bin_thr[order], is_leaf=is_leaf[order], mask=mask[order],
+                gain=fo.node_gain[:n].cpu().numpy()[order], payload=fo.leaf_prob[:n, 0].cpu().numpy()[order],
+                stats=stats[:n].cpu().numpy()[order])
+
+
 class GBTModel:
     """Device-resident boosted trees: one node pool (roots = nodes 0..T-1), payload[node] = tree weight x leaf value."""
 
@@ -98,20 +116,7 @@ class GBTModel:
 
     def export(self):
         """canonical host copy ordered by (tree, node id): the forest export's structure + payload, gain and int64 stats"""
-        fo = self.forest
-        n = fo.n_nodes
-        nodes = fo.nodes[:n].cpu().numpy().view(NODE_DTYPE).reshape(-1)
-        tree = fo.node_tree[:n].cpu().numpy()
-        order = np.lexsort((nodes["nid"], tree))
-        mask = (fo.node_mask[:n].cpu().numpy().view(np.uint64) if fo.node_mask is not None else np.zeros((n, 4), np.uint64))
-        is_leaf = (nodes["feat"] < 0).astype(np.int32)
-        kind = np.where(is_leaf == 1, 0, nodes["kind_bin"] >> 16).astype(np.int32)
-        bin_thr = np.where(is_leaf == 1, 0, nodes["kind_bin"] & 0xffff).astype(np.int32)
-        mask = np.where(is_leaf[:, None] == 1, 0, mask).astype(np.uint64)
-        return dict(tree=tree[order], nid=nodes["nid"][order], feat=np.where(is_leaf == 1, -1, nodes["feat"])[order],
-                    kind=kind[order], bin_thr=bin_thr[order], is_leaf=is_leaf[order], mask=mask[order],
-                    gain=fo.node_gain[:n].cpu().numpy()[order], payload=fo.leaf_prob[:n, 0].cpu().numpy()[order],
-                    stats=self.stats[:n].cpu().numpy()[order])
+        return export_pool(self.forest, self.stats)
 
     def feature_importances(self):
         """featureImportances with perTreeNormalization = false (SPARK-26721): Σ gain · count over the internal nodes of all
@@ -173,6 +178,137 @@ class OvRGBTModel:
         return raw, pred
 
 
+class NodePool:
+    """the growing node pool of a variance-tree fit: roots 0..n_roots-1; a node's stats are 3 int64 {Σw, Σw·q, Σw·q2} = the
+    6 opaque words grow_level copies per node"""
+
+    def __init__(self, n_roots, cap, with_mask, dev):
+        self.dev, self.cap, self.size = dev, cap, n_roots
+        self.nodes = torch.zeros((cap, 16), dtype=torch.uint8, device=dev)
+        self.node_mask = torch.zeros((cap, 4), dtype=torch.int64, device=dev) if with_mask else None
+        self.stats = torch.zeros((cap, 3), dtype=torch.int64, device=dev)
+        self.node_tree = torch.zeros(cap, dtype=torch.int32, device=dev)
+        self.node_gain = torch.zeros(cap, dtype=torch.float64, device=dev)
+        root = np.zeros(n_roots, NODE_DTYPE); root["feat"] = -1; root["left"] = -1; root["nid"] = 1
+        self.nodes[:n_roots] = _lib.h2d(root.view(np.uint8).reshape(n_roots, 16), dev)
+        self.node_tree[:n_roots] = torch.arange(n_roots, dtype=torch.int32, device=dev)
+        self.counters = torch.zeros(8 + 2 * 64 + 1024, dtype=torch.int64, device=dev)
+
+    def grow(self, need):
+        if need <= self.cap:
+            return
+        new_cap = self.cap
+        while new_cap < need:
+            new_cap *= 2
+
+        def ext(t):
+            nt = torch.zeros((new_cap,) + tuple(t.shape[1:]), dtype=t.dtype, device=self.dev)
+            nt[:self.cap] = t
+            return nt
+        self.nodes, self.stats, self.node_tree, self.node_gain = ext(self.nodes), ext(self.stats), ext(self.node_tree), ext(self.node_gain)
+        if self.node_mask is not None:
+            self.node_mask = ext(self.node_mask)
+        self.cap = new_cap
+
+
+class LevelLoop:
+    """the level loop of the variance trees, shared by GBTClassifier, OneVsRest(GBTClassifier) and the regressors
+    (b200flow/regression.py): every level builds the slots' {Σw, Σw·q, Σw·q2} histograms (gbt_hist_level, in slot groups
+    that keep one level within forest.HIST_BUDGET_BYTES), all-reduces them (exact int64 sums), scores them (gbt_score_level
+    with the grid scales S, S2), grows the pool and partitions the entries to the children.  rq [.][2] holds {q, q2} per
+    unique record; n_iter = T makes it OneVsRest's class-major pool (tree k·T + t reads class k's rq block, and draws the
+    feature subsets of tree t)."""
+
+    def __init__(self, tp, stride, rq, U, F, m, n_bins, feat_bins, feat_kind, S, S2, seed, params, group, stats, n_iter=None):
+        self.tp, self.stride, self.rq, self.U, self.F, self.m, self.n_bins = tp, stride, rq, U, F, m, n_bins
+        self.feat_bins, self.feat_kind, self.S, self.S2, self.seed, self.p = feat_bins, feat_kind, S, S2, seed, params
+        self.group, self.stats, self.n_iter = group, stats, n_iter
+        self.per_slot = m * n_bins * 3
+        self.group_slots = max(1, fr.HIST_BUDGET_BYTES // (self.per_slot * 8))
+
+    def _chunk_table(self, lens, dev):
+        """(device chunk offsets, their host copy) of the slots' entry ranges"""
+        CH = fr.CHUNK_ROWS
+        nch = ((lens + (CH - 1)) // CH).to(torch.int32).contiguous()
+        off = torch.empty(nch.shape[0] + 1, dtype=torch.int64, device=dev)
+        total = torch.zeros(1, dtype=torch.int64, device=dev)
+        call("b200flow_exclusive_scan_i32_to_i64", ptr(nch), nch.shape[0], ptr(off), ptr(total))
+        return off, off.cpu()
+
+    def grow(self, pool, ent, ent2, seg_begin, seg_end, slot_tree):
+        """grow the trees rooted at pool nodes slot_tree (one level-0 slot each, whose entries are ent[seg_begin:seg_end])
+        to the end; -> (ent, ent2), swapped as the partitions left them"""
+        from . import dist as bdist
+        p, dev, m, n_bins, tp, stride, rq = self.p, pool.dev, self.m, self.n_bins, self.tp, self.stride, self.rq
+        per_slot, group_slots, group, ovr, T, CH = self.per_slot, self.group_slots, self.group, self.n_iter is not None, self.n_iter, fr.CHUNK_ROWS
+        n_slots, level = int(slot_tree.numel()), 0
+        slot_nid = torch.ones(n_slots, dtype=torch.int32, device=dev)
+        slot_node = slot_tree.clone()
+        pool.counters[0] = pool.size
+        while n_slots > 0:
+            pool.grow(pool.size + 2 * n_slots)
+            if pool.counters.numel() < 8 + 2 * ((n_slots + 255) // 256):
+                pool.counters = torch.cat([pool.counters, torch.zeros(2 * n_slots, dtype=torch.int64, device=dev)])
+            subset = torch.empty((n_slots, m), dtype=torch.int16, device=dev)
+            # the feature subsets are keyed by the iteration, as in the K separate fits: class k's tree t draws tree t's
+            slot_iter = torch.remainder(slot_tree, T) if ovr else slot_tree
+            call("b200flow_feature_subsets", self.seed, n_slots, ptr(slot_iter), ptr(slot_nid), self.F, m, ptr(subset))
+            slot_class = torch.div(slot_tree, T, rounding_mode="floor") if ovr else None
+            chunk_off, off_h = self._chunk_table(seg_end - seg_begin, dev)
+            n_chunks = int(off_h[-1])
+            split = torch.empty((n_slots, 64), dtype=torch.uint8, device=dev)
+            st = torch.empty((3, n_slots, 3), dtype=torch.int64, device=dev)   # node, left, right
+            for g0 in range(0, n_slots, group_slots):      # slot groups keep one level's histograms within HIST_BUDGET_BYTES
+                g1 = min(n_slots, g0 + group_slots)
+                hist = torch.zeros((g1 - g0) * per_slot, dtype=torch.int64, device=dev)
+                gch = int(off_h[g1] - off_h[g0])
+                if gch > 0:
+                    coff = (chunk_off[g0:g1 + 1] - chunk_off[g0]).contiguous()
+                    if ovr:
+                        _timed("gbt_hist_level", "b200flow_gbt_hist_level_classes", ptr(tp), stride, ptr(ent), ptr(rq), self.U,
+                               ptr(slot_class[g0:g1]), g1 - g0, ptr(seg_begin[g0:g1]), ptr(seg_end[g0:g1]), ptr(coff), gch, CH,
+                               ptr(subset[g0:g1]), m, n_bins, ptr(hist))
+                    else:
+                        _timed("gbt_hist_level", "b200flow_gbt_hist_level", ptr(tp), stride, ptr(ent), ptr(rq), g1 - g0,
+                               ptr(seg_begin[g0:g1]), ptr(seg_end[g0:g1]), ptr(coff), gch, CH, ptr(subset[g0:g1]), m, n_bins,
+                               ptr(hist))
+                if group is not None:                   # the one data-path collective: exact int64 sums
+                    bdist.all_reduce_(hist, group)
+                _timed("gbt_score_level", "b200flow_gbt_score_level", ptr(hist), g1 - g0, ptr(subset[g0:g1]), m, n_bins,
+                       ptr(self.feat_bins), ptr(self.feat_kind), self.S, self.S2, level, p.max_depth, int(p.min_instances_per_node),
+                       float(p.min_info_gain), ptr(split[g0:g1]), ptr(st[0, g0:g1]), ptr(st[1, g0:g1]), ptr(st[2, g0:g1]))
+                del hist
+            next_tree = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
+            next_nid = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
+            next_node = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
+            next_parent = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
+            _timed("grow_level", "b200flow_grow_level", n_slots, ptr(slot_tree), ptr(slot_nid), ptr(slot_node), ptr(split), ptr(st[0]),
+                   ptr(st[1]), ptr(st[2]), 6, ptr(pool.nodes), ptr(pool.node_mask), ptr(pool.stats), ptr(pool.node_tree), pool.cap,
+                   ptr(next_tree), ptr(next_nid), ptr(next_node), ptr(next_parent), None, ptr(pool.counters))
+            pool.node_gain[slot_node.long()] = split.view(torch.float64)[:, 2]
+            cnt = pool.counters[:3].cpu()
+            if int(cnt[2]) != 0:
+                raise B200FlowError("node pool overflow (capacity %d)" % pool.cap)
+            pool.size, n_next = int(cnt[0]), int(cnt[1])
+            self.stats["levels"] += 1; self.stats["slots"] += n_slots
+            if n_next == 0:
+                break
+            cursors = torch.zeros(2 * n_slots, dtype=torch.int32, device=dev)
+            if n_chunks > 0:
+                _timed("partition_level", "b200flow_partition_level", ptr(tp), stride, ptr(ent), ptr(ent2), n_slots, ptr(seg_begin),
+                       ptr(seg_end), ptr(chunk_off), n_chunks, CH, ptr(split), ptr(cursors))
+            next_begin = torch.empty(n_next, dtype=torch.int64, device=dev)
+            next_end = torch.empty(n_next, dtype=torch.int64, device=dev)
+            call("b200flow_next_segments", n_next, None, ptr(next_parent), ptr(seg_begin), ptr(seg_end), ptr(cursors), ptr(next_begin),
+                 ptr(next_end))
+            ent, ent2 = ent2, ent
+            slot_tree, slot_nid, slot_node = next_tree[:n_next], next_nid[:n_next], next_node[:n_next]
+            seg_begin, seg_end = next_begin, next_end
+            n_slots = n_next
+            level += 1
+        return ent, ent2
+
+
 def _fit(src, arity, params, row_offset=0, group=None, n_classes=None):
     """the boosting loop.  n_classes None: the binary problem of the label byte.  n_classes = K: the K problems (label == k)
     side by side — the pool holds K·T trees, class-major (tree k·T + t), margin and rq are [K][U], every iteration's entries
@@ -225,38 +361,13 @@ def _fit(src, arity, params, row_offset=0, group=None, n_classes=None):
              cdf_host.ctypes.data if sub else None, ptr(uid), None, U, ptr(W))
     del uid
 
-    # node pool: roots 0..K·T-1; a node's stats are 3 int64 = the 6 opaque words grow_level copies per node
+    # node pool: roots 0..K·T-1
     TK = K * T
-    cap_nodes = max(1024, TK * min(1 << (p.max_depth + 1), 64))
-    nodes = torch.zeros((cap_nodes, 16), dtype=torch.uint8, device=dev)
-    node_mask = torch.zeros((cap_nodes, 4), dtype=torch.int64, device=dev) if bool((rows.kind > 0).any()) else None
-    stats = torch.zeros((cap_nodes, 3), dtype=torch.int64, device=dev)
-    node_tree = torch.zeros(cap_nodes, dtype=torch.int32, device=dev)
-    node_gain = torch.zeros(cap_nodes, dtype=torch.float64, device=dev)
-    root = np.zeros(TK, NODE_DTYPE); root["feat"] = -1; root["left"] = -1; root["nid"] = 1
-    nodes[:TK] = _lib.h2d(root.view(np.uint8).reshape(TK, 16), dev)
-    node_tree[:TK] = torch.arange(TK, dtype=torch.int32, device=dev)
-    pool_size = TK
-
-    def grow_pool(need):
-        nonlocal nodes, node_mask, stats, node_tree, node_gain, cap_nodes
-        if need <= cap_nodes:
-            return
-        new_cap = cap_nodes
-        while new_cap < need:
-            new_cap *= 2
-        def ext(t):
-            nt = torch.zeros((new_cap,) + tuple(t.shape[1:]), dtype=t.dtype, device=dev)
-            nt[:cap_nodes] = t
-            return nt
-        nodes, stats, node_tree, node_gain = ext(nodes), ext(stats), ext(node_tree), ext(node_gain)
-        if node_mask is not None:
-            node_mask = ext(node_mask)
-        cap_nodes = new_cap
+    pool = NodePool(TK, max(1024, TK * min(1 << (p.max_depth + 1), 64)), bool((rows.kind > 0).any()), dev)
 
     weights = [1.0] + [float(p.step_size)] * (T - 1)
     tree_weight = _lib.h2d(np.asarray(weights * K, np.float64), dev)
-    payload = torch.zeros(cap_nodes, dtype=torch.float64, device=dev)
+    payload = torch.zeros(pool.cap, dtype=torch.float64, device=dev)
     margin = torch.zeros(max(K * U, 1), dtype=torch.float64, device=dev)          # [K][U]
     rq = torch.zeros((max(K * U, 1), 2), dtype=torch.int64, device=dev)           # [K][U][2]: class blocks stay 16-byte aligned
     if ovr:
@@ -270,23 +381,13 @@ def _fit(src, arity, params, row_offset=0, group=None, n_classes=None):
     total = torch.zeros(1, dtype=torch.int64, device=dev)
     ent = torch.empty((max(K * U, 1), 2), dtype=torch.int32, device=dev)        # class k's segment starts at k·U
     ent2 = torch.empty_like(ent)
-    CH = fr.CHUNK_ROWS
     stats_t = dict(levels=0, slots=0, rows=n, unique_rows=U, S=S)
+    loop = LevelLoop(tp, stride, rq, U, F, m, n_bins, feat_bins, feat_kind, S, S2, seed, p, group, stats_t,
+                     n_iter=T if ovr else None)
     if ovr:
         cls_base = torch.arange(K, dtype=torch.int64, device=dev) * U
         cls_root = torch.arange(K, dtype=torch.int32, device=dev) * T
 
-    def chunk_table(lens):
-        """(device chunk offsets, their host copy) of the slots' entry ranges"""
-        nch = ((lens + (CH - 1)) // CH).to(torch.int32).contiguous()
-        off = torch.empty(nch.shape[0] + 1, dtype=torch.int64, device=dev)
-        call("b200flow_exclusive_scan_i32_to_i64", ptr(nch), nch.shape[0], ptr(off), ptr(total))
-        return off, off.cpu()
-
-    per_slot = m * n_bins * 3
-    group_slots = max(1, fr.HIST_BUDGET_BYTES // (per_slot * 8))
-
-    counters = torch.zeros(8 + 2 * 64 + 1024, dtype=torch.int64, device=dev)
     for t in range(T):
         # ---- this iteration's entries {unique record, weight}: the non-zero weights, in unique-id order
         Wt = W[(t if sub else 0) * U:(t if sub else 0) * U + max(U, 1)]
@@ -301,88 +402,24 @@ def _fit(src, arity, params, row_offset=0, group=None, n_classes=None):
             seg_begin = cls_base.clone()
             seg_end = cls_base + total
             slot_tree = cls_root + t
-            slot_nid = torch.ones(K, dtype=torch.int32, device=dev)
-            slot_node = slot_tree.clone()
         else:
             seg_begin = torch.zeros(1, dtype=torch.int64, device=dev)
             seg_end = total.clone()
             slot_tree = torch.full((1,), t, dtype=torch.int32, device=dev)
-            slot_nid = torch.ones(1, dtype=torch.int32, device=dev)
-            slot_node = torch.full((1,), t, dtype=torch.int32, device=dev)
-        counters[0] = pool_size
-        n_slots, level = K, 0
-        while n_slots > 0:
-            grow_pool(pool_size + 2 * n_slots)
-            if counters.numel() < 8 + 2 * ((n_slots + 255) // 256):
-                counters = torch.cat([counters, torch.zeros(2 * n_slots, dtype=torch.int64, device=dev)])
-            subset = torch.empty((n_slots, m), dtype=torch.int16, device=dev)
-            # the feature subsets are keyed by the iteration, as in the K separate fits: class k's tree t draws tree t's
-            slot_iter = torch.remainder(slot_tree, T) if ovr else slot_tree
-            call("b200flow_feature_subsets", seed, n_slots, ptr(slot_iter), ptr(slot_nid), F, m, ptr(subset))
-            slot_class = torch.div(slot_tree, T, rounding_mode="floor") if ovr else None
-            chunk_off, off_h = chunk_table(seg_end - seg_begin)
-            n_chunks = int(off_h[-1])
-            split = torch.empty((n_slots, 64), dtype=torch.uint8, device=dev)
-            st = torch.empty((3, n_slots, 3), dtype=torch.int64, device=dev)   # node, left, right
-            for g0 in range(0, n_slots, group_slots):      # slot groups keep one level's histograms within HIST_BUDGET_BYTES
-                g1 = min(n_slots, g0 + group_slots)
-                hist = torch.zeros((g1 - g0) * per_slot, dtype=torch.int64, device=dev)
-                gch = int(off_h[g1] - off_h[g0])
-                if gch > 0:
-                    coff = (chunk_off[g0:g1 + 1] - chunk_off[g0]).contiguous()
-                    if ovr:
-                        _timed("gbt_hist_level", "b200flow_gbt_hist_level_classes", ptr(tp), stride, ptr(ent), ptr(rq), U,
-                               ptr(slot_class[g0:g1]), g1 - g0, ptr(seg_begin[g0:g1]), ptr(seg_end[g0:g1]), ptr(coff), gch, CH,
-                               ptr(subset[g0:g1]), m, n_bins, ptr(hist))
-                    else:
-                        _timed("gbt_hist_level", "b200flow_gbt_hist_level", ptr(tp), stride, ptr(ent), ptr(rq), g1 - g0,
-                               ptr(seg_begin[g0:g1]), ptr(seg_end[g0:g1]), ptr(coff), gch, CH, ptr(subset[g0:g1]), m, n_bins,
-                               ptr(hist))
-                if group is not None:                   # the one data-path collective: exact int64 sums
-                    bdist.all_reduce_(hist, group)
-                _timed("gbt_score_level", "b200flow_gbt_score_level", ptr(hist), g1 - g0, ptr(subset[g0:g1]), m, n_bins,
-                       ptr(feat_bins), ptr(feat_kind), S, S2, level, p.max_depth, int(p.min_instances_per_node),
-                       float(p.min_info_gain), ptr(split[g0:g1]), ptr(st[0, g0:g1]), ptr(st[1, g0:g1]), ptr(st[2, g0:g1]))
-                del hist
-            next_tree = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
-            next_nid = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
-            next_node = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
-            next_parent = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
-            _timed("grow_level", "b200flow_grow_level", n_slots, ptr(slot_tree), ptr(slot_nid), ptr(slot_node), ptr(split), ptr(st[0]),
-                   ptr(st[1]), ptr(st[2]), 6, ptr(nodes), ptr(node_mask), ptr(stats), ptr(node_tree), cap_nodes, ptr(next_tree),
-                   ptr(next_nid), ptr(next_node), ptr(next_parent), None, ptr(counters))
-            node_gain[slot_node.long()] = split.view(torch.float64)[:, 2]
-            cnt = counters[:3].cpu()
-            if int(cnt[2]) != 0:
-                raise B200FlowError("node pool overflow (capacity %d)" % cap_nodes)
-            pool_size, n_next = int(cnt[0]), int(cnt[1])
-            stats_t["levels"] += 1; stats_t["slots"] += n_slots
-            if n_next == 0:
-                break
-            cursors = torch.zeros(2 * n_slots, dtype=torch.int32, device=dev)
-            if n_chunks > 0:
-                _timed("partition_level", "b200flow_partition_level", ptr(tp), stride, ptr(ent), ptr(ent2), n_slots, ptr(seg_begin),
-                       ptr(seg_end), ptr(chunk_off), n_chunks, CH, ptr(split), ptr(cursors))
-            next_begin = torch.empty(n_next, dtype=torch.int64, device=dev)
-            next_end = torch.empty(n_next, dtype=torch.int64, device=dev)
-            call("b200flow_next_segments", n_next, None, ptr(next_parent), ptr(seg_begin), ptr(seg_end), ptr(cursors), ptr(next_begin),
-                 ptr(next_end))
-            ent, ent2 = ent2, ent
-            slot_tree, slot_nid, slot_node = next_tree[:n_next], next_nid[:n_next], next_node[:n_next]
-            seg_begin, seg_end = next_begin, next_end
-            n_slots = n_next
-            level += 1
+        ent, ent2 = loop.grow(pool, ent, ent2, seg_begin, seg_end, slot_tree)
         # ---- leaf values of the pool so far, then F and the next residuals of every unique record
-        if payload.shape[0] < cap_nodes:
-            payload = torch.zeros(cap_nodes, dtype=torch.float64, device=dev)
-        call("b200flow_gbt_leaf_values", pool_size, ptr(stats), ptr(node_tree), ptr(tree_weight), S, ptr(payload))
+        if payload.shape[0] < pool.cap:
+            payload = torch.zeros(pool.cap, dtype=torch.float64, device=dev)
+        call("b200flow_gbt_leaf_values", pool.size, ptr(pool.stats), ptr(pool.node_tree), ptr(tree_weight), S, ptr(payload))
         if ovr:
-            _timed("gbt_update", "b200flow_gbt_update_classes", ptr(tp), stride, F, U, K, ptr(nodes), ptr(node_mask), ptr(payload),
-                   t, T, S, S2, ptr(margin), ptr(rq))
+            _timed("gbt_update", "b200flow_gbt_update_classes", ptr(tp), stride, F, U, K, ptr(pool.nodes), ptr(pool.node_mask),
+                   ptr(payload), t, T, S, S2, ptr(margin), ptr(rq))
         else:
-            _timed("gbt_update", "b200flow_gbt_update", ptr(tp), stride, F, U, ptr(nodes), ptr(node_mask), ptr(payload), t, S, S2,
-                   ptr(margin), ptr(rq))
+            _timed("gbt_update", "b200flow_gbt_update", ptr(tp), stride, F, U, ptr(pool.nodes), ptr(pool.node_mask), ptr(payload), t,
+                   S, S2, ptr(margin), ptr(rq))
 
+    nodes, node_mask, stats, node_tree, node_gain, pool_size = (pool.nodes, pool.node_mask, pool.stats, pool.node_tree,
+                                                                pool.node_gain, pool.size)
     if ovr:
         return _ovr_model(rows, K, T, weights, S, stats_t, nodes, node_mask, stats, node_tree, node_gain, payload, pool_size,
                           margin, U)

@@ -4,7 +4,12 @@ binary_metrics() sorts the scores of each segment by the CUDA radix sort of csrc
 with integer positive / negative counts, down-samples to numBins points as Spark does and sums the trapezoids of the ROC
 and PR curves sequentially in curve order.  Under torch.distributed each rank reduces its shard to distinct triples, the
 triples are all-gathered and reduced once more, so every rank returns the same bits for any world size.
+
+regression_metrics() (RegressionEvaluator, DESIGN.md §5l) sums its per-row terms exactly in 128-bit fixed point on the
+device (csrc/regression.cu) and rounds each sum once on the host, so it too is the same bits for any world size.
 """
+import math
+
 import numpy as np
 import torch
 
@@ -131,3 +136,89 @@ def binary_metrics(scores, labels=None, pos=None, neg=None, num_bins=1000, group
         N = np.array([cf[s, k[s] - 1] if k[s] else 0 for s in range(S)], np.int64)
         out["P"], out["N"] = (int(P[0]), int(N[0])) if one else (P, N)
     return out
+
+
+# ------------------------------------------------------------------ RegressionEvaluator (DESIGN.md §5l)
+_REG_LIMBS = 4                     # 32-bit limbs of one 128-bit fixed-point sum
+
+
+def _fixed_shift(max_abs, n_global):
+    """grid exponent sh of a term whose all-reduced max |t| is max_abs: rint(t 2^sh) keeps |.| <= 2^(126 - ceil(log2 n)), so
+    the sum of n such integers stays below 2^126; 0 for a term that is zero everywhere"""
+    if not max_abs > 0.0:
+        return 0
+    mnt, e = math.frexp(max_abs)
+    E = e - 1 if mnt == 0.5 else e                       # max_abs <= 2^E
+    return 126 - int(math.ceil(math.log2(max(n_global, 2)))) - E
+
+
+def _fixed_value(limbs, sh):
+    """the double nearest to Σ / 2^sh, from the int64 limb sums [4] of one term (one rounding: int -> float)"""
+    total = sum(int(v) << (32 * j) for j, v in enumerate(limbs))
+    if total == 0:
+        return 0.0
+    try:                                                 # Python's int / int is correctly rounded
+        return total / (1 << sh) if sh >= 0 else float(total * (1 << -sh))
+    except OverflowError:
+        return math.copysign(math.inf, total)
+
+
+def _reg_pass(y, p, mode, mean, n_global, grp):
+    """-> (bad row count, [sum of each term]) over every rank's rows, each sum the double nearest to the exact sum of the
+    terms on their fixed-point grid"""
+    import torch.distributed as dist
+    dev = y.device
+    n = y.shape[0]
+    head = torch.zeros(5, dtype=torch.int64, device=dev)
+    call("b200flow_reg_eval_max", ptr(y), ptr(p), n, mode, float(mean), ptr(head))
+    if grp is not None:
+        bdist.all_reduce_(head, grp, op=dist.ReduceOp.MAX)   # [0] only matters as "any"
+    h = head.cpu().numpy()
+    if h[0]:
+        return 1, None
+    K = 4 if mode == 0 else 2
+    sh = [_fixed_shift(float(h[1 + k:2 + k].view(np.float64)[0]), n_global) for k in range(K)] + [0] * (4 - K)
+    limbs = torch.zeros((4, _REG_LIMBS), dtype=torch.int64, device=dev)
+    call("b200flow_reg_eval_sums", ptr(y), ptr(p), n, mode, float(mean), sh[0], sh[1], sh[2], sh[3], ptr(limbs))
+    if grp is not None:
+        bdist.all_reduce_(limbs, grp)                    # exact: integer sums of the limbs
+    L = limbs.cpu().numpy()
+    return 0, [_fixed_value(L[k], sh[k]) for k in range(K)]
+
+
+def regression_metrics(label, pred, group=None, through_origin=False):
+    """RegressionMetrics of (prediction, label) rows: {'mse', 'rmse', 'mae', 'var', 'r2'}.  Each sum is exact in 128-bit
+    fixed point and rounded once, the label mean comes from one such sum, and (y - ȳ)² / (ŷ - ȳ)² are computed per row in fp64
+    without FMA: the result is the same bits for any world size or shard layout.  A non-finite label or prediction (or a
+    term that overflows) makes every metric NaN; no rows give NaN."""
+    _lib.require_cuda()
+    y = label.to(torch.float64).reshape(-1).contiguous()
+    p = pred.to(torch.float64).reshape(-1).contiguous()
+    if y.shape[0] != p.shape[0]:
+        raise ValueError("%d labels for %d predictions" % (y.shape[0], p.shape[0]))
+    grp = group if group is not None else bdist.group()
+    cnt = torch.tensor([y.shape[0]], dtype=torch.int64, device=y.device)
+    if grp is not None:
+        bdist.all_reduce_(cnt, grp)
+    n = int(cnt.item())
+    nan = float("nan")
+    if n == 0:
+        return dict(mse=nan, rmse=nan, mae=nan, var=nan, r2=nan)
+    if n >= (1 << 31):
+        raise ValueError("RegressionEvaluator: more than 2^31 - 1 rows")
+    bad, s0 = _reg_pass(y, p, 0, 0.0, n, grp)
+    if bad:
+        return dict(mse=nan, rmse=nan, mae=nan, var=nan, r2=nan)
+    sy, syy, sserr, sabs = s0
+    mean = sy / n
+    bad, s1 = _reg_pass(y, p, 1, mean, n, grp)
+    if bad:
+        return dict(mse=nan, rmse=nan, mae=nan, var=nan, r2=nan)
+    sstot, ssreg = s1
+    mse = sserr / n
+    den = syy if through_origin else sstot
+    if den != 0.0:
+        r2 = 1.0 - sserr / den
+    else:                                                # Java double division: 0/0 = NaN, x/0 = inf
+        r2 = nan if sserr == 0.0 else -math.inf
+    return dict(mse=mse, rmse=math.sqrt(mse), mae=sabs / n, var=ssreg / n, r2=r2)

@@ -331,7 +331,7 @@ extern "C" int b200flow_gbt_score_level(const int64_t* hist, int32_t n_slots, co
                                         int32_t max_depth, int32_t min_instances, double min_info_gain, b200flow_split* split,
                                         int64_t* node_stats, int64_t* left_stats, int64_t* right_stats, void* stream) {
     B2F_REQUIRE(hist && subset && feat_bins && feat_kind && split && node_stats && left_stats && right_stats, "gbt_score_level: null pointer");
-    B2F_REQUIRE(m > 0 && n_bins > 0 && n_bins <= 256 && S > 0 && S < 1000 && S2 > 0 && S2 < 1000, "gbt_score_level: bad shape");
+    B2F_REQUIRE(m > 0 && n_bins > 0 && n_bins <= 256 && S > -1000 && S < 1000 && S2 > -1000 && S2 < 1000, "gbt_score_level: bad shape");
     if (n_slots <= 0) return B200FLOW_OK;
     const size_t smem = gbt_score_per_warp(n_bins) * (kGbtScoreThreads / 32);
     cudaError_t e = cudaFuncSetAttribute(gbt_score_level_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);

@@ -2,7 +2,8 @@
 
 MulticlassClassificationEvaluator: confusion counts by the b200flow kernel (R10), metrics per MulticlassMetrics (A.8) +
 macro-F1; logLoss from the probability column.  BinaryClassificationEvaluator: areaUnderROC / areaUnderPR by the device
-sort-and-scan of b200flow.metrics (DESIGN.md §5b).  ClusteringEvaluator: the silhouette of b200flow.kmeans (DESIGN.md §5c)."""
+sort-and-scan of b200flow.metrics (DESIGN.md §5b).  ClusteringEvaluator: the silhouette of b200flow.kmeans (DESIGN.md §5c).
+RegressionEvaluator: exact fixed-point sums of b200flow.metrics.regression_metrics (DESIGN.md §5l)."""
 import math
 
 import torch
@@ -14,7 +15,7 @@ from b200flow import metrics as bm
 from .feature import IllegalArgumentException, _materialize
 from .param import Params
 
-__all__ = ["BinaryClassificationEvaluator", "ClusteringEvaluator", "MulticlassClassificationEvaluator"]
+__all__ = ["BinaryClassificationEvaluator", "ClusteringEvaluator", "MulticlassClassificationEvaluator", "RegressionEvaluator"]
 
 
 class MulticlassClassificationEvaluator(Params):
@@ -187,3 +188,37 @@ class ClusteringEvaluator(Params):
 
     def isLargerBetter(self):
         return True
+
+
+class RegressionEvaluator(Params):
+    """rmse (default) / mse / r2 / mae / var of RegressionMetrics(prediction, label), from sums that are exact in 128-bit
+    fixed point on the device: the same bits for any world size or shard layout.  A non-finite label or prediction makes
+    the metric NaN, and so does an empty dataset.  Deviation from Spark: weightCol is not supported."""
+    _defaults = {"predictionCol": "prediction", "labelCol": "label", "metricName": "rmse", "weightCol": None,
+                 "throughOrigin": False}
+    _metrics = ("rmse", "mse", "r2", "mae", "var")
+
+    def __init__(self, predictionCol=None, labelCol=None, metricName=None, weightCol=None, throughOrigin=None):
+        super().__init__(predictionCol=predictionCol, labelCol=labelCol, metricName=metricName, weightCol=weightCol,
+                         throughOrigin=throughOrigin)
+
+    def _check(self):
+        name = self.getOrDefault("metricName")
+        if name not in self._metrics:
+            raise ValueError("metricName must be one of %s, got %r" % (list(self._metrics), name))
+        if self.getOrDefault("weightCol"):
+            raise NotImplementedError("weightCol is not supported by RegressionEvaluator")
+        return name
+
+    def evaluate(self, dataset, params=None):
+        ev = self.copy(params) if params else self
+        name = ev._check()
+        for c in (ev.getOrDefault("labelCol"), ev.getOrDefault("predictionCol")):
+            if c not in dataset._cols:
+                raise IllegalArgumentException("Field \"%s\" does not exist." % c)
+        pred = dataset._column_tensor(ev.getOrDefault("predictionCol"))
+        lab = dataset._column_tensor(ev.getOrDefault("labelCol"))
+        return bm.regression_metrics(lab, pred, through_origin=bool(ev.getOrDefault("throughOrigin")))[name]
+
+    def isLargerBetter(self):
+        return self.getOrDefault("metricName") in ("r2", "var")
