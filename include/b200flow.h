@@ -632,6 +632,17 @@ int b200flow_reg_leaf_table(int64_t n_nodes, const int64_t* stats, int32_t S, in
                             void* stream);
 /* out[i] = in[i] / d for n_rows doubles, IEEE-rounded (in == out allowed): the forest's prediction, Σ over trees / T */
 int b200flow_reg_divide(const double* in, int64_t n_rows, double d, double* out, void* stream);
+/* GBTRegressor (DESIGN.md §5m).  payload[i] = weight * ((Σw·q 2^-S) / Σw) for the pool nodes i < n_nodes with
+ * node_tree[i] == tree (stats int64 [n_nodes][3]); the other nodes' payloads are left as they are.  -1022 < S < 1022. */
+int b200flow_gbr_leaf_values(int64_t n_nodes, const int64_t* stats, const int32_t* node_tree, int32_t tree, double weight,
+                             int32_t S, double* payload, void* stream);
+/* per unique record u (label y[u], or the 8 bytes at [offset, offset + 8) of its record when y == NULL): tree < 0 sets
+ * margin = +0.0 and resid = y; tree >= 0 walks that tree (root = pool node `tree`), margin += its leaf's payload, and
+ * resid = 2 (y - margin) (loss 0, squared) or (y - margin < 0 ? -1 : +1) (loss 1, absolute).  A NaN resid becomes 0.
+ * max_out int64[1] (caller zeroes) = max |resid| over the records, as its bits. */
+int b200flow_gbr_update(const uint8_t* tp, int32_t tp_stride, int32_t offset, const double* y, int64_t n_rows,
+                        const b200flow_node* nodes, const uint64_t* node_mask, const double* payload, int32_t tree, int32_t loss,
+                        double* margin, double* resid, int64_t* max_out, void* stream);
 /* RegressionEvaluator terms of each row: mode 0 {y, y^2, (y - p)^2, |y - p|}, mode 1 {(y - mean)^2, (p - mean)^2}.
  * out int64[5] (caller zeroes): [0] += rows with a non-finite label, prediction or term, [1 + k] = max |term k| (bits). */
 int b200flow_reg_eval_max(const double* label, const double* pred, int64_t n_rows, int32_t mode, double mean, int64_t* out,

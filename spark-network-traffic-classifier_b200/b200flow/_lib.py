@@ -104,6 +104,8 @@ _SIGNATURES = {
     "b200flow_reg_grid": [_P, _I32, _I32, _P, _I64, _I32, _I32, _I32, _P, _P],
     "b200flow_reg_leaf_table": [_I64, _P, _I32, _I32, _P, _I32, _P],
     "b200flow_reg_divide": [_P, _I64, _F64, _P, _P],
+    "b200flow_gbr_leaf_values": [_I64, _P, _P, _I32, _F64, _I32, _P, _P],
+    "b200flow_gbr_update": [_P, _I32, _I32, _P, _I64, _P, _P, _P, _I32, _I32, _P, _P, _P, _P],
     "b200flow_reg_eval_max": [_P, _P, _I64, _I32, _F64, _P, _P],
     "b200flow_reg_eval_sums": [_P, _P, _I64, _I32, _F64, _I32, _I32, _I32, _I32, _P, _P],
     "b200flow_random_split": [_U64, _I64, _I64, _P, _I32, _P, _P],

@@ -12,6 +12,7 @@
 
 #include "common.cuh"
 #include "portable_exp.h"
+#include "tree_walk.cuh"
 
 namespace b200flow {
 
@@ -230,14 +231,7 @@ __device__ __forceinline__ void gbt_update_record(const uint8_t* rec, double y, 
         *rq = gbt_grid(y, S, S2);
         return;
     }
-    int idx = root;
-    int4 nd = __ldg(nodes + idx);
-    while (nd.x >= 0) {
-        const int bin = rec[nd.x];
-        const int right = nd.y < 65536 ? (bin > nd.y) : !((node_mask[(int64_t)idx * 4 + (bin >> 6)] >> (bin & 63)) & 1ull);
-        idx = nd.z + right;
-        nd = __ldg(nodes + idx);
-    }
+    const int idx = variance_tree_leaf(rec, nodes, node_mask, root);
     const double Fm = *margin + payload[idx];
     *margin = Fm;
     double r = 4.0 * y / (1.0 + portable_exp(2.0 * y * Fm));

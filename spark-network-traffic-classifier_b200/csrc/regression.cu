@@ -7,6 +7,11 @@
 // b200flow_reg_tree_weights gives each tree's total bag weight (the bound behind S and S2); b200flow_reg_grid puts every
 // unique record on the grid; b200flow_reg_leaf_table turns the node stats into leaf values (and the leaf variances).
 //
+// GBTRegressor (DESIGN.md §5m).  The boosting residual has no a-priori bound, so each iteration's grid exponent comes from
+// the all-reduced max |r|: b200flow_gbr_update walks the newest tree, adds its payload to F, writes r = -loss.gradient and
+// folds max |r|; b200flow_reg_grid then puts r on that iteration's grid, and b200flow_gbr_leaf_values computes one tree's
+// payloads with that tree's own scale.
+//
 // Evaluator.  Every sum is exact in 128-bit fixed point: a term t becomes rint(t 2^sh) (sh from the all-reduced max |t|,
 // leaving ceil(log2 n) bits of headroom below 2^126), cut into four 32-bit limbs, and each limb is summed in int64 with
 // integer atomics, so that neither the order of the rows nor the number of ranks can change a bit.
@@ -17,6 +22,7 @@
 
 #include "common.cuh"
 #include "portable_exp.h"
+#include "tree_walk.cuh"
 
 namespace b200flow {
 
@@ -108,6 +114,50 @@ __global__ void reg_leaf_table_kernel(int64_t n_nodes, const long long* __restri
 __global__ void reg_divide_kernel(const double* in, int64_t n, double d, double* out) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) out[i] = in[i] / d;
+}
+
+// ------------------------------------------------------------------ GBTRegressor (DESIGN.md §5m)
+// payload[i] = weight * ((Σw·q s1) / Σw) for the nodes of tree `tree` only: every tree keeps the scale of its own grid
+__global__ void gbr_leaf_values_kernel(int64_t n_nodes, const long long* __restrict__ stats, const int32_t* __restrict__ node_tree,
+                                       int tree, double weight, double s1, double* payload) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_nodes || node_tree[i] != tree) return;
+    payload[i] = weight * (((double)stats[3 * i + 1] * s1) / (double)stats[3 * i]);
+}
+
+// root < 0: F = +0.0 and r = y.  root >= 0: walk the tree rooted at pool node `root`, F += its leaf's payload, then
+// r = -loss.gradient(F, y): squared 2 (y - F), absolute -1 if y - F < 0 else +1.  A NaN r (an empty tree's leaf is 0/0)
+// becomes 0.  out = max |r| over the records, as ordered bits.
+__global__ void gbr_update_kernel(const uint8_t* __restrict__ tp, int stride, int offset, const double* __restrict__ y, int64_t n,
+                                  const int4* __restrict__ nodes, const unsigned long long* __restrict__ node_mask,
+                                  const double* __restrict__ payload, int root, int loss, double* margin, double* resid,
+                                  unsigned long long* out) {
+    unsigned long long mx = 0ull;
+    for (int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; u < n; u += (int64_t)gridDim.x * blockDim.x) {
+        const uint8_t* rec = tp + u * stride;
+        double v;
+        if (y) {
+            v = y[u];
+        } else {
+            uint8_t b[8];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) b[k] = rec[offset + k];
+            memcpy(&v, b, 8);
+        }
+        double Fm = 0.0, r = v;
+        if (root >= 0) {
+            Fm = margin[u] + payload[variance_tree_leaf(rec, nodes, node_mask, root)];
+            const double d = v - Fm;
+            r = loss == 0 ? 2.0 * d : (d < 0.0 ? -1.0 : 1.0);
+        }
+        if (r != r) r = 0.0;
+        margin[u] = Fm;
+        resid[u] = r;
+        mx = max(mx, abs_bits(r));
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mx = max(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+    if (lane_id() == 0 && mx) atomicMax(out, mx);
 }
 
 // ------------------------------------------------------------------ evaluator
@@ -260,6 +310,29 @@ extern "C" int b200flow_reg_divide(const double* in, int64_t n_rows, double d, d
     reg_divide_kernel<<<(unsigned)((n_rows + kRegThreads - 1) / kRegThreads), kRegThreads, 0, (cudaStream_t)stream>>>(in, n_rows, d,
                                                                                                                      out);
     return check_launch("reg_divide");
+}
+
+extern "C" int b200flow_gbr_leaf_values(int64_t n_nodes, const int64_t* stats, const int32_t* node_tree, int32_t tree,
+                                        double weight, int32_t S, double* payload, void* stream) {
+    B2F_REQUIRE(stats && node_tree && payload && tree >= 0, "gbr_leaf_values: bad arguments");
+    B2F_REQUIRE(S > -1022 && S < 1022, "gbr_leaf_values: bad scale %d", S);
+    if (n_nodes <= 0) return B200FLOW_OK;
+    gbr_leaf_values_kernel<<<(unsigned)((n_nodes + kRegThreads - 1) / kRegThreads), kRegThreads, 0, (cudaStream_t)stream>>>(
+        n_nodes, (const long long*)stats, node_tree, tree, weight, ldexp(1.0, -S), payload);
+    return check_launch("gbr_leaf_values");
+}
+
+extern "C" int b200flow_gbr_update(const uint8_t* tp, int32_t tp_stride, int32_t offset, const double* y, int64_t n_rows,
+                                   const b200flow_node* nodes, const uint64_t* node_mask, const double* payload, int32_t tree,
+                                   int32_t loss, double* margin, double* resid, int64_t* max_out, void* stream) {
+    B2F_REQUIRE(max_out && (loss == 0 || loss == 1), "gbr_update: bad arguments");
+    if (n_rows <= 0) return B200FLOW_OK;
+    B2F_REQUIRE(tp && margin && resid && (tree < 0 || (nodes && payload)), "gbr_update: null pointer");
+    B2F_REQUIRE(y || (offset >= 0 && offset + 8 <= tp_stride), "gbr_update: the label bytes do not fit in the record");
+    gbr_update_kernel<<<reg_grid_size(n_rows), kRegThreads, 0, (cudaStream_t)stream>>>(
+        tp, tp_stride, offset, y, n_rows, (const int4*)nodes, (const unsigned long long*)node_mask, payload, tree, loss, margin,
+        resid, (unsigned long long*)max_out);
+    return check_launch("gbr_update");
 }
 
 extern "C" int b200flow_reg_eval_max(const double* label, const double* pred, int64_t n_rows, int32_t mode, double mean,

@@ -1,8 +1,9 @@
-"""pyspark.ml.regression shim: DecisionTreeRegressor and RandomForestRegressor on the device variance-tree loop
-(b200flow/regression.py, csrc/regression.cu, DESIGN.md §5l).  Their models are the same bits for any number of ranks.
+"""pyspark.ml.regression shim: DecisionTreeRegressor, RandomForestRegressor and GBTRegressor on the device variance-tree
+loop (b200flow/regression.py, b200flow/gbt_regression.py, csrc/regression.cu, DESIGN.md §5l, §5m).  Their models are the
+same bits for any number of ranks.
 
-Deviations from Spark: a NaN or infinite label raises IllegalArgumentException (Spark trains on it); labels beyond 2^300
-in magnitude are refused; weightCol is not offered."""
+Deviations from Spark: a NaN or infinite label raises IllegalArgumentException (Spark trains on it); labels (and GBT
+residuals) beyond 2^300 in magnitude are refused; weightCol is not offered."""
 import numpy as np
 import torch
 
@@ -14,7 +15,8 @@ from ..sql import ColumnData
 from .classification import _arity_from_attrs, _default_seed, _lazy_plan
 from .feature import IllegalArgumentException
 
-__all__ = ["DecisionTreeRegressionModel", "DecisionTreeRegressor", "RandomForestRegressionModel", "RandomForestRegressor"]
+__all__ = ["DecisionTreeRegressionModel", "DecisionTreeRegressor", "GBTRegressionModel", "GBTRegressor",
+           "RandomForestRegressionModel", "RandomForestRegressor"]
 
 
 class _TreeRegressorParams:
@@ -155,8 +157,13 @@ class _RegressionModelBase(Model):
                 cols[name] = ColumnData("numeric", val, "f64")
         return df._with(cols=cols)
 
+    def _leaf_values(self, ex):
+        """the value toDebugString prints for each exported node"""
+        return ex["payload"]
+
     def _tree_lines(self, t):
         ex = self._reg.export()
+        vals = self._leaf_values(ex)
         thr = self._reg.forest.thresholds.cpu().numpy()
         sel = np.nonzero(ex["tree"] == t)[0]
         idx = {int(ex["nid"][i]): i for i in sel}
@@ -166,7 +173,7 @@ class _RegressionModelBase(Model):
             i = idx[nid]
             pad = " " * (depth + 1)
             if ex["is_leaf"][i]:
-                lines.append("%sPredict: %r" % (pad, float(ex["payload"][i])))
+                lines.append("%sPredict: %r" % (pad, float(vals[i])))
                 return
             f = int(ex["feat"][i])
             if ex["kind"][i] == 0:
@@ -220,3 +227,96 @@ class RandomForestRegressionModel(_RegressionModelBase, _RandomForestRegressorPa
 
     def __repr__(self):
         return "RandomForestRegressionModel with %d trees" % self._reg.T
+
+
+# ------------------------------------------------------------------------------- gradient-boosted trees
+class _GBTRegressorParams:
+    _defaults = {**{k: v for k, v in _TreeRegressorParams._defaults.items() if k != "varianceCol"},
+                 "maxIter": 20, "stepSize": 0.1, "subsamplingRate": 1.0, "featureSubsetStrategy": "all", "lossType": "squared",
+                 "validationTol": 0.01, "validationIndicatorCol": None, "weightCol": None, "minWeightFractionPerNode": 0.0,
+                 "leafCol": ""}
+
+
+class GBTRegressor(_TreeRegressorBase, _GBTRegressorParams):
+    """Spark 3's GBTRegressor: boosting of regression trees under squared or absolute loss, trained on the device with a
+    residual grid re-derived every iteration (b200flow/gbt_regression.py, DESIGN.md §5m); the model is the same bits for
+    any number of ranks.  Under absolute loss the leaves keep the tree's mean, as Spark's do."""
+
+    def __init__(self, featuresCol=None, labelCol=None, predictionCol=None, maxDepth=None, maxBins=None,
+                 minInstancesPerNode=None, minInfoGain=None, maxMemoryInMB=None, cacheNodeIds=None, checkpointInterval=None,
+                 lossType=None, maxIter=None, stepSize=None, seed=None, subsamplingRate=None, impurity=None,
+                 featureSubsetStrategy=None, validationTol=None, validationIndicatorCol=None, leafCol=None,
+                 minWeightFractionPerNode=None, weightCol=None):
+        kw = dict(locals()); kw.pop("self"); kw.pop("__class__", None)
+        super().__init__(**kw)
+
+    def _params(self):
+        """Spark's param validators, and the params the device trainer does not implement -> GBTRegressorParams"""
+        from b200flow import gbt_regression as bgr
+        g = self.getOrDefault
+        loss = str(g("lossType")).lower()
+        if loss not in bgr.LOSSES:
+            raise IllegalArgumentException("GBTRegressor lossType must be 'squared' or 'absolute', got %r" % (g("lossType"),))
+        if str(g("impurity")).lower() != "variance":
+            raise IllegalArgumentException("GBTRegressor impurity must be 'variance', got %r" % (g("impurity"),))
+        if g("validationIndicatorCol"):
+            raise IllegalArgumentException("validationIndicatorCol (early stopping) is not supported by the b200flow GBT trainer")
+        if g("weightCol"):
+            raise IllegalArgumentException("weightCol is not supported by the b200flow GBT trainer")
+        if float(g("minWeightFractionPerNode")) != 0.0:
+            raise IllegalArgumentException("minWeightFractionPerNode must be 0.0 on the b200flow GBT trainer")
+        it, step, rate = g("maxIter"), float(g("stepSize")), float(g("subsamplingRate"))
+        if int(it) != it or int(it) < 1:
+            raise IllegalArgumentException("maxIter must be an integer >= 1, got %r" % (it,))
+        if not 0.0 < step <= 1.0:
+            raise IllegalArgumentException("stepSize must be in (0, 1], got %r" % (step,))
+        if not 0.0 < rate <= 1.0:
+            raise IllegalArgumentException("subsamplingRate must be in (0, 1], got %r" % (rate,))
+        if int(g("maxBins")) < 2 or int(g("minInstancesPerNode")) < 1 or float(g("minInfoGain")) < 0.0 or int(g("maxDepth")) < 0:
+            raise IllegalArgumentException("maxBins >= 2, minInstancesPerNode >= 1, minInfoGain >= 0 and maxDepth >= 0 are required")
+        strategy = str(g("featureSubsetStrategy"))
+        seed = g("seed")
+        return bgr.GBTRegressorParams(max_iter=int(it), step_size=step, max_depth=int(g("maxDepth")), max_bins=int(g("maxBins")),
+                                      min_instances_per_node=int(g("minInstancesPerNode")), min_info_gain=float(g("minInfoGain")),
+                                      subsampling_rate=rate, feature_subset_strategy="all" if strategy == "auto" else strategy,
+                                      seed=_default_seed(self) if seed is None else int(seed), loss=loss)
+
+    def _fit(self, df):
+        from b200flow import gbt_regression as bgr
+        return self._model(GBTRegressionModel, self._train(df, self._params(), bgr.fit_gbt_regressor))
+
+
+class GBTRegressionModel(_RegressionModelBase, _GBTRegressorParams):
+    @property
+    def getNumTrees(self):
+        return self._reg.T
+
+    @property
+    def treeWeights(self):
+        return list(self._reg.tree_weights)
+
+    def evaluateEachIteration(self, dataset, loss):
+        """the mean loss ('squared' or 'absolute') of the model cut to its first m + 1 trees, for every m: RegressionEvaluator's
+        mse / mae on each prefix model's predictions"""
+        fcol, lcol = self.getOrDefault("featuresCol"), self.getOrDefault("labelCol")
+        for c in (fcol, lcol):
+            if c not in dataset._cols:
+                raise IllegalArgumentException("Field \"%s\" does not exist." % c)
+        if str(loss).lower() not in ("squared", "absolute"):
+            raise IllegalArgumentException("loss must be 'squared' or 'absolute', got %r" % (loss,))
+        y = dataset._column_tensor(lcol).to(torch.float64).reshape(-1).contiguous()
+        return self._reg.evaluate_each_iteration(dataset._cols[fcol].data, y, str(loss).lower(), group=bdist.group())
+
+    def _leaf_values(self, ex):
+        return self._reg.leaf_values(ex)                 # unweighted, in label units, each tree on its own grid
+
+    @property
+    def toDebugString(self):
+        parts = ["GBTRegressionModel with %d trees" % self._reg.T]
+        for t in range(self._reg.T):
+            parts.append("  Tree %d (weight %r):" % (t, self._reg.tree_weights[t]))
+            parts += ["  " + l for l in self._tree_lines(t)[1]]
+        return "\n".join(parts) + "\n"
+
+    def __repr__(self):
+        return "GBTRegressionModel with %d trees" % self._reg.T
