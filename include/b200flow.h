@@ -480,6 +480,24 @@ int b200flow_svc_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, int64
 int b200flow_svc_margins(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, int32_t D, int64_t K,
                          const double* weights, double* raw, void* stream);
 
+/* ------------------------------------------------------------ linear regression ---
+ * LinearRegression, DESIGN.md §5n.  Features x [n_rows][ld] f32 or f64 (converted to f64 first), 1 <= D <= 255; labels y
+ * [n_rows] f64; shift [D] (NULL: no centring) and inv [D] f64; w [D] f64; b_sigma = [b, sigma] f64 (read in huber mode
+ * only), all device.  xs_j = (x_j - shift[j]) * inv[j] (no shift: x_j * inv[j]); m = sum_j xs_j w_j over j ascending.
+ * partials [n_chunks][D + 3] (device; n_chunks = b200flow_group_sums_chunks(row_offset, n_rows)): for each 4096-row global
+ * chunk the rows touch, sums over the chunk's present rows in row order from +0.0 of
+ *   slot 0: the row's loss term, slots 1..D: a xs, slot D + 1: a, slot D + 2: the sigma derivative, where
+ *   B200FLOW_LINREG_SQUARED: d = m - (y - y_shift) y_scale, loss d^2, a = d, sigma derivative 0;
+ *   B200FLOW_LINREG_HUBER: z = (y - m - b) / sigma; |z| <= epsilon: loss sigma + z^2 sigma, a = -2z, derivative 1 - z^2;
+ *     otherwise loss sigma + (2 epsilon |z| - epsilon^2) sigma, a = -2 epsilon sign(z), derivative 1 - epsilon^2.
+ * A chunk's partial depends only on which of its rows are present and on the inputs. */
+#define B200FLOW_LINREG_SQUARED 0
+#define B200FLOW_LINREG_HUBER 1
+int b200flow_linreg_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, int32_t D, const double* y,
+                              const double* shift, const double* inv, double y_shift, double y_scale, const double* w,
+                              const double* b_sigma, double epsilon, int32_t mode, int64_t row_offset, double* partials,
+                              void* stream);
+
 /* ------------------------------------------------------------ factorization machines ---
  * FMClassifier and OneVsRest(FMClassifier), DESIGN.md §5k.  Features x [n_rows][ld] are f32 (x_dtype B200FLOW_F32) or
  * f64 (B200FLOW_F64), converted to f64 before any arithmetic; 1 <= D <= 255, factor_size F >= 1, K >= 1 class columns.

@@ -37,6 +37,8 @@ MAX_D = 256
 # device memory for one batch of chunks' partial rows.  At D = 256 a partial row is 263 KB, so the 897 chunks of 3.67 M rows
 # (236 MB) are summed in batches rather than held at once.
 PARTIALS_BUDGET = 64 << 20
+# device memory for one staged [x, y] batch of the labelled Gram matrix (LinearRegression's normal equations)
+STAGE_BUDGET = 256 << 20
 
 
 class PCAFit:
@@ -97,10 +99,14 @@ def column_sums(x, sh):
     return grouped_sum(x, None, 1, sh)[0].reshape(-1)
 
 
-def centered_gram_total(x, mean, sh):
+def centered_gram_total(x, mean, sh, y=None, y_mean=None):
     """[D(D+1)/2] f64 device: the packed upper triangle of sum (x - mean)(x - mean)^T over every rank's rows in chunk
     order (mean device f64 [D] or None); the same bits on every rank.  The chunks are computed in batches of at most
-    PARTIALS_BUDGET bytes of partial rows."""
+    PARTIALS_BUDGET bytes of partial rows.  With a label y [n] f64 (and y_mean, a float), the Gram matrix is that of the
+    rows [x, y] shifted by [mean, y_mean], [(D+1)(D+2)/2]: each batch is staged as an f64 [rows, D + 1] matrix of at most
+    STAGE_BUDGET bytes (x may then be f32)."""
+    if y is not None:
+        return _labelled_gram_total(x, mean, y, y_mean, sh)
     D = x.shape[1]
     P = D * (D + 1) // 2
     lead, off = sh.lead[sh.rank], sh.offs[sh.rank]
@@ -114,6 +120,43 @@ def centered_gram_total(x, mean, sh):
         nc = (xs.shape[0] + bdist.CHUNK - 1) // bdist.CHUNK
         parts = torch.empty((nc, P), dtype=torch.float64, device=x.device)
         centered_gram(xs, mean, go, parts)
+        return parts, nc
+
+    if not pieces:
+        return bdist.chunk_chain(torch.empty((1, P), dtype=torch.float64, device=x.device), 0, 1, P, sh).reshape(-1)
+    first, nc = run(*pieces[0])
+    return bdist.chunk_chain(first, nc, 1, P, sh, more=(run(*p) for p in pieces[1:])).reshape(-1)
+
+
+def stage_rows(D):
+    """rows of one staged [x, y] batch of _labelled_gram_total: whole chunks within STAGE_BUDGET and PARTIALS_BUDGET"""
+    P = (D + 1) * (D + 2) // 2
+    nb = max(1, min(PARTIALS_BUDGET // (8 * P), STAGE_BUDGET // (8 * (D + 1) * bdist.CHUNK)))
+    return nb * bdist.CHUNK
+
+
+def _labelled_gram_total(x, mean, y, y_mean, sh):
+    """centered_gram_total of the rows [x, y] shifted by [mean, y_mean], staged batch by batch"""
+    D = x.shape[1]
+    W = D + 1
+    P = W * (W + 1) // 2
+    lead, off = sh.lead[sh.rank], sh.offs[sh.rank]
+    t0, tail_x, _ = bdist.chunk_tail(x, None, sh)
+    tail_y = bdist.chunk_tail(y.reshape(-1, 1), None, sh)[1].reshape(-1)
+    step = stage_rows(D)
+    pieces = [(x[s:min(s + step, t0)], y[s:min(s + step, t0)], off + s) for s in range(lead, t0, step)]
+    if tail_x.shape[0]:
+        pieces.append((tail_x, tail_y, off + t0))
+    shift = torch.cat([mean.to(torch.float64).reshape(-1),
+                       torch.tensor([float(y_mean)], dtype=torch.float64, device=x.device)]).contiguous()
+
+    def run(xs, ys, go):
+        xy = torch.empty((xs.shape[0], W), dtype=torch.float64, device=x.device)
+        xy[:, :D] = xs
+        xy[:, D] = ys
+        nc = (go + xs.shape[0] - 1) // bdist.CHUNK - go // bdist.CHUNK + 1
+        parts = torch.empty((nc, P), dtype=torch.float64, device=x.device)
+        centered_gram(xy, shift, go, parts)
         return parts, nc
 
     if not pieces:

@@ -1,6 +1,7 @@
 """pyspark.ml.regression shim: DecisionTreeRegressor, RandomForestRegressor and GBTRegressor on the device variance-tree
-loop (b200flow/regression.py, b200flow/gbt_regression.py, csrc/regression.cu, DESIGN.md §5l, §5m).  Their models are the
-same bits for any number of ranks.
+loop (b200flow/regression.py, b200flow/gbt_regression.py, csrc/regression.cu, DESIGN.md §5l, §5m), and LinearRegression
+on the normal equations and the fused least-squares / Huber kernel (b200flow/linreg.py, csrc/linreg.cu, DESIGN.md §5n).
+Their models are the same bits for any number of ranks.
 
 Deviations from Spark: a NaN or infinite label raises IllegalArgumentException (Spark trains on it); labels (and GBT
 residuals) beyond 2^300 in magnitude are refused; weightCol is not offered."""
@@ -16,7 +17,8 @@ from .classification import _arity_from_attrs, _default_seed, _lazy_plan
 from .feature import IllegalArgumentException
 
 __all__ = ["DecisionTreeRegressionModel", "DecisionTreeRegressor", "GBTRegressionModel", "GBTRegressor",
-           "RandomForestRegressionModel", "RandomForestRegressor"]
+           "LinearRegression", "LinearRegressionModel", "LinearRegressionSummary", "LinearRegressionTrainingSummary",
+           "RandomForestRegressionModel", "RandomForestRegressor", "UnsupportedOperationException"]
 
 
 class _TreeRegressorParams:
@@ -27,6 +29,18 @@ class _TreeRegressorParams:
 
 class _RandomForestRegressorParams(_TreeRegressorParams):
     _defaults = {"numTrees": 20, "featureSubsetStrategy": "auto", "subsamplingRate": 1.0}
+
+
+def _features_and_label(est, df):
+    """(the features column, the label as a contiguous f64 tensor) of a regressor's input, after Spark's column checks"""
+    fcol, lcol = est.getOrDefault("featuresCol"), est.getOrDefault("labelCol")
+    for c in (fcol, lcol):
+        if c not in df._cols:
+            raise IllegalArgumentException("Field \"%s\" does not exist." % c)
+    fc = df._cols[fcol]
+    if fc.kind != "vector":
+        raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+    return fc, df._column_tensor(lcol).to(torch.float64).reshape(-1).contiguous()
 
 
 class _TreeRegressorBase(Estimator):
@@ -50,15 +64,8 @@ class _TreeRegressorBase(Estimator):
                                   seed=_default_seed(self) if seed is None else int(seed), bootstrap=bootstrap)
 
     def _train(self, df, params, fit):
-        fcol, lcol = self.getOrDefault("featuresCol"), self.getOrDefault("labelCol")
-        for c in (fcol, lcol):
-            if c not in df._cols:
-                raise IllegalArgumentException("Field \"%s\" does not exist." % c)
-        fc = df._cols[fcol]
-        if fc.kind != "vector":
-            raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+        fc, y = _features_and_label(self, df)
         x = fc.data                         # a lazy VectorAssembler column is assembled here, once
-        y = df._column_tensor(lcol).to(torch.float64).reshape(-1).contiguous()
         try:
             grp = bdist.group()
             off, _ = bdist.global_offset(x.shape[0], x.device, grp)
@@ -320,3 +327,186 @@ class GBTRegressionModel(_RegressionModelBase, _GBTRegressorParams):
 
     def __repr__(self):
         return "GBTRegressionModel with %d trees" % self._reg.T
+
+
+# ------------------------------------------------------------------------------- linear regression
+class UnsupportedOperationException(RuntimeError):
+    pass
+
+
+class _LinearRegressionParams:
+    _defaults = {"featuresCol": "features", "labelCol": "label", "predictionCol": "prediction", "maxIter": 100,
+                 "regParam": 0.0, "elasticNetParam": 0.0, "tol": 1e-6, "fitIntercept": True, "standardization": True,
+                 "solver": "auto", "loss": "squaredError", "epsilon": 1.35, "aggregationDepth": 2,
+                 "maxBlockSizeInMB": 0.0, "weightCol": None}
+
+
+class LinearRegression(Estimator, _LinearRegressionParams):
+    """Spark 3's LinearRegression [recalled]: squared loss through the normal equations (solver auto or normal) or L-BFGS /
+    OWL-QN, and Huber loss through L-BFGS, on the device (b200flow/linreg.py, DESIGN.md §5n).  aggregationDepth and
+    maxBlockSizeInMB are validated but do not change the result: the sums have one fixed order.  weightCol raises."""
+
+    def __init__(self, featuresCol=None, labelCol=None, predictionCol=None, maxIter=None, regParam=None,
+                 elasticNetParam=None, tol=None, fitIntercept=None, standardization=None, solver=None, weightCol=None,
+                 aggregationDepth=None, loss=None, epsilon=None, maxBlockSizeInMB=None):
+        kw = dict(locals()); kw.pop("self"); kw.pop("__class__", None)
+        super().__init__(**kw)
+
+    def _check(self):
+        """Spark's param validators, and the refusal of weightCol -> b200flow.linreg.LinRegParams"""
+        from b200flow import linreg as blr
+        g = self.getOrDefault
+        it, depth = g("maxIter"), g("aggregationDepth")
+        if isinstance(it, bool) or int(it) != it or int(it) < 0:
+            raise IllegalArgumentException("maxIter must be an integer >= 0, got %r" % (it,))
+        if isinstance(depth, bool) or int(depth) != depth or int(depth) < 2:
+            raise IllegalArgumentException("aggregationDepth must be an integer >= 2, got %r" % (depth,))
+        if not float(g("maxBlockSizeInMB")) >= 0:
+            raise IllegalArgumentException("maxBlockSizeInMB must be >= 0, got %r" % (g("maxBlockSizeInMB"),))
+        if g("weightCol"):
+            raise IllegalArgumentException("weightCol is not supported by the b200flow LinearRegression")
+        p = blr.LinRegParams(max_iter=int(it), reg_param=float(g("regParam")), elastic_net_param=float(g("elasticNetParam")),
+                             tol=float(g("tol")), fit_intercept=bool(g("fitIntercept")),
+                             standardization=bool(g("standardization")), solver=g("solver"), loss=g("loss"),
+                             epsilon=float(g("epsilon")))
+        try:
+            blr.check_params(p)
+        except ValueError as e:
+            raise IllegalArgumentException(str(e))
+        return p
+
+    def _fit(self, df):
+        from b200flow import linreg as blr
+        p = self._check()
+        fc, y = _features_and_label(self, df)
+        x = fc.data
+        try:
+            grp = bdist.group()
+            off, _ = bdist.global_offset(x.shape[0], x.device, grp)
+            fit = blr.linreg_fit(x, y, p, row_offset=off, group=grp)
+        except ValueError as e:        # includes b200flow's UnsupportedParamError; CUDA failures propagate as they are
+            raise IllegalArgumentException(str(e))
+        m = LinearRegressionModel(fit)
+        m._paramMap = {k: v for k, v in self._paramMap.items() if k in m._all_defaults()}
+        m._training = df
+        return m
+
+
+class LinearRegressionModel(Model, _LinearRegressionParams):
+    """coefficients (original feature scale), intercept and scale (Huber's sigma, 1.0 for squared loss); prediction =
+    x . coefficients + intercept."""
+
+    def __init__(self, fit):
+        super().__init__()
+        self._fit_result = fit             # b200flow.linreg.LinRegFit
+        self._training = None
+        self._summary = None
+
+    @property
+    def coefficients(self):
+        from .linalg import DenseVector
+        return DenseVector(self._fit_result.coef.copy())
+
+    @property
+    def intercept(self):
+        return self._fit_result.intercept
+
+    @property
+    def scale(self):
+        return self._fit_result.scale
+
+    @property
+    def numFeatures(self):
+        return int(self._fit_result.coef.shape[0])
+
+    @property
+    def hasSummary(self):
+        return self._training is not None
+
+    @property
+    def summary(self):
+        if self._training is None:
+            raise RuntimeError("No training summary available for this LinearRegressionModel")
+        if self._summary is None:
+            self._summary = LinearRegressionTrainingSummary(self, self._training)
+        return self._summary
+
+    def evaluate(self, dataset):
+        """a LinearRegressionSummary of the model on another dataset"""
+        return LinearRegressionSummary(self, dataset)
+
+    def _transform(self, df):
+        from b200flow import linreg as blr
+        fcol = self.getOrDefault("featuresCol")
+        if fcol not in df._cols or df._cols[fcol].kind != "vector":
+            raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+        pcol = self.getOrDefault("predictionCol")
+        if not pcol:
+            return df
+        if pcol in df._cols:
+            raise IllegalArgumentException("Output column %s already exists." % pcol)
+        try:
+            pred = blr.linreg_predict(df._cols[fcol].data, self._fit_result)
+        except ValueError as e:
+            raise IllegalArgumentException(str(e))
+        cols = dict(df._cols)
+        cols[pcol] = ColumnData("numeric", pred, "f64")
+        return df._with(cols=cols)
+
+    def __repr__(self):
+        return "LinearRegressionModel: uid=%s, numFeatures=%d" % (self.uid, self.numFeatures)
+
+
+class LinearRegressionSummary:
+    """Spark 3's LinearRegressionSummary [recalled]: the metrics of RegressionMetrics (through the origin without an
+    intercept), r2adj, residuals, degrees of freedom, the residual range, and the coefficient standard errors, t values
+    and p values of the Cholesky path (the intercept last)."""
+
+    def __init__(self, model, dataset):
+        from b200flow import linreg as blr
+        self._model = model
+        self.predictionCol = model.getOrDefault("predictionCol") or "prediction"
+        self.labelCol, self.featuresCol = model.getOrDefault("labelCol"), model.getOrDefault("featuresCol")
+        fc, y = _features_and_label(model, dataset)
+        fit = model._fit_result
+        self._s = blr.summarize(fc.data, y, fit, bool(model.getOrDefault("fitIntercept")), group=bdist.group())
+        cols = dict(dataset._cols)
+        cols[self.predictionCol] = ColumnData("numeric", self._s.predictions, "f64")
+        self.predictions = dataset._with(cols=cols)
+
+    explainedVariance = property(lambda self: self._s.explained_variance)
+    meanAbsoluteError = property(lambda self: self._s.mae)
+    meanSquaredError = property(lambda self: self._s.mse)
+    rootMeanSquaredError = property(lambda self: self._s.rmse)
+    r2 = property(lambda self: self._s.r2)
+    r2adj = property(lambda self: self._s.r2adj)
+    numInstances = property(lambda self: self._s.num_instances)
+    degreesOfFreedom = property(lambda self: self._s.degrees_of_freedom)
+    devianceResiduals = property(lambda self: list(self._s.deviance_residuals))
+
+    @property
+    def residuals(self):
+        """a frame with one column, residuals = label - prediction"""
+        return self.predictions._with(cols={"residuals": ColumnData("numeric", self._s.residuals, "f64")})
+
+    def _coefficient_stat(self, name):
+        v = getattr(self._s, name)
+        if v is None:
+            raise UnsupportedOperationException("No Std. Error of coefficients available for this LinearRegressionModel")
+        return [float(t) for t in v]
+
+    coefficientStandardErrors = property(lambda self: self._coefficient_stat("std_errors"))
+    tValues = property(lambda self: self._coefficient_stat("t_values"))
+    pValues = property(lambda self: self._coefficient_stat("p_values"))
+
+
+class LinearRegressionTrainingSummary(LinearRegressionSummary):
+    """the summary of the training rows, with the optimiser's objective history"""
+
+    @property
+    def objectiveHistory(self):
+        return list(self._model._fit_result.objective_history)
+
+    @property
+    def totalIterations(self):
+        return len(self._model._fit_result.objective_history) - 1
