@@ -498,6 +498,45 @@ int b200flow_linreg_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, in
                               const double* b_sigma, double epsilon, int32_t mode, int64_t row_offset, double* partials,
                               void* stream);
 
+/* ------------------------------------------------------------ generalized linear regression ---
+ * GeneralizedLinearRegression, DESIGN.md §5o.  Features x [n_rows][ld] f32 or f64 (converted to f64 first), 1 <= D <= 255;
+ * labels y, prior weights `weight` and offsets `offset` [n_rows] f64 (weight NULL: 1.0, offset NULL: 0.0); coef [D] f64; all
+ * device.  family / link are the codes below; variance_power is tweedie's V(mu) = mu^p, link_power the power link's
+ * (0: log).  Rows [0, n_rows) are global rows row_offset + i.  With m = x . coef (eight lane sums over j = s mod 8 in
+ * ascending j, combined ((p0 + p4) + (p2 + p6)) + ((p1 + p5) + (p3 + p7))), eta = (m + intercept) + offset and
+ * mu = project(unlink(eta)):
+ *   B200FLOW_GLM_INIT: z = link(initialize(y, weight)) - offset, w = weight; rows_out [n_rows][2] = (z, w);
+ *   B200FLOW_GLM_REWEIGHT: z = (eta - offset) + (y - mu) g'(mu), w = weight / (g'(mu)^2 V(mu)); rows_out = (z, w);
+ *     partials [n_chunks][D + 2] of both: sum w, sum w x_j (j < D), sum w z;
+ *   B200FLOW_GLM_SUMMARY (coef NULL: mu = mu_const, eta = link(mu) for every row): rows_out NULL or [n_rows][4] = the
+ *     deviance, pearson, working and response residuals; partials [n_chunks][8] = sum weight, sum weight y, the deviance,
+ *     the squared pearson residuals, the AIC log-likelihood terms, and for gamma sum weight log y, sum weight y / mu and
+ *     sum weight log mu (0 otherwise);
+ *   B200FLOW_GLM_PREDICT: rows_out [n_rows][2] = (mu, eta); y, weight and partials are not read.
+ * n_chunks = b200flow_group_sums_chunks(row_offset, n_rows); each partial sums the chunk's present rows in row order from
+ * +0.0, so it depends only on which of its rows are present and on the inputs. */
+#define B200FLOW_GLM_GAUSSIAN 0
+#define B200FLOW_GLM_BINOMIAL 1
+#define B200FLOW_GLM_POISSON 2
+#define B200FLOW_GLM_GAMMA 3
+#define B200FLOW_GLM_TWEEDIE 4
+#define B200FLOW_GLM_IDENTITY 0
+#define B200FLOW_GLM_LOG 1
+#define B200FLOW_GLM_INVERSE 2
+#define B200FLOW_GLM_LOGIT 3
+#define B200FLOW_GLM_PROBIT 4
+#define B200FLOW_GLM_CLOGLOG 5
+#define B200FLOW_GLM_SQRT 6
+#define B200FLOW_GLM_POWER 7
+#define B200FLOW_GLM_INIT 0
+#define B200FLOW_GLM_REWEIGHT 1
+#define B200FLOW_GLM_SUMMARY 2
+#define B200FLOW_GLM_PREDICT 3
+int b200flow_glm_rows(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, int32_t D, const double* y,
+                      const double* weight, const double* offset, const double* coef, double intercept, double mu_const,
+                      int32_t family, int32_t link, double variance_power, double link_power, int32_t mode,
+                      int64_t row_offset, double* rows_out, double* partials, void* stream);
+
 /* ------------------------------------------------------------ factorization machines ---
  * FMClassifier and OneVsRest(FMClassifier), DESIGN.md §5k.  Features x [n_rows][ld] are f32 (x_dtype B200FLOW_F32) or
  * f64 (B200FLOW_F64), converted to f64 before any arithmetic; 1 <= D <= 255, factor_size F >= 1, K >= 1 class columns.
@@ -552,6 +591,11 @@ int b200flow_gmm_moments(const double* x, int64_t n_rows, int32_t D, int64_t ld,
  * only on which of its rows are present. */
 int b200flow_centered_gram(const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* shift, int64_t row_offset,
                            double* partials, void* stream);
+/* b200flow_weighted_centered_gram: as b200flow_centered_gram with a row weight w [n_rows] f64: the packed upper triangle
+ * of (X - shift)^T W (X - shift), each staged (x_b - shift_b) multiplied by its row's weight as the contraction loads it
+ * (GeneralizedLinearRegression's IRLS, DESIGN.md §5o). */
+int b200flow_weighted_centered_gram(const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* shift,
+                                    const double* w, int64_t row_offset, double* partials, void* stream);
 /* b200flow_pca_project: out [n_rows][k] = x pc, pc [D][k] row-major, 1 <= k <= 256; out[i][j] accumulates x[i][a] pc[a][j]
  * over a in ascending order (fp64 tensor cores), so a row's output depends on that row and pc alone, not on its position. */
 int b200flow_pca_project(const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* pc, int32_t k, double* out,

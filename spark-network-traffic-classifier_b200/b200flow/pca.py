@@ -99,14 +99,21 @@ def column_sums(x, sh):
     return grouped_sum(x, None, 1, sh)[0].reshape(-1)
 
 
-def centered_gram_total(x, mean, sh, y=None, y_mean=None):
+def weighted_centered_gram(x, shift, w, row_offset, partials):
+    """b200flow_weighted_centered_gram on the rows x [n, D] with row weights w [n] (device f64): shift device f64 [D]."""
+    n, D = x.shape
+    call("b200flow_weighted_centered_gram", ptr(x), n, D, D, ptr(shift), ptr(w), row_offset, ptr(partials))
+
+
+def centered_gram_total(x, mean, sh, y=None, y_mean=None, w=None):
     """[D(D+1)/2] f64 device: the packed upper triangle of sum (x - mean)(x - mean)^T over every rank's rows in chunk
     order (mean device f64 [D] or None); the same bits on every rank.  The chunks are computed in batches of at most
     PARTIALS_BUDGET bytes of partial rows.  With a label y [n] f64 (and y_mean, a float), the Gram matrix is that of the
     rows [x, y] shifted by [mean, y_mean], [(D+1)(D+2)/2]: each batch is staged as an f64 [rows, D + 1] matrix of at most
-    STAGE_BUDGET bytes (x may then be f32)."""
+    STAGE_BUDGET bytes (x may then be f32).  With a row weight w [n] f64 as well, it is sum w (a - shift)(a - shift)^T over
+    those rows (GeneralizedLinearRegression's IRLS); w travels with y."""
     if y is not None:
-        return _labelled_gram_total(x, mean, y, y_mean, sh)
+        return _labelled_gram_total(x, mean, y, y_mean, sh, w)
     D = x.shape[1]
     P = D * (D + 1) // 2
     lead, off = sh.lead[sh.rank], sh.offs[sh.rank]
@@ -135,28 +142,33 @@ def stage_rows(D):
     return nb * bdist.CHUNK
 
 
-def _labelled_gram_total(x, mean, y, y_mean, sh):
-    """centered_gram_total of the rows [x, y] shifted by [mean, y_mean], staged batch by batch"""
+def _labelled_gram_total(x, mean, y, y_mean, sh, w=None):
+    """centered_gram_total of the rows [x, y] shifted by [mean, y_mean] (weighted by w when given), staged batch by batch"""
     D = x.shape[1]
     W = D + 1
     P = W * (W + 1) // 2
     lead, off = sh.lead[sh.rank], sh.offs[sh.rank]
     t0, tail_x, _ = bdist.chunk_tail(x, None, sh)
     tail_y = bdist.chunk_tail(y.reshape(-1, 1), None, sh)[1].reshape(-1)
+    tail_w = bdist.chunk_tail(w.reshape(-1, 1), None, sh)[1].reshape(-1).contiguous() if w is not None else None
     step = stage_rows(D)
-    pieces = [(x[s:min(s + step, t0)], y[s:min(s + step, t0)], off + s) for s in range(lead, t0, step)]
+    cut = lambda t, s: t[s:min(s + step, t0)] if t is not None else None          # noqa: E731
+    pieces = [(x[s:min(s + step, t0)], y[s:min(s + step, t0)], cut(w, s), off + s) for s in range(lead, t0, step)]
     if tail_x.shape[0]:
-        pieces.append((tail_x, tail_y, off + t0))
+        pieces.append((tail_x, tail_y, tail_w, off + t0))
     shift = torch.cat([mean.to(torch.float64).reshape(-1),
                        torch.tensor([float(y_mean)], dtype=torch.float64, device=x.device)]).contiguous()
 
-    def run(xs, ys, go):
+    def run(xs, ys, ws, go):
         xy = torch.empty((xs.shape[0], W), dtype=torch.float64, device=x.device)
         xy[:, :D] = xs
         xy[:, D] = ys
         nc = (go + xs.shape[0] - 1) // bdist.CHUNK - go // bdist.CHUNK + 1
         parts = torch.empty((nc, P), dtype=torch.float64, device=x.device)
-        centered_gram(xy, shift, go, parts)
+        if ws is None:
+            centered_gram(xy, shift, go, parts)
+        else:
+            weighted_centered_gram(xy, shift, ws, go, parts)
         return parts, nc
 
     if not pieces:

@@ -10,6 +10,9 @@
 // four 8x8 MMA tiles that share two A and two B fragments per 4 rows.  A pass holds 8 x 8 blocks in registers (block j of
 // the pass belongs to warp j % 8, slot j / 8) and contracts them over the chunk's tiles, 4 rows per MMA; passes repeat
 // until every block is done (one pass up to D = 176, three at D = 256).
+// b200flow_weighted_centered_gram is the Weighted instantiation: the tile's row weights are staged beside it (0 outside
+// [0, n)) and every B fragment (x_b − shift_b of one row) is multiplied by its row's weight as it is loaded, so the
+// contraction is (X − shift)ᵀ W (X − shift) in the same order.  The unweighted instantiation is the same code as before.
 //
 // b200flow_pca_project: one CTA per 1024 rows walks 32-row tiles.  The tile's x (Dp = ceil8(D) columns) is staged once; pc
 // sits in shared memory in slabs of 64 columns: the only slab stays for the whole CTA when k <= 64, otherwise the slabs
@@ -31,13 +34,16 @@ constexpr int kProjSlab = 64;                     // columns of pc per shared-me
 
 __host__ __device__ inline int pad16(int v) { return (v + 15) / 16 * 16; }
 
+template <bool Weighted>
 __global__ void __launch_bounds__(kPcaThreads, 1) centered_gram_kernel(const double* __restrict__ x, int64_t n, int64_t ld, int D,
                                                                       const double* __restrict__ shift, int64_t row_offset,
-                                                                      double* __restrict__ partials) {
+                                                                      double* __restrict__ partials,
+                                                                      const double* __restrict__ w) {
     extern __shared__ double sm[];
     const int Dq = pad16(D), pitch = Dq + 4, nb = Dq / 16, B = nb * (nb + 1) / 2;    // pitch 4 mod 8: 2-wavefront fragment loads
     double* xs = sm;                              // [kPcaTile][pitch]
     double* ss = xs + kPcaTile * pitch;           // [Dq]
+    double* wt = ss + Dq;                         // [kPcaTile]: the tile's row weights (Weighted only)
     const int lane = lane_id(), warp = warp_id(), qr = lane >> 2, qc = lane & 3;
     const int64_t c0 = (row_offset / kChunkRows + blockIdx.x) * kChunkRows - row_offset;   // local index of the chunk's row 0
     const int64_t lo = c0 > 0 ? c0 : 0, hi = c0 + kChunkRows < n ? c0 + kChunkRows : n;
@@ -63,6 +69,12 @@ __global__ void __launch_bounds__(kPcaThreads, 1) centered_gram_kernel(const dou
                 const int64_t gr = base + r;
                 xs[r * pitch + j] = gr >= 0 && gr < n && j < D ? x[gr * ld + j] - ss[j] : 0.0;
             }
+            if constexpr (Weighted) {
+                if (threadIdx.x < kPcaTile) {
+                    const int64_t gr = base + threadIdx.x;
+                    wt[threadIdx.x] = gr >= 0 && gr < n ? w[gr] : 0.0;
+                }
+            }
             __syncthreads();
 #pragma unroll
             for (int q = 0; q < kPcaSlots; ++q) {
@@ -72,7 +84,13 @@ __global__ void __launch_bounds__(kPcaThreads, 1) centered_gram_kernel(const dou
 #pragma unroll 4
                     for (int kk = 0; kk < kPcaTile / 4; ++kk) {
                         const int o = kk * 4 * pitch;
-                        const double al = pa[o], ah = pa[o + 8], bl = pb[o], bh = pb[o + 8];
+                        const double al = pa[o], ah = pa[o + 8];
+                        double bl = pb[o], bh = pb[o + 8];
+                        if constexpr (Weighted) {
+                            const double wr = wt[kk * 4 + qc];    // the B fragment's row: kk * 4 + qc
+                            bl = bl * wr;
+                            bh = bh * wr;
+                        }
                         dmma(acc[q][0], al, bl);
                         dmma(acc[q][1], al, bh);
                         dmma(acc[q][2], ah, bl);
@@ -154,19 +172,35 @@ __global__ void __launch_bounds__(kPcaThreads, 4) pca_project_kernel(const doubl
 
 using namespace b200flow;
 
-extern "C" int b200flow_centered_gram(const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* shift,
-                                      int64_t row_offset, double* partials, void* stream) {
-    B2F_REQUIRE(D >= 1 && D <= kPcaMaxD, "centered_gram: 1 <= D <= %d", kPcaMaxD);
-    B2F_REQUIRE(n_rows >= 0 && row_offset >= 0 && ld >= D, "centered_gram: n >= 0, row_offset >= 0, ld >= D");
+namespace {
+
+template <bool Weighted>
+int launch_centered_gram(const char* what, const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* shift,
+                         const double* w, int64_t row_offset, double* partials, void* stream) {
+    B2F_REQUIRE(D >= 1 && D <= kPcaMaxD, "%s: 1 <= D <= %d", what, kPcaMaxD);
+    B2F_REQUIRE(n_rows >= 0 && row_offset >= 0 && ld >= D, "%s: n >= 0, row_offset >= 0, ld >= D", what);
     if (n_rows == 0) return B200FLOW_OK;
     const int64_t nc = (row_offset + n_rows - 1) / kChunkRows - row_offset / kChunkRows + 1;
-    B2F_REQUIRE(nc <= 0x7fffffffll, "centered_gram: too many rows");
-    B2F_REQUIRE(x && partials, "centered_gram: null pointer");
+    B2F_REQUIRE(nc <= 0x7fffffffll, "%s: too many rows", what);
+    B2F_REQUIRE(x && partials && (w || !Weighted), "%s: null pointer", what);
     const int Dq = pad16(D);
-    const size_t smem = ((size_t)kPcaTile * (Dq + 4) + Dq) * sizeof(double);
-    cudaFuncSetAttribute(centered_gram_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    centered_gram_kernel<<<(unsigned)nc, kPcaThreads, smem, (cudaStream_t)stream>>>(x, n_rows, ld, D, shift, row_offset, partials);
-    return check_launch("centered_gram");
+    const size_t smem = ((size_t)kPcaTile * (Dq + 4) + Dq + (Weighted ? kPcaTile : 0)) * sizeof(double);
+    cudaFuncSetAttribute(centered_gram_kernel<Weighted>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    centered_gram_kernel<Weighted><<<(unsigned)nc, kPcaThreads, smem, (cudaStream_t)stream>>>(x, n_rows, ld, D, shift,
+                                                                                              row_offset, partials, w);
+    return check_launch(what);
+}
+
+}  // namespace
+
+extern "C" int b200flow_centered_gram(const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* shift,
+                                      int64_t row_offset, double* partials, void* stream) {
+    return launch_centered_gram<false>("centered_gram", x, n_rows, D, ld, shift, nullptr, row_offset, partials, stream);
+}
+
+extern "C" int b200flow_weighted_centered_gram(const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* shift,
+                                               const double* w, int64_t row_offset, double* partials, void* stream) {
+    return launch_centered_gram<true>("weighted_centered_gram", x, n_rows, D, ld, shift, w, row_offset, partials, stream);
 }
 
 extern "C" int b200flow_pca_project(const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* pc, int32_t k,

@@ -1,10 +1,12 @@
 """pyspark.ml.regression shim: DecisionTreeRegressor, RandomForestRegressor and GBTRegressor on the device variance-tree
 loop (b200flow/regression.py, b200flow/gbt_regression.py, csrc/regression.cu, DESIGN.md §5l, §5m), and LinearRegression
-on the normal equations and the fused least-squares / Huber kernel (b200flow/linreg.py, csrc/linreg.cu, DESIGN.md §5n).
+on the normal equations and the fused least-squares / Huber kernel (b200flow/linreg.py, csrc/linreg.cu, DESIGN.md §5n),
+and GeneralizedLinearRegression by IRLS on the per-row GLM kernel and the weighted Gram kernel (b200flow/glm.py,
+csrc/glm.cu, DESIGN.md §5o).
 Their models are the same bits for any number of ranks.
 
 Deviations from Spark: a NaN or infinite label raises IllegalArgumentException (Spark trains on it); labels (and GBT
-residuals) beyond 2^300 in magnitude are refused; weightCol is not offered."""
+residuals) beyond 2^300 in magnitude are refused; weightCol is not offered except by GeneralizedLinearRegression."""
 import numpy as np
 import torch
 
@@ -17,6 +19,8 @@ from .classification import _arity_from_attrs, _default_seed, _lazy_plan
 from .feature import IllegalArgumentException
 
 __all__ = ["DecisionTreeRegressionModel", "DecisionTreeRegressor", "GBTRegressionModel", "GBTRegressor",
+           "GeneralizedLinearRegression", "GeneralizedLinearRegressionModel", "GeneralizedLinearRegressionSummary",
+           "GeneralizedLinearRegressionTrainingSummary",
            "LinearRegression", "LinearRegressionModel", "LinearRegressionSummary", "LinearRegressionTrainingSummary",
            "RandomForestRegressionModel", "RandomForestRegressor", "UnsupportedOperationException"]
 
@@ -510,3 +514,204 @@ class LinearRegressionTrainingSummary(LinearRegressionSummary):
     @property
     def totalIterations(self):
         return len(self._model._fit_result.objective_history) - 1
+
+
+# ------------------------------------------------------------------------------- generalized linear regression
+class _GLRParams:
+    _defaults = {"featuresCol": "features", "labelCol": "label", "predictionCol": "prediction", "family": "gaussian",
+                 "link": None, "variancePower": 0.0, "linkPower": None, "fitIntercept": True, "maxIter": 25, "tol": 1e-6,
+                 "regParam": 0.0, "solver": "irls", "aggregationDepth": 2, "weightCol": None, "offsetCol": None,
+                 "linkPredictionCol": None}
+
+
+def _glr_params(est):
+    """Spark's param validators -> b200flow.glm.GLMParams"""
+    from b200flow import glm as bg
+    g = est.getOrDefault
+    it, depth = g("maxIter"), g("aggregationDepth")
+    if isinstance(it, bool) or int(it) != it or int(it) < 0:
+        raise IllegalArgumentException("maxIter must be an integer >= 0, got %r" % (it,))
+    if isinstance(depth, bool) or int(depth) != depth or int(depth) < 2:
+        raise IllegalArgumentException("aggregationDepth must be an integer >= 2, got %r" % (depth,))
+    p = bg.GLMParams(family=g("family"), link=g("link"), variance_power=float(g("variancePower")),
+                     link_power=g("linkPower"), fit_intercept=bool(g("fitIntercept")), max_iter=int(it),
+                     tol=float(g("tol")), reg_param=float(g("regParam")), solver=g("solver"))
+    try:
+        bg.check_params(p)
+    except ValueError as e:
+        raise IllegalArgumentException(str(e))
+    return p
+
+
+def _glr_columns(est, df):
+    """(features, label, weight or None, offset or None) of a frame, after Spark's column checks"""
+    fc, y = _features_and_label(est, df)
+    extra = []
+    for name in ("weightCol", "offsetCol"):
+        c = est.getOrDefault(name)
+        if c and c not in df._cols:
+            raise IllegalArgumentException("Field \"%s\" does not exist." % c)
+        extra.append(df._column_tensor(c).to(torch.float64).reshape(-1).contiguous() if c else None)
+    return fc, y, extra[0], extra[1]
+
+
+class GeneralizedLinearRegression(Estimator, _GLRParams):
+    """Spark 3's GeneralizedLinearRegression [recalled]: gaussian, binomial, poisson, gamma and tweedie families fitted by
+    IRLS on the device (b200flow/glm.py, csrc/glm.cu, DESIGN.md §5o).  aggregationDepth is validated but does not change
+    the result: the sums have one fixed order."""
+
+    def __init__(self, labelCol=None, featuresCol=None, predictionCol=None, family=None, link=None, fitIntercept=None,
+                 maxIter=None, tol=None, regParam=None, weightCol=None, solver=None, linkPredictionCol=None,
+                 variancePower=None, linkPower=None, offsetCol=None, aggregationDepth=None):
+        kw = dict(locals()); kw.pop("self"); kw.pop("__class__", None)
+        super().__init__(**kw)
+
+    def _fit(self, df):
+        from b200flow import glm as bg
+        p = _glr_params(self)
+        fc, y, w, off = _glr_columns(self, df)
+        x = fc.data
+        try:
+            grp = bdist.group()
+            ro, _ = bdist.global_offset(x.shape[0], x.device, grp)
+            fit = bg.glm_fit(x, y, p, weight=w, offset=off, row_offset=ro, group=grp)
+        except ValueError as e:        # includes b200flow's UnsupportedParamError; CUDA failures propagate as they are
+            raise IllegalArgumentException(str(e))
+        m = GeneralizedLinearRegressionModel(fit)
+        m._paramMap = {k: v for k, v in self._paramMap.items() if k in m._all_defaults()}
+        m._training = df
+        return m
+
+
+class GeneralizedLinearRegressionModel(Model, _GLRParams):
+    """coefficients and intercept; prediction = linkInv(x . coefficients + intercept + offset), and with
+    linkPredictionCol the linear predictor as well."""
+
+    def __init__(self, fit):
+        super().__init__()
+        self._fit_result = fit             # b200flow.glm.GLMFit
+        self._training = None
+        self._summary = None
+
+    @property
+    def coefficients(self):
+        from .linalg import DenseVector
+        return DenseVector(self._fit_result.coef.copy())
+
+    @property
+    def intercept(self):
+        return self._fit_result.intercept
+
+    @property
+    def numFeatures(self):
+        return int(self._fit_result.coef.shape[0])
+
+    @property
+    def hasSummary(self):
+        return self._training is not None
+
+    @property
+    def summary(self):
+        if self._training is None:
+            raise RuntimeError("No training summary available for this GeneralizedLinearRegressionModel")
+        if self._summary is None:
+            self._summary = GeneralizedLinearRegressionTrainingSummary(self, self._training)
+        return self._summary
+
+    def evaluate(self, dataset):
+        """a GeneralizedLinearRegressionSummary of the model on another dataset"""
+        return GeneralizedLinearRegressionSummary(self, dataset)
+
+    def _transform(self, df):
+        from b200flow import glm as bg
+        fcol = self.getOrDefault("featuresCol")
+        if fcol not in df._cols or df._cols[fcol].kind != "vector":
+            raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+        pcol, lcol, ocol = (self.getOrDefault(k) for k in ("predictionCol", "linkPredictionCol", "offsetCol"))
+        outs = [c for c in (pcol, lcol) if c]
+        if not outs:
+            return df
+        for c in outs:
+            if c in df._cols:
+                raise IllegalArgumentException("Output column %s already exists." % c)
+        if ocol and ocol not in df._cols:
+            raise IllegalArgumentException("Field \"%s\" does not exist." % ocol)
+        off = df._column_tensor(ocol).to(torch.float64).reshape(-1).contiguous() if ocol else None
+        try:
+            me = bg.glm_predict(df._cols[fcol].data, self._fit_result, off)
+        except ValueError as e:
+            raise IllegalArgumentException(str(e))
+        cols = dict(df._cols)
+        if pcol:
+            cols[pcol] = ColumnData("numeric", me[:, 0].contiguous(), "f64")
+        if lcol:
+            cols[lcol] = ColumnData("numeric", me[:, 1].contiguous(), "f64")
+        return df._with(cols=cols)
+
+    def __repr__(self):
+        return "GeneralizedLinearRegressionModel: uid=%s, family=%s, link=%s, numFeatures=%d" % (
+            self.uid, self.getOrDefault("family"), self.getOrDefault("link"), self.numFeatures)
+
+
+class GeneralizedLinearRegressionSummary:
+    """Spark 3's GeneralizedLinearRegressionSummary [recalled]: predictions, counts and degrees of freedom, deviance,
+    nullDeviance, dispersion, aic (tweedie raises) and residuals(residualsType)."""
+
+    def __init__(self, model, dataset):
+        from b200flow import glm as bg
+        self._model = model
+        self.predictionCol = model.getOrDefault("predictionCol") or "prediction"
+        fc, y, w, off = _glr_columns(model, dataset)
+        try:
+            self._s = bg.summarize(fc.data, y, model._fit_result, _glr_params(model), weight=w, offset=off,
+                                   group=bdist.group())
+        except ValueError as e:
+            raise IllegalArgumentException(str(e))
+        cols = dict(dataset._cols)
+        cols[self.predictionCol] = ColumnData("numeric", self._s.predictions[:, 0].contiguous(), "f64")
+        lcol = model.getOrDefault("linkPredictionCol")
+        if lcol:
+            cols[lcol] = ColumnData("numeric", self._s.predictions[:, 1].contiguous(), "f64")
+        self.predictions = dataset._with(cols=cols)
+
+    numInstances = property(lambda self: self._s.num_instances)
+    rank = property(lambda self: self._s.rank)
+    degreesOfFreedom = property(lambda self: self._s.degrees_of_freedom)
+    residualDegreeOfFreedom = property(lambda self: self._s.residual_dof)
+    residualDegreeOfFreedomNull = property(lambda self: self._s.residual_dof_null)
+    deviance = property(lambda self: self._s.deviance)
+    nullDeviance = property(lambda self: self._s.null_deviance)
+    dispersion = property(lambda self: self._s.dispersion)
+
+    @property
+    def aic(self):
+        if self._s.aic is None:
+            raise UnsupportedOperationException("No AIC available for the tweedie family")
+        return self._s.aic
+
+    def residuals(self, residualsType="deviance"):
+        """a frame with one column, <type>Residuals"""
+        from b200flow import glm as bg
+        t = str(residualsType).lower()
+        if t not in bg.RESIDUALS:
+            raise IllegalArgumentException("residualsType must be one of %s, got %r" % (list(bg.RESIDUALS), residualsType))
+        col = self._s.residuals[:, bg.RESIDUALS.index(t)].contiguous()
+        return self.predictions._with(cols={t + "Residuals": ColumnData("numeric", col, "f64")})
+
+
+class GeneralizedLinearRegressionTrainingSummary(GeneralizedLinearRegressionSummary):
+    """the summary of the training rows, with the IRLS iteration count and the coefficient statistics"""
+
+    numIterations = property(lambda self: self._model._fit_result.iterations)
+    solver = property(lambda self: "irls")
+
+    def _coefficient_stat(self, name):
+        v = getattr(self._s, name)
+        if v is None:
+            raise UnsupportedOperationException("No Std. Error of coefficients available for this "
+                                                "GeneralizedLinearRegressionModel")
+        return [float(t) for t in v]
+
+    coefficientStandardErrors = property(lambda self: self._coefficient_stat("std_errors"))
+    tValues = property(lambda self: self._coefficient_stat("t_values"))
+    pValues = property(lambda self: self._coefficient_stat("p_values"))
