@@ -537,6 +537,28 @@ int b200flow_glm_rows(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld
                       int32_t family, int32_t link, double variance_power, double link_power, int32_t mode,
                       int64_t row_offset, double* rows_out, double* partials, void* stream);
 
+/* ------------------------------------------------------------ isotonic regression ---
+ * IsotonicRegression, DESIGN.md §5p.  Row i (0 <= i < n < 2^32) is (label[i * label_stride], feature[i * feature_stride],
+ * weight[i * weight_stride]) with the feature f32 (B200FLOW_F32) or f64 (B200FLOW_F64) and label / weight f64 (weight
+ * NULL: 1.0), all device.  checks int64 [2] (device) = the rows with a non-finite label, feature or weight, and the rows
+ * with a negative weight; the fit is only meaningful when both are 0.  Rows with weight 0 are dropped.  isotonic == 0 fits
+ * an antitonic model (labels negated, then the predictions).  Writes the model, *n_out (device int64) increasing
+ * boundaries and their predictions, into boundaries / predictions [n] (device f64); an empty input gives *n_out = 0.
+ * The model is Spark's one-partition result (makeUnique, PAV, compress, PAV again) with PAV run as a chunked merge tree:
+ * chunk 0 takes the library's chunk size, any other value (<= 2^30) forces that one.  The bits depend only on the rows, in
+ * order, and on the chunk size.
+ * scratch: device, 256-byte aligned, b200flow_isotonic_scratch(n) bytes (host-only query, no device needed).
+ * b200flow_isotonic_predict: out[i] = the model's prediction at x[i * stride] (f32 or f64): java.util.Arrays.binarySearch
+ * over the K >= 1 boundaries, the first or last prediction outside them, the hit's on a hit, else
+ * y1 + (y2 - y1) * (x - x1) / (x2 - x1).  A NaN x predicts the last prediction. */
+int b200flow_isotonic_scratch(int64_t n, int64_t* scratch_bytes);
+int b200flow_isotonic_fit(const void* feature, int32_t feature_dtype, int64_t feature_stride, const double* label,
+                          int64_t label_stride, const double* weight, int64_t weight_stride, int64_t n, int32_t isotonic,
+                          int64_t chunk, void* scratch, int64_t scratch_bytes, double* boundaries, double* predictions,
+                          int64_t* n_out, int64_t* checks, void* stream);
+int b200flow_isotonic_predict(const void* x, int32_t x_dtype, int64_t stride, int64_t n, const double* boundaries,
+                              const double* predictions, int64_t K, double* out, void* stream);
+
 /* ------------------------------------------------------------ factorization machines ---
  * FMClassifier and OneVsRest(FMClassifier), DESIGN.md §5k.  Features x [n_rows][ld] are f32 (x_dtype B200FLOW_F32) or
  * f64 (B200FLOW_F64), converted to f64 before any arithmetic; 1 <= D <= 255, factor_size F >= 1, K >= 1 class columns.

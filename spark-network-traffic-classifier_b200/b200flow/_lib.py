@@ -85,6 +85,8 @@ _SIGNATURES = {
     "b200flow_linreg_loss_grad": [_P, _I32, _I64, _I64, _I32, _P, _P, _P, _F64, _F64, _P, _P, _F64, _I32, _I64, _P, _P],
     "b200flow_glm_rows": [_P, _I32, _I64, _I64, _I32, _P, _P, _P, _P, _F64, _F64, _I32, _I32, _F64, _F64, _I32, _I64, _P, _P,
                           _P],
+    "b200flow_isotonic_fit": [_P, _I32, _I64, _P, _I64, _P, _I64, _I64, _I32, _I64, _P, _I64, _P, _P, _P, _P, _P],
+    "b200flow_isotonic_predict": [_P, _I32, _I64, _I64, _P, _P, _I64, _P, _P],
     "b200flow_fm_loss_grad": [_P, _I32, _I64, _I64, _I32, _I32, _P, _P, _I64, _P, _F64, _U64, _I64, _P, _P],
     "b200flow_fm_raw": [_P, _I32, _I64, _I64, _I32, _I32, _I64, _P, _P, _P],
     "b200flow_gmm_estep": [_P, _I64, _I32, _I64, _I32, _P, _P, _P, _I64, _P, _P, _P, _P],
@@ -123,7 +125,8 @@ _SIGNATURES = {
 EXPORTS = sorted(list(_SIGNATURES) + ["b200flow_last_error", "b200flow_version", "b200flow_route_hist_config",
                                        "b200flow_packed_layout", "b200flow_binary_counts_scratch",
                                        "b200flow_group_sums_chunks", "b200flow_mlp_config",
-                                       "b200flow_svc_config", "b200flow_fm_config"])
+                                       "b200flow_svc_config", "b200flow_fm_config",
+                                       "b200flow_isotonic_scratch"])
 
 _lib = None
 launches = 0   # kernels of OURS launched so far (counted per C-ABI call); bench.py reads the delta over the timed region
@@ -159,6 +162,8 @@ def load():
         lib.b200flow_svc_config.restype = C.c_int
         lib.b200flow_fm_config.argtypes = [_I32, _I32, _I64, C.POINTER(_I32), C.POINTER(_I32), C.POINTER(_I64)]
         lib.b200flow_fm_config.restype = C.c_int
+        lib.b200flow_isotonic_scratch.argtypes = [_I64, C.POINTER(_I64)]
+        lib.b200flow_isotonic_scratch.restype = C.c_int
         _lib = lib
     return _lib
 
@@ -189,6 +194,15 @@ def binary_counts_scratch(S, n):
     lib = load()
     if lib.b200flow_binary_counts_scratch(int(S), int(n), C.byref(out)) != 0:
         raise B200FlowError("b200flow_binary_counts_scratch failed: %s" % lib.b200flow_last_error().decode())
+    return int(out.value)
+
+
+def isotonic_scratch(n):
+    """bytes of device scratch b200flow_isotonic_fit needs for n rows (host-only call)."""
+    out = _I64(0)
+    lib = load()
+    if lib.b200flow_isotonic_scratch(int(n), C.byref(out)) != 0:
+        raise B200FlowError("b200flow_isotonic_scratch failed: %s" % lib.b200flow_last_error().decode())
     return int(out.value)
 
 

@@ -8,14 +8,10 @@
 //
 // b200flow_binary_curve: the distinct triples -> the binned curve points (Spark's numBins rule) and the two trapezoid
 // areas, each summed sequentially from 0.0 in curve order (Spark's AreaUnderCurve on one partition).
-#include "common.cuh"
+#include "radix_sort.cuh"
 
 namespace b200flow {
 
-constexpr int kSortThreads = 256;
-constexpr int kSortItems = 16;                                   // items per thread and pass
-constexpr int kSortTile = kSortThreads * kSortItems;             // 4096 items per block and pass
-constexpr int kSortWarps = kSortThreads / 32;
 constexpr unsigned long long kInvalidKey = ~0ull;                // NaN scores and zero-count items: sorted last, never a run
 
 // descending order of x as an ascending uint64: -0.0 is +0.0; the only key equal to kInvalidKey is a NaN's
@@ -47,77 +43,6 @@ __global__ void __launch_bounds__(256) bc_keys_kernel(const double* __restrict__
     }
     nan_local = warp_sum(nan_local);
     if (lane_id() == 0 && nan_local) atomicAdd(n_nan, nan_local);
-}
-
-// digit of item p in this pass: key bits, or (seg_pass) bits of the segment id of the item's original index
-template <bool kSegPass>
-__device__ __forceinline__ int sort_digit(unsigned long long k, uint32_t id, int shift, int64_t n) {
-    if (kSegPass) return (int)(((uint64_t)id / (uint64_t)n) >> shift) & 255;
-    return (int)(k >> shift) & 255;
-}
-
-// per-block digit counts, digit-major: hist[d * nb + b] (a scan over it gives every (digit, block) its first output slot)
-template <bool kSegPass>
-__global__ void __launch_bounds__(kSortThreads) radix_hist_kernel(const unsigned long long* __restrict__ key,
-                                                                  const uint32_t* __restrict__ idx, int64_t M, int64_t n,
-                                                                  int shift, int32_t* hist) {
-    __shared__ int cnt[256];
-    cnt[threadIdx.x] = 0;
-    __syncthreads();
-    const int64_t base = (int64_t)blockIdx.x * kSortTile;
-#pragma unroll 4
-    for (int k = 0; k < kSortItems; ++k) {
-        const int64_t p = base + (int64_t)k * kSortThreads + threadIdx.x;
-        if (p < M) atomicAdd(&cnt[sort_digit<kSegPass>(kSegPass ? 0ull : key[p], kSegPass ? idx[p] : 0u, shift, n)], 1);
-    }
-    __syncthreads();
-    hist[(int64_t)threadIdx.x * gridDim.x + blockIdx.x] = cnt[threadIdx.x];
-}
-
-// stable scatter of one pass.  Warp w owns items [w*512, (w+1)*512) of the block's tile, 32 at a time in order; lanes with
-// equal digits find each other with __match_any_sync and rank by lane, and a per-warp digit counter in shared memory
-// carries the rank across rounds.  Warp bases per digit follow from the counters, block bases from the global scan.
-template <bool kSegPass>
-__global__ void __launch_bounds__(kSortThreads) radix_scatter_kernel(const unsigned long long* __restrict__ key,
-                                                                     const uint32_t* __restrict__ idx, int64_t M, int64_t n,
-                                                                     int shift, const int64_t* __restrict__ offs,
-                                                                     unsigned long long* key_out, uint32_t* idx_out) {
-    __shared__ int cnt[kSortWarps][257];                         // digit 256: items past the end
-    __shared__ int64_t wbase[kSortWarps][256];
-    const int w = warp_id(), lane = lane_id();
-    for (int i = threadIdx.x; i < kSortWarps * 257; i += kSortThreads) (&cnt[0][0])[i] = 0;
-    __syncthreads();
-    const unsigned lt = (1u << lane) - 1u;
-    const int64_t base = (int64_t)blockIdx.x * kSortTile + (int64_t)w * (kSortTile / kSortWarps);
-    unsigned long long k[kSortItems]; uint32_t id[kSortItems]; int dg[kSortItems], rk[kSortItems];
-#pragma unroll
-    for (int r = 0; r < kSortItems; ++r) {
-        const int64_t p = base + r * 32 + lane;
-        const bool live = p < M;
-        k[r] = live ? key[p] : 0ull;
-        id[r] = live ? idx[p] : 0u;
-        dg[r] = live ? sort_digit<kSegPass>(k[r], id[r], shift, n) : 256;
-        const unsigned peers = __match_any_sync(0xffffffffu, dg[r]);
-        const int before = cnt[w][dg[r]];
-        __syncwarp();
-        if ((peers & lt) == 0) cnt[w][dg[r]] = before + __popc(peers);      // the lowest lane of each digit group
-        __syncwarp();
-        rk[r] = before + __popc(peers & lt);
-    }
-    __syncthreads();
-    {
-        const int d = threadIdx.x;                                   // kSortThreads == 256 digits
-        int64_t run = offs[(int64_t)d * gridDim.x + blockIdx.x];
-        for (int ww = 0; ww < kSortWarps; ++ww) { wbase[ww][d] = run; run += cnt[ww][d]; }
-    }
-    __syncthreads();
-#pragma unroll
-    for (int r = 0; r < kSortItems; ++r) {
-        if (dg[r] == 256) continue;
-        const int64_t q = wbase[w][dg[r]] + rk[r];
-        key_out[q] = k[r];
-        idx_out[q] = id[r];
-    }
 }
 
 // after the sort: run heads, and each item's counts in sorted order (0 for NaN / zero-count items)
@@ -262,7 +187,7 @@ static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 static CountsScratch counts_layout(int32_t S, int64_t n) {
     CountsScratch L;
     L.M = (int64_t)S * n;
-    L.nb = (L.M + kSortTile - 1) / kSortTile;
+    L.nb = radix_blocks(L.M);
     size_t o = 0;
     auto take = [&](size_t bytes) { const size_t at = o; o += align256(bytes); return at; };
     L.key0 = take(8 * L.M); L.key1 = take(8 * L.M);
@@ -317,12 +242,9 @@ extern "C" int b200flow_binary_counts(const double* scores, int64_t score_stride
     for (int pass = 0; pass < 8 + seg_passes; ++pass) {
         const bool seg = pass >= 8;
         const int shift = seg ? 8 * (pass - 8) : 8 * pass;
-        if (seg) radix_hist_kernel<true><<<(unsigned)L.nb, kSortThreads, 0, st>>>(key[cur], idx[cur], M, n, shift, hist);
-        else radix_hist_kernel<false><<<(unsigned)L.nb, kSortThreads, 0, st>>>(key[cur], idx[cur], M, n, shift, hist);
-        int rc = b200flow_exclusive_scan_i32_to_i64(hist, 256 * L.nb, offs, nullptr, stream);
+        const int rc = seg ? radix_pass<true>(key[cur], idx[cur], M, n, shift, hist, offs, key[cur ^ 1], idx[cur ^ 1], stream)
+                           : radix_pass<false>(key[cur], idx[cur], M, n, shift, hist, offs, key[cur ^ 1], idx[cur ^ 1], stream);
         if (rc) return rc;
-        if (seg) radix_scatter_kernel<true><<<(unsigned)L.nb, kSortThreads, 0, st>>>(key[cur], idx[cur], M, n, shift, offs, key[cur ^ 1], idx[cur ^ 1]);
-        else radix_scatter_kernel<false><<<(unsigned)L.nb, kSortThreads, 0, st>>>(key[cur], idx[cur], M, n, shift, offs, key[cur ^ 1], idx[cur ^ 1]);
         cur ^= 1;
     }
     bc_heads_kernel<<<grid, 256, 0, st>>>(key[cur], idx[cur], pos, neg, count_stride, n, M, head, pos_s, neg_s);

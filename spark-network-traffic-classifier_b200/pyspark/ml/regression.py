@@ -1,12 +1,15 @@
 """pyspark.ml.regression shim: DecisionTreeRegressor, RandomForestRegressor and GBTRegressor on the device variance-tree
 loop (b200flow/regression.py, b200flow/gbt_regression.py, csrc/regression.cu, DESIGN.md §5l, §5m), and LinearRegression
 on the normal equations and the fused least-squares / Huber kernel (b200flow/linreg.py, csrc/linreg.cu, DESIGN.md §5n),
-and GeneralizedLinearRegression by IRLS on the per-row GLM kernel and the weighted Gram kernel (b200flow/glm.py,
-csrc/glm.cu, DESIGN.md §5o).
+GeneralizedLinearRegression by IRLS on the per-row GLM kernel and the weighted Gram kernel (b200flow/glm.py,
+csrc/glm.cu, DESIGN.md §5o), and IsotonicRegression on a device sort and a chunked pool-adjacent-violators merge
+(b200flow/isotonic.py, csrc/isotonic.cu, DESIGN.md §5p).
 Their models are the same bits for any number of ranks.
 
 Deviations from Spark: a NaN or infinite label raises IllegalArgumentException (Spark trains on it); labels (and GBT
-residuals) beyond 2^300 in magnitude are refused; weightCol is not offered except by GeneralizedLinearRegression."""
+residuals) beyond 2^300 in magnitude are refused; weightCol is not offered except by GeneralizedLinearRegression and
+IsotonicRegression.  IsotonicRegression also refuses a non-finite feature or weight at fit time, and its empty model (every
+weight 0) raises IllegalArgumentException where Spark throws NoSuchElementException."""
 import numpy as np
 import torch
 
@@ -20,7 +23,7 @@ from .feature import IllegalArgumentException
 
 __all__ = ["DecisionTreeRegressionModel", "DecisionTreeRegressor", "GBTRegressionModel", "GBTRegressor",
            "GeneralizedLinearRegression", "GeneralizedLinearRegressionModel", "GeneralizedLinearRegressionSummary",
-           "GeneralizedLinearRegressionTrainingSummary",
+           "GeneralizedLinearRegressionTrainingSummary", "IsotonicRegression", "IsotonicRegressionModel",
            "LinearRegression", "LinearRegressionModel", "LinearRegressionSummary", "LinearRegressionTrainingSummary",
            "RandomForestRegressionModel", "RandomForestRegressor", "UnsupportedOperationException"]
 
@@ -715,3 +718,108 @@ class GeneralizedLinearRegressionTrainingSummary(GeneralizedLinearRegressionSumm
     coefficientStandardErrors = property(lambda self: self._coefficient_stat("std_errors"))
     tValues = property(lambda self: self._coefficient_stat("t_values"))
     pValues = property(lambda self: self._coefficient_stat("p_values"))
+
+
+# ------------------------------------------------------------------------------- isotonic regression
+class _IsotonicRegressionParams:
+    _defaults = {"featuresCol": "features", "labelCol": "label", "predictionCol": "prediction", "weightCol": None,
+                 "isotonic": True, "featureIndex": 0}
+
+
+def _isotonic_feature(est, df):
+    """the feature as one value per row: featuresCol itself when numeric, its element featureIndex when a vector (a strided
+    view, f32 or f64)"""
+    fcol = est.getOrDefault("featuresCol")
+    if fcol not in df._cols:
+        raise IllegalArgumentException("Field \"%s\" does not exist." % fcol)
+    k = est.getOrDefault("featureIndex")
+    if isinstance(k, bool) or int(k) != k or int(k) < 0:
+        raise IllegalArgumentException("%s parameter featureIndex given invalid value %r." % (est.uid, k))
+    c = df._cols[fcol]
+    if c.kind == "vector":
+        x = c.data
+        if int(k) >= x.shape[1]:
+            raise IllegalArgumentException("featureIndex %d is out of range for the %d-element vectors of column %s"
+                                           % (int(k), x.shape[1], fcol))
+        return x[:, int(k)]
+    x = df._column_tensor(fcol)
+    return x if x.dtype in (torch.float32, torch.float64) else x.to(torch.float64)
+
+
+class IsotonicRegression(Estimator, _IsotonicRegressionParams):
+    """Spark 3's IsotonicRegression [recalled]: the weighted isotonic (or antitonic) least-squares fit of the label on one
+    feature by pool-adjacent-violators, on the device (b200flow/isotonic.py, csrc/isotonic.cu, DESIGN.md §5p).  The model
+    is the same bits for any world size; it equals Spark's sequential PAV to rounding.  A NaN or infinite label, feature or
+    weight raises IllegalArgumentException."""
+
+    def __init__(self, featuresCol=None, labelCol=None, predictionCol=None, weightCol=None, isotonic=None,
+                 featureIndex=None):
+        kw = dict(locals()); kw.pop("self"); kw.pop("__class__", None)
+        super().__init__(**kw)
+
+    def _fit(self, df):
+        from b200flow import isotonic as biso
+        x = _isotonic_feature(self, df)
+        lcol, wcol = self.getOrDefault("labelCol"), self.getOrDefault("weightCol")
+        for c in (lcol, wcol):
+            if c and c not in df._cols:
+                raise IllegalArgumentException("Field \"%s\" does not exist." % c)
+        y = df._column_tensor(lcol).to(torch.float64).reshape(-1)
+        w = df._column_tensor(wcol).to(torch.float64).reshape(-1) if wcol else None
+        try:
+            fit = biso.isotonic_fit(x, y, w, isotonic=bool(self.getOrDefault("isotonic")), group=bdist.group())
+        except ValueError as e:
+            raise IllegalArgumentException(str(e))
+        m = IsotonicRegressionModel(fit)
+        m._paramMap = {k: v for k, v in self._paramMap.items() if k in m._all_defaults()}
+        return m
+
+
+class IsotonicRegressionModel(Model, _IsotonicRegressionParams):
+    """boundaries (increasing) and predictions; predict(x) interpolates linearly between the boundaries around x and is
+    constant outside them."""
+
+    def __init__(self, fit):
+        super().__init__()
+        self._fit_result = fit             # b200flow.isotonic.IsotonicFit
+
+    @property
+    def boundaries(self):
+        from .linalg import DenseVector
+        return DenseVector(self._fit_result.boundaries.copy())
+
+    @property
+    def predictions(self):
+        from .linalg import DenseVector
+        return DenseVector(self._fit_result.predictions.copy())
+
+    @property
+    def numFeatures(self):
+        return 1
+
+    def predict(self, value):
+        """the prediction at one feature value, on the host (the kernel's arithmetic, so the same bits)"""
+        from b200flow import isotonic as biso
+        try:
+            return biso.predict_value(float(value), self._fit_result)
+        except ValueError as e:
+            raise IllegalArgumentException(str(e))
+
+    def _transform(self, df):
+        from b200flow import isotonic as biso
+        x = _isotonic_feature(self, df)
+        pcol = self.getOrDefault("predictionCol")
+        if not pcol:
+            return df
+        if pcol in df._cols:
+            raise IllegalArgumentException("Output column %s already exists." % pcol)
+        try:
+            pred = biso.isotonic_predict(x, self._fit_result)
+        except ValueError as e:
+            raise IllegalArgumentException(str(e))
+        cols = dict(df._cols)
+        cols[pcol] = ColumnData("numeric", pred, "f64")
+        return df._with(cols=cols)
+
+    def __repr__(self):
+        return "IsotonicRegressionModel: uid=%s, numFeatures=1, boundaries=%d" % (self.uid, len(self._fit_result.boundaries))
