@@ -497,6 +497,14 @@ int b200flow_linreg_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, in
                               const double* shift, const double* inv, double y_shift, double y_scale, const double* w,
                               const double* b_sigma, double epsilon, int32_t mode, int64_t row_offset, double* partials,
                               void* stream);
+/* AFTSurvivalRegression (Weibull), DESIGN.md §5q: b200flow_linreg_loss_grad's staging, margin and partials layout with
+ * y = log_t [n_rows] f64 (the log of the survival time), censor [n_rows] int32 (1 when the event was observed, 0 when the
+ * row is censored) and b_sigma = [b, sigma, log sigma] f64, all device.  z = (log t - m - b) / sigma and delta = censor:
+ * loss delta log sigma - delta z + e^z, a = (delta - e^z) / sigma, sigma derivative (with respect to log sigma)
+ * delta + (delta - e^z) z. */
+int b200flow_aft_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, int32_t D, const double* log_t,
+                           const int32_t* censor, const double* shift, const double* inv, const double* w,
+                           const double* b_sigma, int64_t row_offset, double* partials, void* stream);
 
 /* ------------------------------------------------------------ generalized linear regression ---
  * GeneralizedLinearRegression, DESIGN.md §5o.  Features x [n_rows][ld] f32 or f64 (converted to f64 first), 1 <= D <= 255;
@@ -586,6 +594,13 @@ int b200flow_fm_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, int64_
 /* raw [n_rows][K] f64: raw[i][k] = r of row i under weights[k], with b200flow_fm_loss_grad's arithmetic. */
 int b200flow_fm_raw(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, int32_t D, int32_t factor_size, int64_t K,
                     const double* weights, double* raw, void* stream);
+/* FMRegressor, DESIGN.md §5r: b200flow_fm_loss_grad's partials for one column (K = 1) under the squared error, with labels
+ * y [n_rows] f64 (device, used as they are): g = 2 (r - y), loss (r - y)^2.  The layout, the mini-batch draw and the
+ * summation order are b200flow_fm_loss_grad's. */
+int b200flow_fm_regression_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, int32_t D,
+                                     int32_t factor_size, const double* labels, const double* weights,
+                                     double mini_batch_fraction, uint64_t batch_seed, int64_t row_offset, double* partials,
+                                     void* stream);
 
 /* ------------------------------------------------------------ mixture models ---
  * GaussianMixture (full covariance), DESIGN.md §5g.  Features x [n_rows][ld] f64, rows [0, n_rows) are global rows

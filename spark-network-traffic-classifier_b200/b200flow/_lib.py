@@ -83,11 +83,13 @@ _SIGNATURES = {
     "b200flow_svc_loss_grad": [_P, _I32, _I64, _I64, _I32, _P, _P, _I64, _P, _P, _I64, _P, _P],
     "b200flow_svc_margins": [_P, _I32, _I64, _I64, _I32, _I64, _P, _P, _P],
     "b200flow_linreg_loss_grad": [_P, _I32, _I64, _I64, _I32, _P, _P, _P, _F64, _F64, _P, _P, _F64, _I32, _I64, _P, _P],
+    "b200flow_aft_loss_grad": [_P, _I32, _I64, _I64, _I32, _P, _P, _P, _P, _P, _P, _I64, _P, _P],
     "b200flow_glm_rows": [_P, _I32, _I64, _I64, _I32, _P, _P, _P, _P, _F64, _F64, _I32, _I32, _F64, _F64, _I32, _I64, _P, _P,
                           _P],
     "b200flow_isotonic_fit": [_P, _I32, _I64, _P, _I64, _P, _I64, _I64, _I32, _I64, _P, _I64, _P, _P, _P, _P, _P],
     "b200flow_isotonic_predict": [_P, _I32, _I64, _I64, _P, _P, _I64, _P, _P],
     "b200flow_fm_loss_grad": [_P, _I32, _I64, _I64, _I32, _I32, _P, _P, _I64, _P, _F64, _U64, _I64, _P, _P],
+    "b200flow_fm_regression_loss_grad": [_P, _I32, _I64, _I64, _I32, _I32, _P, _P, _F64, _U64, _I64, _P, _P],
     "b200flow_fm_raw": [_P, _I32, _I64, _I64, _I32, _I32, _I64, _P, _P, _P],
     "b200flow_gmm_estep": [_P, _I64, _I32, _I64, _I32, _P, _P, _P, _I64, _P, _P, _P, _P],
     "b200flow_gmm_moments": [_P, _I64, _I32, _I64, _I32, _P, _I64, _P, _P],

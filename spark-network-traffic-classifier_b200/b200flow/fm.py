@@ -1,6 +1,7 @@
-"""FMClassifier and OneVsRest(FMClassifier) on the device (DESIGN.md §5k): the logistic factorization-machine loss and
-its gradient from csrc/fm.cu's fused fp64 tensor-core kernel, summed in the chunk order of dist.Shards, and mllib's
-mini-batch gradient descent with the gd or adamW updater, one optimiser per class column, all of them advanced together.
+"""FMClassifier, OneVsRest(FMClassifier) and FMRegressor on the device (DESIGN.md §5k, §5r): the logistic (classifier)
+or squared-error (regressor) factorization-machine loss and its gradient from csrc/fm.cu's fused fp64 tensor-core kernel,
+summed in the chunk order of dist.Shards, and mllib's mini-batch gradient descent with the gd or adamW updater, one
+optimiser per class column, all of them advanced together.
 
 Spark [recalled; Spark 3 `ml/regression/FMRegressor.scala` (trait FactorizationMachines), `FMClassifier.scala`, mllib
 `GradientDescent.runMiniBatchSGD`]:
@@ -13,6 +14,8 @@ Spark [recalled; Spark 3 `ml/regression/FMRegressor.scala` (trait FactorizationM
     regVal_0 = 1/2 regParam |w_0|^2; for i = 1..maxIter, over the rows drawn with fraction miniBatchFraction: if the
     batch is not empty, history += lossSum / batchSize + regVal, then the updater takes gradSum / batchSize; stop when
     |w_i - w_{i-1}| < tol max(|w_i|, 1), from the second update on.
+    FMRegressor (MSEFactorizationMachinesGradient): the same loop on one column, with the label y used as it is,
+    g = 2 (r - y) and loss = (r - y)^2; the prediction is r.
     gd (SquaredL2Updater): eta = stepSize / sqrt(i), w <- w (1 - eta regParam) - eta g.
     adamW (AdamWUpdater): m = b1 m + (1 - b1) g, v = b2 v + (1 - b2) g^2, b1^t *= b1, b2^t *= b2,
     w -= stepSize m_hat / (sqrt(v_hat) + eps) + regParam w.  Both return regVal = 1/2 regParam |w|^2.
@@ -21,8 +24,9 @@ Spark samples each iteration's batch with `data.sample(false, fraction, 42 + i)`
 is in the batch iff its Philox draw (purpose FMMB, key seed 42 + i, counter the global row) is below floor(fraction 2^32).
 The draw depends neither on the class nor on the estimator seed, so the classes of a OneVsRest fit share each batch.
 
-One code path serves both estimators: the standalone FMClassifier is fm_fit_classes(positives=[1]), OneVsRest
-(FMClassifier) is positives=range(K).  Each iteration makes ONE kernel pass over the classes still running.  A column's
+One code path serves both classifier estimators: the standalone FMClassifier is fm_fit_classes(positives=[1]), OneVsRest
+(FMClassifier) is positives=range(K); FMRegressor (fm_regression_fit) runs the same optimiser loop (_minibatch_sgd) on
+the squared-error totals.  Each iteration makes ONE kernel pass over the classes still running.  A column's
 partial does not depend on the other columns of the launch (csrc/fm.cu); the updates are elementwise, and every reduction
 (|w|, |w - w_prev|) is taken per class on a fresh tensor of the standalone fit's shape, so every class takes exactly the
 steps of its standalone fit.  The optimiser state is f64 on the device: host reductions pick their vector width by CPU
@@ -142,6 +146,25 @@ def fm_raw(x, weights, factor_size):
     return raw[:n]
 
 
+def regression_loss_grad(x, y, weights, factor_size, fraction, batch_seed, row_offset, partials):
+    """b200flow_fm_regression_loss_grad on the rows x [n, D] (f32/f64): partials [n_chunks, 1, D (k + 1) + D + 3] f64
+    device; labels y f64 [n] and weights f64 [1, D (k + 1) + 1], device."""
+    n, D = x.shape
+    call("b200flow_fm_regression_loss_grad", ptr(x), _lib.dtype_code(x), n, x.stride(0), D, int(factor_size), ptr(y),
+         ptr(weights), float(fraction), int(batch_seed), int(row_offset), ptr(partials))
+
+
+def fm_regression_loss_grad_totals(x, y, weights, factor_size, fraction, batch_seed, sh):
+    """[1, D (k + 1) + D + 3] f64 device: b200flow_fm_regression_loss_grad's sums over every rank's rows, in chunk order;
+    the same bits on every rank."""
+    D = x.shape[1]
+
+    def launch(xs, _, ys, go, parts):
+        regression_loss_grad(xs, ys, weights, factor_size, fraction, batch_seed, go, parts)
+
+    return selection.chunk_total(x, None, y, sh, 1, D * (factor_size + 1) + D + 3, launch)
+
+
 def _norm(v):
     """|v| of one class's coefficients on a fresh tensor, so that the reduction is the standalone fit's whatever row of a
     class batch v came from"""
@@ -184,7 +207,54 @@ def fm_fit_classes(x, labels, positives, params, row_offset=None, group=None):
         raise ValueError("Classifier was given dataset with invalid label. Labels must be integers in [0, %d)." % n_labels)
     if int(bad[1].item()):
         raise ValueError("FMClassifier needs finite features")
+    pos_dev = torch.tensor(positives, dtype=torch.int32, device=dev)
 
+    def totals(wk, ia, act, it):
+        sel = pos_dev if len(act) == K else pos_dev[ia].contiguous()
+        return fm_loss_grad_totals(x, yi, sel, wk, kf, params.mini_batch_fraction, 42 + it, sh)
+
+    return _minibatch_sgd(K, D, params, dev, totals)
+
+
+def fm_regression_fit(x, labels, params, row_offset=None, group=None):
+    """FMRegressor fit of this rank's rows x [n, D] (f32 or f64) and finite labels [n].  An empty shard still joins every
+    collective.  -> FMFit(factors f64 [D, k], linear f64 [D], intercept float, objective history, iterations)."""
+    x = _check_x(x)
+    n_local, D = x.shape
+    if params.solver not in SOLVERS:
+        raise ValueError("solver must be 'gd' or 'adamW', got %r" % (params.solver,))
+    kf = params.factor_size
+    _lib.fm_config(D, kf, 1)
+    grp = group if group is not None else bdist.group()
+    dev = x.device
+    if row_offset is None:
+        row_offset, _ = bdist.global_offset(n_local, dev, grp)
+    sh = bdist.Shards(n_local, row_offset, grp, dev)
+    y = labels.to(device=dev, dtype=torch.float64).reshape(-1).contiguous()
+    bad = torch.stack([(~torch.isfinite(y)).any(), (~torch.isfinite(x)).any(), torch.tensor(y.shape[0] != n_local, device=dev)])
+    bad = bad.to(torch.int64)
+    if grp is not None:
+        bdist.all_reduce_(bad, grp)
+    if int(bad[2].item()):                                  # the kernel reads one label per row
+        raise ValueError("FMRegressor needs one label per row (a shard has %d rows and %d labels)" % (n_local, y.shape[0]))
+    if sh.total == 0:
+        raise ValueError("FMRegressor needs at least one row")
+    if int(bad[0].item()):
+        raise ValueError("FMRegressor needs finite labels")
+    if int(bad[1].item()):
+        raise ValueError("FMRegressor needs finite features")
+
+    def totals(wk, ia, act, it):
+        return fm_regression_loss_grad_totals(x, y, wk, kf, params.mini_batch_fraction, 42 + it, sh)
+
+    return _minibatch_sgd(1, D, params, dev, totals)[0]
+
+
+def _minibatch_sgd(K, D, params, dev, totals):
+    """runMiniBatchSGD for K columns in lockstep: totals(wk [len(act), D (k + 1) + 1] kernel weights, ia (device indices of
+    the active columns), act (their list), iteration) -> the kernel layout's sums [len(act), D (k + 1) + D + 3] of the
+    active columns.  -> [FMFit] per column."""
+    kf = params.factor_size
     # the coefficients in Spark's layout [V | w if fitLinear | b if fitIntercept], one row per class, f64 on the device
     nv = D * kf
     P = nv + (D if params.fit_linear else 0) + (1 if params.fit_intercept else 0)
@@ -195,7 +265,6 @@ def fm_fit_classes(x, labels, positives, params, row_offset=None, group=None):
     v = torch.zeros_like(coef)
     b1t = b2t = 1.0
     reg = params.reg_param
-    pos_dev = torch.tensor(positives, dtype=torch.int32, device=dev)
     half_reg = torch.tensor(0.5 * reg, dtype=torch.float64, device=dev)
 
     def reg_val(nrm):
@@ -217,8 +286,7 @@ def fm_fit_classes(x, labels, positives, params, row_offset=None, group=None):
             wk[:, nv:nv + D] = cur[:, nv:nv + D]
         if params.fit_intercept:
             wk[:, -1] = cur[:, -1]
-        sel = pos_dev if len(act) == K else pos_dev[ia].contiguous()
-        tot = fm_loss_grad_totals(x, yi, sel, wk, kf, params.mini_batch_fraction, 42 + it, sh)
+        tot = totals(wk, ia, act, it)
         batch = float(tot[0, 1].item())
         if batch == 0.0:                                    # an empty batch: no update, the iteration still counts
             continue

@@ -1,4 +1,5 @@
-// fm.cu — FMClassifier: the logistic factorization-machine loss + gradient and the raw values, DESIGN.md §5k.
+// fm.cu — FMClassifier and FMRegressor: the logistic / squared-error factorization-machine loss + gradient and the raw
+// values, DESIGN.md §5k, §5r.
 //
 // K binary problems over the same rows at once: column k treats label == positives[k] as y = 1 and every other label as
 // y = 0, with weights [V_k (D x F, row-major), w_k (D), b_k].  Per row and column, with s_f = sum_i v_if x_i and
@@ -20,6 +21,9 @@
 // ones column, S and Q, then per (row, class) r, g and the loss, a sequential row-order loss sum per class, and the
 // gradient products.  The gradient accumulates in registers for the whole chunk: tile t belongs to warp t % 8, slot t / 8.
 // Rows outside the launch, and rows the mini-batch draw leaves out, are masked (g = 0, no loss), never padded in.
+//
+// b200flow_fm_regression_loss_grad: the same kernel with the squared-error policy (kReg): one column, f64 labels read as
+// they are, g = 2 (r - y), loss (r - y)^2; no class labels or positives are read.
 //
 // b200flow_fm_raw: the same tile load, products and per-row arithmetic, r written out per row.
 #include "common.cuh"
@@ -160,13 +164,14 @@ __device__ __forceinline__ double fm_raw_value(const double* Srow, const double*
 
 __device__ __forceinline__ double log1p_exp(double v) { return v > 0.0 ? v + log1p(exp(-v)) : log1p(exp(v)); }
 
-template <typename T>
+template <typename T, bool kReg>
 __global__ void __launch_bounds__(kFmThreads, 1) fm_loss_grad_kernel(const T* __restrict__ x, int64_t n, int64_t ld,
                                                                      const int32_t* __restrict__ y,
                                                                      const int32_t* __restrict__ positives, const FmShape s,
                                                                      const double* __restrict__ w, double fraction,
                                                                      uint64_t batch_seed, int64_t row_offset,
-                                                                     double* __restrict__ partials) {
+                                                                     double* __restrict__ partials,
+                                                                     const double* __restrict__ yreg) {
     extern __shared__ double sm[];
     __shared__ double bsh[kFmMaxBlockClasses];
     __shared__ int ylab[kFmTile], yval[kFmTile], posb[kFmMaxBlockClasses];
@@ -184,7 +189,7 @@ __global__ void __launch_bounds__(kFmThreads, 1) fm_loss_grad_kernel(const T* __
     const int64_t lo = c0 > 0 ? c0 : 0, hi = c0 + kChunkRows < n ? c0 + kChunkRows : n;
     const bool sampled = fraction < 1.0;
     const uint64_t keep_below = (uint64_t)floor(fraction * 4294967296.0);
-    if (threadIdx.x < nk) posb[threadIdx.x] = positives[k0 + threadIdx.x];
+    if (!kReg && threadIdx.x < nk) posb[threadIdx.x] = positives[k0 + threadIdx.x];
     double acc[kFmSlots][2];
 #pragma unroll
     for (int q = 0; q < kFmSlots; ++q) acc[q][0] = acc[q][1] = 0.0;
@@ -200,7 +205,7 @@ __global__ void __launch_bounds__(kFmThreads, 1) fm_loss_grad_kernel(const T* __
                 valid = philox_keyed(batch_seed, PURPOSE_FMMB, (uint32_t)row, (uint32_t)(row >> 32), 0u, 0u).x < keep_below;
             }
             yval[threadIdx.x] = valid;
-            ylab[threadIdx.x] = valid ? y[gr] : 0;
+            if (!kReg) ylab[threadIdx.x] = valid ? y[gr] : 0;
         }
         __syncthreads();
         fm_products_tile(s, X, sm, S, Q);
@@ -211,9 +216,15 @@ __global__ void __launch_bounds__(kFmThreads, 1) fm_loss_grad_kernel(const T* __
             double g = 0.0, l = 0.0;
             if (yval[r]) {
                 const double rv = fm_raw_value(Sr, Q + r * s.pm, col0, F, bsh[c]);
-                const bool pos = ylab[r] == posb[c];
-                g = 1.0 / (1.0 + exp(-rv)) - (pos ? 1.0 : 0.0);
-                l = pos ? log1p_exp(-rv) : log1p_exp(rv);
+                if (kReg) {
+                    const double d = rv - yreg[base + r];
+                    g = 2.0 * d;
+                    l = d * d;
+                } else {
+                    const bool pos = ylab[r] == posb[c];
+                    g = 1.0 / (1.0 + exp(-rv)) - (pos ? 1.0 : 0.0);
+                    l = pos ? log1p_exp(-rv) : log1p_exp(rv);
+                }
             }
             for (int f = 0; f < F; ++f) Sr[col0 + f] = yval[r] ? g * Sr[col0 + f] : 0.0;
             Sr[col0 + F] = g;
@@ -338,15 +349,49 @@ extern "C" int b200flow_fm_loss_grad(const void* x, int32_t x_dtype, int64_t n_r
     const dim3 grid((unsigned)nc, (unsigned)s.blocks);
     cudaStream_t st = (cudaStream_t)stream;
     if (x_dtype == B200FLOW_F64) {
-        cudaFuncSetAttribute(fm_loss_grad_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        fm_loss_grad_kernel<double><<<grid, kFmThreads, smem, st>>>((const double*)x, n_rows, ld, labels, positives, s, weights,
-                                                                    mini_batch_fraction, batch_seed, row_offset, partials);
+        cudaFuncSetAttribute(fm_loss_grad_kernel<double, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        fm_loss_grad_kernel<double, false><<<grid, kFmThreads, smem, st>>>((const double*)x, n_rows, ld, labels, positives, s,
+                                                                           weights, mini_batch_fraction, batch_seed,
+                                                                           row_offset, partials, nullptr);
     } else {
-        cudaFuncSetAttribute(fm_loss_grad_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        fm_loss_grad_kernel<float><<<grid, kFmThreads, smem, st>>>((const float*)x, n_rows, ld, labels, positives, s, weights,
-                                                                   mini_batch_fraction, batch_seed, row_offset, partials);
+        cudaFuncSetAttribute(fm_loss_grad_kernel<float, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        fm_loss_grad_kernel<float, false><<<grid, kFmThreads, smem, st>>>((const float*)x, n_rows, ld, labels, positives, s,
+                                                                          weights, mini_batch_fraction, batch_seed,
+                                                                          row_offset, partials, nullptr);
     }
     return check_launch("fm_loss_grad");
+}
+
+extern "C" int b200flow_fm_regression_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, int32_t D,
+                                                int32_t factor_size, const double* labels, const double* weights,
+                                                double mini_batch_fraction, uint64_t batch_seed, int64_t row_offset,
+                                                double* partials, void* stream) {
+    FmShape s;
+    const int rc = fm_shape(D, factor_size, 1, &s);
+    if (rc != B200FLOW_OK) return rc;
+    B2F_REQUIRE(n_rows >= 0 && row_offset >= 0 && ld >= D && (x_dtype == B200FLOW_F32 || x_dtype == B200FLOW_F64),
+                "fm_regression_loss_grad: n >= 0, row_offset >= 0, ld >= D, f32 or f64 features");
+    B2F_REQUIRE(mini_batch_fraction > 0.0 && mini_batch_fraction <= 1.0,
+                "fm_regression_loss_grad: miniBatchFraction in (0, 1], got %g", mini_batch_fraction);
+    if (n_rows == 0) return B200FLOW_OK;
+    B2F_REQUIRE(x && labels && weights && partials, "fm_regression_loss_grad: null pointer");
+    const int64_t nc = (row_offset + n_rows - 1) / kChunkRows - row_offset / kChunkRows + 1;
+    B2F_REQUIRE(nc <= 0x7fffffffll, "fm_regression_loss_grad: too many rows");
+    const size_t smem = (size_t)s.smem_doubles * sizeof(double);
+    const dim3 grid((unsigned)nc, (unsigned)s.blocks);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (x_dtype == B200FLOW_F64) {
+        cudaFuncSetAttribute(fm_loss_grad_kernel<double, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        fm_loss_grad_kernel<double, true><<<grid, kFmThreads, smem, st>>>((const double*)x, n_rows, ld, nullptr, nullptr, s,
+                                                                          weights, mini_batch_fraction, batch_seed,
+                                                                          row_offset, partials, labels);
+    } else {
+        cudaFuncSetAttribute(fm_loss_grad_kernel<float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        fm_loss_grad_kernel<float, true><<<grid, kFmThreads, smem, st>>>((const float*)x, n_rows, ld, nullptr, nullptr, s,
+                                                                         weights, mini_batch_fraction, batch_seed,
+                                                                         row_offset, partials, labels);
+    }
+    return check_launch("fm_regression_loss_grad");
 }
 
 extern "C" int b200flow_fm_raw(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, int32_t D, int32_t factor_size, int64_t K,

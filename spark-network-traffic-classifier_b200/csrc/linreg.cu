@@ -1,4 +1,5 @@
-// linreg.cu — LinearRegression: the per-row least-squares / Huber loss and gradient sums, DESIGN.md §5n.
+// linreg.cu — LinearRegression and AFTSurvivalRegression: the per-row least-squares / Huber / Weibull AFT loss and gradient
+// sums, DESIGN.md §5n, §5q.
 //
 // One pass over the rows per optimiser evaluation.  At one weight column the pass is bound by HBM (about 0.5 FLOP per
 // byte at f64), so it uses plain fp64 FMA-free arithmetic, not tensor cores; what matters is that every element of x is read
@@ -12,6 +13,8 @@
 //       squared: d = m − (y − c)·t, l = d², a = d, s = 0;
 //       huber:   z = (y − m − b)/σ; |z| <= ε: l = σ + z²σ, a = −2z, s = 1 − z²;  else l = σ + (2ε|z| − ε²)σ, a = −2ε·sign(z),
 //                s = 1 − ε².
+//     aft (a separate instantiation, kAft): y = log t, δ the censor (1 observed, 0 censored), z = (y − m − b)/σ;
+//                l = δ·log σ − δ·z + e^z, a = (δ − e^z)/σ, s = δ + (δ − e^z)·z.
 //   gradient phase: thread j < D adds a[r]·xs[r][j] over the tile's rows in order; the last thread adds l, a and s.
 // Each sum runs over the chunk's rows in row order from +0.0, so a chunk's partial depends only on its rows and the
 // inputs.  No atomics.
@@ -30,7 +33,7 @@ __host__ __device__ inline int lr_pitch(int D) { return D | 1; }    // odd: the 
 
 inline size_t lr_smem(int D) { return ((size_t)kLrTile * lr_pitch(D) + 3 * (size_t)D) * sizeof(double); }
 
-template <typename T>
+template <typename T, bool kAft>
 __global__ void __launch_bounds__(kLrThreads) linreg_loss_grad_kernel(const T* __restrict__ x, int64_t n, int64_t ld, int D,
                                                                       const double* __restrict__ y,
                                                                       const double* __restrict__ shift,
@@ -38,7 +41,8 @@ __global__ void __launch_bounds__(kLrThreads) linreg_loss_grad_kernel(const T* _
                                                                       double y_scale, const double* __restrict__ w,
                                                                       const double* __restrict__ b_sigma, double eps,
                                                                       int mode, int64_t row_offset,
-                                                                      double* __restrict__ partials) {
+                                                                      double* __restrict__ partials,
+                                                                      const int32_t* __restrict__ censor) {
     extern __shared__ double sm[];
     __shared__ double av[kLrTile], lv[kLrTile], sv[kLrTile];
     const int pitch = lr_pitch(D);
@@ -52,7 +56,8 @@ __global__ void __launch_bounds__(kLrThreads) linreg_loss_grad_kernel(const T* _
         is[j] = inv[j];
     }
     const bool huber = mode == B200FLOW_LINREG_HUBER, shifted = shift != nullptr;
-    const double b = huber ? b_sigma[0] : 0.0, sigma = huber ? b_sigma[1] : 1.0;
+    const double b = huber || kAft ? b_sigma[0] : 0.0, sigma = huber || kAft ? b_sigma[1] : 1.0;
+    const double log_sigma = kAft ? b_sigma[2] : 0.0;
     const int64_t c0 = (row_offset / kChunkRows + blockIdx.x) * kChunkRows - row_offset;   // local index of the chunk's row 0
     const int64_t lo = c0 > 0 ? c0 : 0, hi = c0 + kChunkRows < n ? c0 + kChunkRows : n;
     const int tid = threadIdx.x;
@@ -80,7 +85,12 @@ __global__ void __launch_bounds__(kLrThreads) linreg_loss_grad_kernel(const T* _
                 double m = 0.0;
                 for (int j = 0; j < D; ++j) m = m + xr[j] * ws[j];
                 const double yv = y[gr];
-                if (!huber) {
+                if (kAft) {
+                    const double z = (yv - m - b) / sigma, ez = exp(z), dl = censor[gr] ? 1.0 : 0.0;
+                    l = dl * log_sigma - dl * z + ez;
+                    a = (dl - ez) / sigma;
+                    s = dl + (dl - ez) * z;
+                } else if (!huber) {
                     const double d = m - (yv - y_shift) * y_scale;
                     l = d * d;
                     a = d;
@@ -143,15 +153,45 @@ extern "C" int b200flow_linreg_loss_grad(const void* x, int32_t x_dtype, int64_t
     const size_t smem = lr_smem(D);
     cudaStream_t st = (cudaStream_t)stream;
     if (x_dtype == B200FLOW_F64) {
-        cudaFuncSetAttribute(linreg_loss_grad_kernel<double>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        linreg_loss_grad_kernel<double><<<(unsigned)nc, kLrThreads, smem, st>>>((const double*)x, n_rows, ld, D, y, shift, inv,
-                                                                               y_shift, y_scale, w, b_sigma, epsilon, mode,
-                                                                               row_offset, partials);
+        cudaFuncSetAttribute(linreg_loss_grad_kernel<double, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        linreg_loss_grad_kernel<double, false><<<(unsigned)nc, kLrThreads, smem, st>>>((const double*)x, n_rows, ld, D, y,
+                                                                                      shift, inv, y_shift, y_scale, w, b_sigma,
+                                                                                      epsilon, mode, row_offset, partials,
+                                                                                      nullptr);
     } else {
-        cudaFuncSetAttribute(linreg_loss_grad_kernel<float>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        linreg_loss_grad_kernel<float><<<(unsigned)nc, kLrThreads, smem, st>>>((const float*)x, n_rows, ld, D, y, shift, inv,
-                                                                              y_shift, y_scale, w, b_sigma, epsilon, mode,
-                                                                              row_offset, partials);
+        cudaFuncSetAttribute(linreg_loss_grad_kernel<float, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        linreg_loss_grad_kernel<float, false><<<(unsigned)nc, kLrThreads, smem, st>>>((const float*)x, n_rows, ld, D, y,
+                                                                                     shift, inv, y_shift, y_scale, w, b_sigma,
+                                                                                     epsilon, mode, row_offset, partials,
+                                                                                     nullptr);
     }
     return check_launch("linreg_loss_grad");
+}
+
+extern "C" int b200flow_aft_loss_grad(const void* x, int32_t x_dtype, int64_t n_rows, int64_t ld, int32_t D, const double* log_t,
+                                      const int32_t* censor, const double* shift, const double* inv, const double* w,
+                                      const double* b_sigma, int64_t row_offset, double* partials, void* stream) {
+    B2F_REQUIRE(D >= 1 && D <= kLrMaxD, "aft_loss_grad: 1 <= D <= %d features, got %d", kLrMaxD, D);
+    B2F_REQUIRE(n_rows >= 0 && row_offset >= 0 && ld >= D && (x_dtype == B200FLOW_F32 || x_dtype == B200FLOW_F64),
+                "aft_loss_grad: n >= 0, row_offset >= 0, ld >= D, f32 or f64 features");
+    if (n_rows == 0) return B200FLOW_OK;
+    B2F_REQUIRE(x && log_t && censor && inv && w && b_sigma && partials, "aft_loss_grad: null pointer");
+    const int64_t nc = (row_offset + n_rows - 1) / kChunkRows - row_offset / kChunkRows + 1;
+    B2F_REQUIRE(nc <= 0x7fffffffll, "aft_loss_grad: too many rows");
+    const size_t smem = lr_smem(D);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (x_dtype == B200FLOW_F64) {
+        cudaFuncSetAttribute(linreg_loss_grad_kernel<double, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        linreg_loss_grad_kernel<double, true><<<(unsigned)nc, kLrThreads, smem, st>>>((const double*)x, n_rows, ld, D, log_t,
+                                                                                     shift, inv, 0.0, 1.0, w, b_sigma, 0.0,
+                                                                                     B200FLOW_LINREG_SQUARED, row_offset,
+                                                                                     partials, censor);
+    } else {
+        cudaFuncSetAttribute(linreg_loss_grad_kernel<float, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        linreg_loss_grad_kernel<float, true><<<(unsigned)nc, kLrThreads, smem, st>>>((const float*)x, n_rows, ld, D, log_t,
+                                                                                    shift, inv, 0.0, 1.0, w, b_sigma, 0.0,
+                                                                                    B200FLOW_LINREG_SQUARED, row_offset,
+                                                                                    partials, censor);
+    }
+    return check_launch("aft_loss_grad");
 }

@@ -2,8 +2,10 @@
 loop (b200flow/regression.py, b200flow/gbt_regression.py, csrc/regression.cu, DESIGN.md §5l, §5m), and LinearRegression
 on the normal equations and the fused least-squares / Huber kernel (b200flow/linreg.py, csrc/linreg.cu, DESIGN.md §5n),
 GeneralizedLinearRegression by IRLS on the per-row GLM kernel and the weighted Gram kernel (b200flow/glm.py,
-csrc/glm.cu, DESIGN.md §5o), and IsotonicRegression on a device sort and a chunked pool-adjacent-violators merge
-(b200flow/isotonic.py, csrc/isotonic.cu, DESIGN.md §5p).
+csrc/glm.cu, DESIGN.md §5o), IsotonicRegression on a device sort and a chunked pool-adjacent-violators merge
+(b200flow/isotonic.py, csrc/isotonic.cu, DESIGN.md §5p), AFTSurvivalRegression on the Weibull instantiation of the
+per-row linear-regression kernel (b200flow/aft.py, csrc/linreg.cu, DESIGN.md §5q), and FMRegressor on the squared-error
+factorization-machine kernel (b200flow/fm.py, csrc/fm.cu, DESIGN.md §5r).
 Their models are the same bits for any number of ranks.
 
 Deviations from Spark: a NaN or infinite label raises IllegalArgumentException (Spark trains on it); labels (and GBT
@@ -21,7 +23,8 @@ from ..sql import ColumnData
 from .classification import _arity_from_attrs, _default_seed, _lazy_plan
 from .feature import IllegalArgumentException
 
-__all__ = ["DecisionTreeRegressionModel", "DecisionTreeRegressor", "GBTRegressionModel", "GBTRegressor",
+__all__ = ["AFTSurvivalRegression", "AFTSurvivalRegressionModel", "DecisionTreeRegressionModel", "DecisionTreeRegressor",
+           "FMRegressionModel", "FMRegressor", "GBTRegressionModel", "GBTRegressor",
            "GeneralizedLinearRegression", "GeneralizedLinearRegressionModel", "GeneralizedLinearRegressionSummary",
            "GeneralizedLinearRegressionTrainingSummary", "IsotonicRegression", "IsotonicRegressionModel",
            "LinearRegression", "LinearRegressionModel", "LinearRegressionSummary", "LinearRegressionTrainingSummary",
@@ -823,3 +826,261 @@ class IsotonicRegressionModel(Model, _IsotonicRegressionParams):
 
     def __repr__(self):
         return "IsotonicRegressionModel: uid=%s, numFeatures=1, boundaries=%d" % (self.uid, len(self._fit_result.boundaries))
+
+
+# ------------------------------------------------------------------------------- survival regression
+class _AFTSurvivalRegressionParams:
+    _defaults = {"featuresCol": "features", "labelCol": "label", "predictionCol": "prediction", "censorCol": "censor",
+                 "quantileProbabilities": [0.01, 0.05, 0.1, 0.25, 0.5, 0.75, 0.9, 0.95, 0.99], "quantilesCol": None,
+                 "fitIntercept": True, "maxIter": 100, "tol": 1e-6, "aggregationDepth": 2, "maxBlockSizeInMB": 0.0}
+
+
+class AFTSurvivalRegression(Estimator, _AFTSurvivalRegressionParams):
+    """Spark 3's AFTSurvivalRegression [recalled]: the Weibull accelerated-failure-time model of a positive lifetime with
+    right censoring (censor 1.0: the event was observed, 0.0: censored), fitted by L-BFGS on the device
+    (b200flow/aft.py, DESIGN.md §5q).  aggregationDepth and maxBlockSizeInMB are validated but do not change the result:
+    the sums have one fixed order."""
+
+    def __init__(self, featuresCol=None, labelCol=None, predictionCol=None, fitIntercept=None, maxIter=None, tol=None,
+                 censorCol=None, quantileProbabilities=None, quantilesCol=None, aggregationDepth=None,
+                 maxBlockSizeInMB=None):
+        kw = dict(locals()); kw.pop("self"); kw.pop("__class__", None)
+        super().__init__(**kw)
+
+    def _check(self):
+        """Spark's param validators -> b200flow.aft.AFTParams"""
+        from b200flow import aft as baft
+        g = self.getOrDefault
+        it, depth = g("maxIter"), g("aggregationDepth")
+        if isinstance(it, bool) or int(it) != it or int(it) < 0:
+            raise IllegalArgumentException("maxIter must be an integer >= 0, got %r" % (it,))
+        if isinstance(depth, bool) or int(depth) != depth or int(depth) < 2:
+            raise IllegalArgumentException("aggregationDepth must be an integer >= 2, got %r" % (depth,))
+        if not float(g("maxBlockSizeInMB")) >= 0:
+            raise IllegalArgumentException("maxBlockSizeInMB must be >= 0, got %r" % (g("maxBlockSizeInMB"),))
+        try:
+            p = baft.AFTParams(max_iter=int(it), tol=float(g("tol")), fit_intercept=bool(g("fitIntercept")),
+                               quantile_probabilities=list(g("quantileProbabilities")))
+            baft.check_params(p)
+        except (TypeError, ValueError) as e:
+            raise IllegalArgumentException(str(e))
+        return p
+
+    def _fit(self, df):
+        from b200flow import aft as baft
+        p = self._check()
+        fc, y = _features_and_label(self, df)
+        ccol = self.getOrDefault("censorCol")
+        if ccol not in df._cols:
+            raise IllegalArgumentException("Field \"%s\" does not exist." % ccol)
+        c = df._column_tensor(ccol).to(torch.float64).reshape(-1).contiguous()
+        x = fc.data
+        try:
+            grp = bdist.group()
+            off, _ = bdist.global_offset(x.shape[0], x.device, grp)
+            fit = baft.aft_fit(x, y, c, p, row_offset=off, group=grp)
+        except ValueError as e:        # includes b200flow's UnsupportedParamError; CUDA failures propagate as they are
+            raise IllegalArgumentException(str(e))
+        m = AFTSurvivalRegressionModel(fit)
+        m._paramMap = {k: v for k, v in self._paramMap.items() if k in m._all_defaults()}
+        return m
+
+
+class AFTSurvivalRegressionModel(Model, _AFTSurvivalRegressionParams):
+    """coefficients (original feature scale), intercept and scale (the Weibull sigma); prediction = exp(x . coefficients +
+    intercept), the quantiles lambda exp(log(-log1p(-p)) scale) for each p of quantileProbabilities.  Spark has no
+    training summary for this model."""
+
+    def __init__(self, fit):
+        super().__init__()
+        self._fit_result = fit             # b200flow.aft.AFTFit
+
+    @property
+    def coefficients(self):
+        from .linalg import DenseVector
+        return DenseVector(self._fit_result.coef.copy())
+
+    @property
+    def intercept(self):
+        return self._fit_result.intercept
+
+    @property
+    def scale(self):
+        return self._fit_result.scale
+
+    @property
+    def numFeatures(self):
+        return int(self._fit_result.coef.shape[0])
+
+    def _probs(self):
+        from b200flow import aft as baft
+        probs = list(self.getOrDefault("quantileProbabilities"))
+        try:
+            baft.check_quantiles(probs)
+        except ValueError as e:
+            raise IllegalArgumentException(str(e))
+        return probs
+
+    def _row(self, features):
+        v = np.asarray(features.toArray() if hasattr(features, "toArray") else features, np.float64).reshape(1, -1)
+        if v.shape[1] != self.numFeatures:
+            raise IllegalArgumentException("the model has %d features, the vector %d" % (self.numFeatures, v.shape[1]))
+        return torch.from_numpy(v).cuda()
+
+    def predict(self, features):
+        """the prediction for one feature vector: exp(features . coefficients + intercept), transform's arithmetic"""
+        from b200flow import aft as baft
+        return float(baft.aft_predict(self._row(features), self._fit_result)[0].item())
+
+    def predictQuantiles(self, features):
+        """DenseVector of the quantiles of one feature vector's lifetime at quantileProbabilities"""
+        from b200flow import aft as baft
+        from .linalg import DenseVector
+        q = baft.aft_predict_quantiles(self._row(features), self._fit_result, self._probs())
+        return DenseVector(q[0].cpu().numpy())
+
+    def _transform(self, df):
+        from b200flow import aft as baft
+        fcol = self.getOrDefault("featuresCol")
+        if fcol not in df._cols or df._cols[fcol].kind != "vector":
+            raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+        pcol, qcol = self.getOrDefault("predictionCol"), self.getOrDefault("quantilesCol")
+        outs = [c for c in (pcol, qcol) if c]
+        if not outs:
+            return df
+        for c in outs:
+            if c in df._cols:
+                raise IllegalArgumentException("Output column %s already exists." % c)
+        probs = self._probs() if qcol else None
+        x = df._cols[fcol].data
+        if x.shape[1] != self.numFeatures:
+            raise IllegalArgumentException("the model has %d features, the input %d" % (self.numFeatures, x.shape[1]))
+        lam = baft.aft_predict(x, self._fit_result)
+        cols = dict(df._cols)
+        if pcol:
+            cols[pcol] = ColumnData("numeric", lam, "f64")
+        if qcol:
+            cols[qcol] = ColumnData("vector", baft.aft_predict_quantiles(x, self._fit_result, probs, lam=lam), "f64")
+        return df._with(cols=cols)
+
+    def __repr__(self):
+        return "AFTSurvivalRegressionModel: uid=%s, numFeatures=%d" % (self.uid, self.numFeatures)
+
+
+# ------------------------------------------------------------------------------- factorization machines
+class _FMRegressorParams:
+    _defaults = {"featuresCol": "features", "labelCol": "label", "predictionCol": "prediction", "factorSize": 8,
+                 "fitIntercept": True, "fitLinear": True, "regParam": 0.0, "miniBatchFraction": 1.0, "initStd": 0.01,
+                 "maxIter": 100, "stepSize": 1.0, "tol": 1e-6, "solver": "adamW", "seed": None, "weightCol": None}
+
+
+class FMRegressor(Estimator, _FMRegressorParams):
+    """Spark 3's FMRegressor [recalled]: a factorization machine with the squared error, trained by mllib's mini-batch
+    gradient descent with the adamW or gd updater, on the device (b200flow/fm.py, csrc/fm.cu, DESIGN.md §5r).  Features
+    and labels are not scaled.  weightCol raises."""
+
+    def __init__(self, featuresCol=None, labelCol=None, predictionCol=None, factorSize=None, fitIntercept=None,
+                 fitLinear=None, regParam=None, miniBatchFraction=None, initStd=None, maxIter=None, stepSize=None, tol=None,
+                 solver=None, seed=None, weightCol=None):
+        kw = dict(locals()); kw.pop("self"); kw.pop("__class__", None)
+        super().__init__(**kw)
+
+    def _check(self):
+        """Spark's param validators, and the refusal of weightCol -> b200flow.fm.FMParams (FMClassifier's rules)"""
+        from b200flow import fm as bfm
+        g = self.getOrDefault
+        fs, it = g("factorSize"), g("maxIter")
+        if isinstance(fs, bool) or int(fs) != fs or int(fs) < 1:
+            raise IllegalArgumentException("factorSize must be an integer >= 1, got %r" % (fs,))
+        if isinstance(it, bool) or int(it) != it or int(it) < 0:
+            raise IllegalArgumentException("maxIter must be an integer >= 0, got %r" % (it,))
+        for name in ("regParam", "initStd", "tol"):
+            if not float(g(name)) >= 0:
+                raise IllegalArgumentException("%s must be >= 0, got %r" % (name, g(name)))
+        if not float(g("stepSize")) > 0:
+            raise IllegalArgumentException("stepSize must be > 0, got %r" % (g("stepSize"),))
+        if not 0.0 < float(g("miniBatchFraction")) <= 1.0:
+            raise IllegalArgumentException("miniBatchFraction must be in (0, 1], got %r" % (g("miniBatchFraction"),))
+        if g("solver") not in bfm.SOLVERS:
+            raise IllegalArgumentException("solver must be 'gd' or 'adamW', got %r" % (g("solver"),))
+        if g("weightCol"):
+            raise IllegalArgumentException("weightCol is not supported by the b200flow FMRegressor (out of scope)")
+        seed = g("seed")
+        return bfm.FMParams(factor_size=int(fs), fit_intercept=bool(g("fitIntercept")), fit_linear=bool(g("fitLinear")),
+                            reg_param=float(g("regParam")), mini_batch_fraction=float(g("miniBatchFraction")),
+                            init_std=float(g("initStd")), max_iter=int(it), step_size=float(g("stepSize")),
+                            tol=float(g("tol")), solver=g("solver"), seed=_default_seed(self) if seed is None else int(seed))
+
+    def _fit(self, df):
+        from b200flow import fm as bfm
+        params = self._check()
+        fc, y = _features_and_label(self, df)
+        try:
+            fit = bfm.fm_regression_fit(fc.data, y, params, group=bdist.group())
+        except ValueError as e:        # includes b200flow's UnsupportedParamError
+            raise IllegalArgumentException(str(e))
+        m = FMRegressionModel(fit)
+        m._paramMap = {k: v for k, v in self._paramMap.items() if k in m._all_defaults()}
+        return m
+
+
+class FMRegressionModel(Model, _FMRegressorParams):
+    """intercept, linear (DenseVector [D]), factors (DenseMatrix D x k); prediction = r, the factorization machine's raw
+    value.  Spark has no training summary for this model."""
+
+    def __init__(self, fit):
+        super().__init__()
+        self._fit_result = fit             # b200flow.fm.FMFit
+
+    @property
+    def intercept(self):
+        return self._fit_result.intercept
+
+    @property
+    def linear(self):
+        from .linalg import DenseVector
+        return DenseVector(self._fit_result.linear.copy())
+
+    @property
+    def factors(self):
+        from .linalg import DenseMatrix
+        f = self._fit_result.factors
+        return DenseMatrix(f.shape[0], f.shape[1], f.T.reshape(-1))
+
+    @property
+    def numFeatures(self):
+        return int(self._fit_result.factors.shape[0])
+
+    def _weights(self):
+        """[1, D (k + 1) + 1] f64 host: [V (row-major) | w | b], fm_raw's layout"""
+        f = self._fit_result
+        return torch.from_numpy(np.concatenate([f.factors.reshape(-1), f.linear, [f.intercept]])).reshape(1, -1)
+
+    def _raw(self, x):
+        from b200flow import fm as bfm
+        try:
+            return bfm.fm_raw(x, self._weights(), self._fit_result.factors.shape[1])[:, 0].contiguous()
+        except ValueError as e:
+            raise IllegalArgumentException(str(e))
+
+    def predict(self, features):
+        """the prediction for one feature vector, transform's arithmetic"""
+        v = np.asarray(features.toArray() if hasattr(features, "toArray") else features, np.float64).reshape(1, -1)
+        return float(self._raw(torch.from_numpy(v).cuda())[0].item())
+
+    def _transform(self, df):
+        fcol = self.getOrDefault("featuresCol")
+        if fcol not in df._cols or df._cols[fcol].kind != "vector":
+            raise IllegalArgumentException("Column %s must be of type vector" % fcol)
+        pcol = self.getOrDefault("predictionCol")
+        if not pcol:
+            return df
+        if pcol in df._cols:
+            raise IllegalArgumentException("Output column %s already exists." % pcol)
+        cols = dict(df._cols)
+        cols[pcol] = ColumnData("numeric", self._raw(df._cols[fcol].data), "f64")
+        return df._with(cols=cols)
+
+    def __repr__(self):
+        return "FMRegressionModel: uid=%s, numFeatures=%d, factorSize=%d" % (self.uid, self.numFeatures,
+                                                                              self._fit_result.factors.shape[1])

@@ -13,10 +13,14 @@ It reports
   * a binary fit (normal vs attack) at the defaults, host-timed after one untimed fit;
   * OneVsRest(FMClassifier) at maxIter = --ovr-max-iter: the class-batched fit against K standalone fits run one after
     the other, both host-timed, and a hash of every model of each (they must be equal);
-  * the OneVsRest transform (K raw values in one launch and the first argmax), CUDA events, median of --repeats.
+  * the OneVsRest transform (K raw values in one launch and the first argmax), CUDA events, median of --repeats;
+  * FMRegressor: one squared-error evaluation (b200flow.fm.fm_regression_loss_grad_totals) against the torch fp64 arm,
+    as above, and a fit at the defaults but stepSize 0.01, host-timed after one untimed fit, of a seeded label with a
+    pairwise and a linear part.  --regressor-only skips the classifier arms.
 One JSON line.
 
     python tools/bench_fm.py [--rows 4898431] [--classes 23] [--factor-size 8] [--repeats 10] [--ovr-max-iter 30]
+                             [--regressor-only]
 """
 import argparse
 import hashlib
@@ -51,7 +55,8 @@ def work(n, D, kf, K):
 
 
 def torch_totals(x, y, pos, w, kf):
-    """the same totals as fm_loss_grad_totals ([K, D (k + 1) + D + 3]) with cuBLAS and torch ops, over row blocks"""
+    """the same totals as fm_loss_grad_totals ([K, D (k + 1) + D + 3]) with cuBLAS and torch ops, over row blocks; pos None:
+    fm_regression_loss_grad_totals' squared error against the f64 labels y"""
     n, D = x.shape
     K, nv = w.shape[0], D * kf
     U = torch.cat([w[:, :nv].reshape(K, D, kf), w[:, nv:nv + D].reshape(K, D, 1)], 2).permute(1, 0, 2).reshape(D, -1)
@@ -64,9 +69,14 @@ def torch_totals(x, y, pos, w, kf):
         S = (xc @ U).view(m, K, kf + 1)
         Q = (x2 @ U2).view(m, K, kf + 1)
         r = b + S[:, :, kf] + 0.5 * (S[:, :, :kf] * S[:, :, :kf] - Q[:, :, :kf]).sum(2)
-        yk = (yc.long()[:, None] == pos.long()[None, :]).to(torch.float64)
-        g = torch.sigmoid(r) - yk
-        loss = torch.where(yk > 0, torch.nn.functional.softplus(-r), torch.nn.functional.softplus(r)).sum(0)
+        if pos is None:
+            d = r - yc[:, None]
+            g = 2.0 * d
+            loss = (d * d).sum(0)
+        else:
+            yk = (yc.long()[:, None] == pos.long()[None, :]).to(torch.float64)
+            g = torch.sigmoid(r) - yk
+            loss = torch.where(yk > 0, torch.nn.functional.softplus(-r), torch.nn.functional.softplus(r)).sum(0)
         M = S * g[:, :, None]
         M[:, :, kf] = g
         G = (xc.t() @ M.view(m, -1)).view(D, K, kf + 1)
@@ -94,6 +104,7 @@ def main():
     ap.add_argument("--factor-size", type=int, default=8)
     ap.add_argument("--repeats", type=int, default=10)
     ap.add_argument("--ovr-max-iter", type=int, default=30)
+    ap.add_argument("--regressor-only", action="store_true")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_fm.py needs a CUDA device")
@@ -106,12 +117,8 @@ def main():
     sh = bdist.Shards(n, 0, None, x.device)
     rng = np.random.default_rng(1)
     med = lambda ts: sorted(ts)[len(ts) // 2]                             # noqa: E731
-    evals = {}
-    for k in (1, K):
-        pos = torch.arange(k, dtype=torch.int32, device="cuda")
-        w = torch.from_numpy(rng.normal(0.0, 0.05, (k, D * (kf + 1) + 1))).cuda()
-        ours = lambda: bfm.fm_loss_grad_totals(x, y, pos, w, kf, 1.0, 43, sh)   # noqa: E731
-        ref = lambda: torch_totals(x, y, pos, w, kf)                           # noqa: E731
+
+    def timed_eval(ours, ref, nbytes, flops):
         for f in (ours, ref, ours, ref):                                   # warm-up: modules, cuBLAS algorithms
             f()
         torch.cuda.synchronize()
@@ -127,13 +134,38 @@ def main():
         got, want = ours(), ref()
         diff = float(((got - want).abs().max() / want.abs().max()).item())
         ms = med(t_ours)
-        nbytes, flops = work(n, D, kf, k)
         tb, tf = nbytes / PEAK_HBM, flops / PEAK_FP64_TC
-        evals["K%d" % k] = {"ms": round(ms, 3), "torch_fp64_ms": round(med(t_ref), 3), "max_rel_diff": diff,
-                            "gb_per_s": round(nbytes / (ms * 1e-3) / 1e9, 1), "fp64_tflops": round(flops / (ms * 1e-3) / 1e12, 2),
-                            "datasheet_bound_ms": round(max(tb, tf) * 1e3, 3), "bound": "fp64" if tf >= tb else "hbm",
-                            "share_of_bound": round(max(tb, tf) / (ms * 1e-3), 4)}
-        del got, want
+        return {"ms": round(ms, 3), "torch_fp64_ms": round(med(t_ref), 3), "max_rel_diff": diff,
+                "gb_per_s": round(nbytes / (ms * 1e-3) / 1e9, 1), "fp64_tflops": round(flops / (ms * 1e-3) / 1e12, 2),
+                "datasheet_bound_ms": round(max(tb, tf) * 1e3, 3), "bound": "fp64" if tf >= tb else "hbm",
+                "share_of_bound": round(max(tb, tf) / (ms * 1e-3), 4)}
+
+    # FMRegressor: a label with a pairwise and a linear part, and noise
+    beta = torch.from_numpy(rng.normal(0.0, 0.3, D)).cuda()
+    yr = (x[:, 0] * x[:, 1] + x @ beta + 0.5 * torch.from_numpy(rng.normal(0.0, 1.0, n)).cuda()).contiguous()
+    wr = torch.from_numpy(rng.normal(0.0, 0.05, (1, D * (kf + 1) + 1))).cuda()
+    nbytes, flops = work(n, D, kf, 1)
+    regressor = {"eval": timed_eval(lambda: bfm.fm_regression_loss_grad_totals(x, yr, wr, kf, 1.0, 43, sh),
+                                    lambda: torch_totals(x, yr, None, wr, kf), nbytes + 4.0 * n, flops)}
+    pr = bfm.FMParams(factor_size=kf, step_size=0.01, seed=11)            # stepSize 1.0 diverges on these heavy tails
+    bfm.fm_regression_fit(x, yr, pr)                                       # untimed fit
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    rfit = bfm.fm_regression_fit(x, yr, pr)
+    torch.cuda.synchronize()
+    regressor.update(fit_s=round(time.perf_counter() - t0, 3), step_size=pr.step_size, iterations=rfit.iterations,
+                     first_objective=rfit.objective_history[0], objective=rfit.objective_history[-1],
+                     label_variance=float(yr.var().item()))
+    if a.regressor_only:
+        print(json.dumps({"rows": n, "D": D, "factor_size": kf, "regressor": regressor, "card": dev_card}), flush=True)
+        return
+    evals = {}
+    for k in (1, K):
+        pos = torch.arange(k, dtype=torch.int32, device="cuda")
+        w = torch.from_numpy(rng.normal(0.0, 0.05, (k, D * (kf + 1) + 1))).cuda()
+        nbytes, flops = work(n, D, kf, k)
+        evals["K%d" % k] = timed_eval(lambda: bfm.fm_loss_grad_totals(x, y, pos, w, kf, 1.0, 43, sh),
+                                      lambda: torch_totals(x, y, pos, w, kf), nbytes, flops)
     # binary fit at the defaults: normal (label 0 after StringIndexer's frequency order) vs attack
     yb = (y != 0).to(torch.int32)
     p = bfm.FMParams(factor_size=kf, seed=11)
@@ -172,7 +204,8 @@ def main():
         "ovr_max_iter": a.ovr_max_iter, "ovr_batched_s": round(batched_s, 3), "ovr_sequential_s": round(seq_s, 3),
         "ovr_batched_hash": model_hash(batched), "ovr_sequential_hash": model_hash(seq),
         "ovr_iterations": sorted({f.iterations for f in batched}),
-        "transform_ms": round(med(tr), 3), "train_accuracy": round(acc, 4), "card": dev_card}), flush=True)
+        "transform_ms": round(med(tr), 3), "train_accuracy": round(acc, 4), "regressor": regressor, "card": dev_card}),
+        flush=True)
 
 
 if __name__ == "__main__":
