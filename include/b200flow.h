@@ -351,6 +351,24 @@ int b200flow_predict(const uint8_t* tp, int32_t tp_stride, int64_t n_rows,
 int b200flow_build_top_nodes(const b200flow_node* nodes, const int32_t* node_tree, int64_t n_nodes, int32_t T,
                              int32_t top_levels, void* top, void* stream);
 
+/* per-tree compact layout for b200flow_predict_forest, built once per model in two calls.  Tree t (t < T; pool nodes of
+ * other trees are ignored) owns the 8-byte words [tree_off[t], tree_off[t+1]) of `layout`: its nodes in pool order (8-byte
+ * records, child and payload offsets local to the tree), the C fp64 votes of its leaves (leaf_prob, or pool_counts as fp64
+ * when dt_mode != 0) and the left-set masks of its categorical splits.
+ * b200flow_forest_layout_size fills tree_off[T+1] (tree_off[T] = the words `layout` must hold) and the int32 scratch
+ * [2*n_nodes + 4*T]; b200flow_build_forest_layout then writes `layout` (16-byte aligned) from the same scratch. */
+int b200flow_forest_layout_size(const b200flow_node* nodes, const int32_t* node_tree, int64_t n_nodes, int32_t T, int32_t C,
+                                int32_t* scratch, int64_t* tree_off, void* stream);
+int b200flow_build_forest_layout(const b200flow_node* nodes, const uint64_t* node_mask, const double* leaf_prob,
+                                 const uint32_t* pool_counts, const int32_t* node_tree, int64_t n_nodes, int32_t T, int32_t C,
+                                 int32_t dt_mode, const int32_t* scratch, const int64_t* tree_off, uint64_t* layout, void* stream);
+
+/* R9 over the compact layout: what b200flow_predict computes (raw, prob, pred bit for bit; raw/prob may be NULL), with each
+ * tree staged whole in shared memory (the first words of a tree larger than the buffer; the rest read from global).
+ * F = features (bins tp[row][0..F-1]). */
+int b200flow_predict_forest(const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows, const uint64_t* layout,
+                            const int64_t* tree_off, int32_t T, int32_t C, double* raw, double* prob, double* pred, void* stream);
+
 /* R9 helper (model.transform, kdd99.py:82, cicids17.py:86): out[i] = src[idx[i]] for rows of row_bytes (multiple of 4): spreads the predictions computed once per UNIQUE test record
  * (b200flow_dedup_rows) back to the rows. */
 int b200flow_gather_rows(const void* src, int32_t row_bytes, const int32_t* idx, int64_t n_rows, void* out, void* stream);

@@ -64,6 +64,9 @@ _SIGNATURES = {
     "b200flow_finalize_forest": [_I64, _P, _I32, _P, _P],
     "b200flow_predict": [_P, _I32, _I64, _P, _P, _P, _P, _I32, _I32, _I32, _P, _I32, _P, _P, _P, _P],
     "b200flow_build_top_nodes": [_P, _P, _I64, _I32, _I32, _P, _P],
+    "b200flow_forest_layout_size": [_P, _P, _I64, _I32, _I32, _P, _P, _P],
+    "b200flow_build_forest_layout": [_P, _P, _P, _P, _P, _I64, _I32, _I32, _I32, _P, _P, _P, _P],
+    "b200flow_predict_forest": [_P, _I32, _I32, _I64, _P, _P, _I32, _I32, _P, _P, _P, _P],
     "b200flow_gather_rows": [_P, _I32, _P, _I64, _P, _P],
     "b200flow_confusion": [_P, _P, _I64, _I32, _P, _P],
     "b200flow_predict_grid_confusion": [_P, _I32, _I32, _I64, _P, _P, _P, _P, _P, _I32, _I32, _I32, _P, _I32, _P, _I32, _P, _I32,

@@ -254,15 +254,33 @@ class ForestModel:
             call("b200flow_build_top_nodes", ptr(self.nodes), ptr(self.node_tree), self.n_nodes, self.T, TOP_LEVELS, ptr(self._top))
         return self._top, TOP_LEVELS
 
+    def _forest_layout(self):
+        """(layout uint64 [words], tree_off int64 [T+1]): every tree's nodes, left-set masks and leaf votes in one contiguous
+        block, which the predict kernel stages whole in shared memory (built once per model; one host read of the size)."""
+        if getattr(self, "_layout", None) is None:
+            dev = self.nodes.device
+            scratch = torch.empty(2 * self.n_nodes + 4 * self.T, dtype=torch.int32, device=dev)
+            tree_off = torch.empty(self.T + 1, dtype=torch.int64, device=dev)
+            call("b200flow_forest_layout_size", ptr(self.nodes), ptr(self.node_tree), self.n_nodes, self.T, self.C, ptr(scratch),
+                 ptr(tree_off))
+            layout = torch.empty(max(int(tree_off[self.T].item()), 2), dtype=torch.int64, device=dev)
+            call("b200flow_build_forest_layout", ptr(self.nodes), ptr(self.node_mask), ptr(self.leaf_prob), ptr(self.pool_counts),
+                 ptr(self.node_tree), self.n_nodes, self.T, self.C, 1 if self.dt_mode else 0, ptr(scratch), ptr(tree_off),
+                 ptr(layout))
+            self._layout = (layout, tree_off)
+        return self._layout
+
     def predict_binned(self, tp, want_raw=True, want_prob=True):
         n = tp.shape[0]
         dev = tp.device
         raw = torch.empty((n, self.C), dtype=torch.float64, device=dev) if want_raw else None
         prob = torch.empty((n, self.C), dtype=torch.float64, device=dev) if want_prob else None
         pred = torch.empty(n, dtype=torch.float64, device=dev)
-        top, K = self._top_table()
-        _timed("predict", "b200flow_predict", ptr(tp), tp.shape[1], n, ptr(self.nodes), ptr(self.node_mask), ptr(self.leaf_prob),
-             ptr(self.pool_counts), self.T, self.C, 1 if self.dt_mode else 0, ptr(top), K, ptr(raw), ptr(prob), ptr(pred))
+        if n == 0:
+            return raw, prob, pred
+        layout, tree_off = self._forest_layout()
+        _timed("predict", "b200flow_predict_forest", ptr(tp), tp.shape[1], self.F, n, ptr(layout), ptr(tree_off), self.T, self.C,
+               ptr(raw), ptr(prob), ptr(pred))
         return raw, prob, pred
 
     def predict(self, x, want_raw=True, want_prob=True):

@@ -79,6 +79,7 @@ class GBTRegressionModel:
         top, _ = fo._top_table()
         if top is not None:                              # heap-indexed per tree: the first k trees' rows are the prefix's
             pre._top = top
+        pre._layout = fo._forest_layout()                # per-tree blocks in tree order: the first k are the prefix's
         return pre
 
     def prefix_predictions(self, x):

@@ -4,6 +4,7 @@
 // Reference call sites: model.transform(test_set) kdd99.py:82 / cicids17.py:86; evaluator.evaluate
 // kdd99.py:86-91; randomSplit kdd99.py:52; where / handleInvalid="skip" cicids17.py:30-35,41.
 #include <stdlib.h>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -119,6 +120,242 @@ __global__ void __launch_bounds__(128) predict_kernel(const uint8_t* __restrict_
         }
         if (top) { cp_async_wait_all(); __syncthreads(); }                  // the look-ahead copy of the last tree is a no-op commit
     }
+}
+
+// ------------------------------------------------------------------ R9 predict over the per-tree compact layout
+// predict_kernel's walk is bound by L1 tag lookups: below the heap-indexed top table every lane's node load (and, at the
+// leaf, each of its C vote loads) is a separate request.  A KDD tree is small once compacted (~1,900 nodes: ~15 KB of
+// 8-byte nodes plus ~37 KB of C = 5 fp64 leaf votes), so the whole tree is staged in shared memory and every walk step and
+// vote add becomes a scattered LDS.
+//
+// Layout (8-byte words), built once per model: tree t owns words [tree_off[t], tree_off[t+1]), padded to an even count.
+//   [0, n_t)            node records in pool order (the pool is level-major, so this is the tree's BFS order), uint2 {a, b}:
+//                         a = feat | min(bin_thr, 255) << 16 | kCat | kLeaf, b = word offset in the tree's block of
+//                         the left child (continuous split), of the categorical record (categorical split) or of the C
+//                         fp64 votes (leaf).  The root is word 0; a node's right child is its left child + 1.
+//   [n_t, ...)          one 5-word record per categorical split: left child, then the 4-word left-set mask
+//   [..., end)          the leaves' C fp64 votes (leaf_prob, or pool_counts as fp64 in dt_mode), in leaf order
+// The categorical records, read at every categorical step, come before the votes, read once per walk: a tree larger than
+// the shared-memory buffer leaves its votes in global memory first.
+// All offsets are 32-bit, so a tree of any size is exact.
+constexpr uint32_t kLayoutLeaf = 1u << 31, kLayoutCat = 1u << 30;
+constexpr int kLayoutCatWords = 5;
+constexpr int kLayoutRankBlock = 1024, kLayoutRankPer = 4;
+constexpr int kVoteBatch = 8;                                                 // leaf votes loaded together (C = 5 on KDD99)
+constexpr int kPredForestRegC = 8;                                           // classes whose votes accumulate in registers
+constexpr int kPredForestRegThreads = 896;                                   // its block bound: 72 registers, no spills
+
+// block-wide exclusive scan of one uint64 per thread (blockDim == kLayoutRankBlock); sh holds 33 words
+__device__ __forceinline__ unsigned long long block_exclusive_scan_u64(unsigned long long v, unsigned long long* sh,
+                                                                      unsigned long long* total) {
+    const unsigned long long inc = warp_inclusive_scan(v);
+    if (lane_id() == 31) sh[warp_id()] = inc;
+    __syncthreads();
+    if (warp_id() == 0) {
+        const unsigned long long w = sh[lane_id()];
+        const unsigned long long winc = warp_inclusive_scan(w);
+        sh[lane_id()] = winc - w;
+        if (lane_id() == 31) sh[32] = winc;
+    }
+    __syncthreads();
+    const unsigned long long res = inc - v + sh[warp_id()];
+    *total = sh[32];
+    __syncthreads();                                                          // sh is reused by the next chunk
+    return res;
+}
+
+// one CTA per tree t: scans the pool in order and gives each of t's nodes its rank in the tree (local[i]) and its rank
+// among the tree's leaves or categorical splits (ord[i]); cnt[t] = {nodes, leaves, categorical splits}, words[t] = the
+// tree's block size.  Counts travel packed in 21-bit fields of one uint64 (a chunk holds 4096 nodes).
+__global__ void __launch_bounds__(kLayoutRankBlock) layout_rank_kernel(const int4* __restrict__ nodes,
+                                                                        const int32_t* __restrict__ node_tree, int64_t n, int C,
+                                                                        int32_t* local, int32_t* ord, int32_t* cnt, int32_t* words) {
+    __shared__ unsigned long long sh[33];
+    const int t = blockIdx.x;
+    constexpr unsigned long long kOne = 1ull, kLeafOne = 1ull << 21, kCatOne = 1ull << 42, kField = (1ull << 21) - 1;
+    int64_t base_n = 0, base_l = 0, base_c = 0;
+    for (int64_t c0 = 0; c0 < n; c0 += (int64_t)kLayoutRankBlock * kLayoutRankPer) {
+        const int64_t i0 = c0 + (int64_t)threadIdx.x * kLayoutRankPer;
+        unsigned long long inc[kLayoutRankPer], v = 0;
+#pragma unroll
+        for (int j = 0; j < kLayoutRankPer; ++j) {
+            inc[j] = 0;
+            const int64_t i = i0 + j;
+            if (i < n && node_tree[i] == t) {
+                const int4 nd = __ldg(nodes + i);
+                inc[j] = kOne | (nd.x < 0 ? kLeafOne : ((uint32_t)nd.y >= 65536u ? kCatOne : 0ull));
+            }
+            v += inc[j];
+        }
+        unsigned long long total;
+        unsigned long long pre = block_exclusive_scan_u64(v, sh, &total);
+#pragma unroll
+        for (int j = 0; j < kLayoutRankPer; ++j) {
+            if (inc[j]) {
+                const int64_t i = i0 + j;
+                local[i] = (int32_t)(base_n + (pre & kField));
+                ord[i] = (int32_t)((inc[j] & kLeafOne) ? base_l + ((pre >> 21) & kField)
+                                                       : base_c + ((pre >> 42) & kField));
+            }
+            pre += inc[j];
+        }
+        base_n += total & kField; base_l += (total >> 21) & kField; base_c += (total >> 42) & kField;
+    }
+    if (threadIdx.x == 0) {
+        cnt[3 * t] = (int32_t)base_n; cnt[3 * t + 1] = (int32_t)base_l; cnt[3 * t + 2] = (int32_t)base_c;
+        const int64_t w = base_n + base_l * C + base_c * kLayoutCatWords;
+        words[t] = (int32_t)((w + 1) & ~1ll);                                 // even: every tree block starts 16-byte aligned
+    }
+}
+
+// one thread per pool node of trees [0, T): its node record, and its votes or categorical record
+__global__ void __launch_bounds__(256) layout_fill_kernel(const int4* __restrict__ nodes,
+                                                          const unsigned long long* __restrict__ node_mask,
+                                                          const double* __restrict__ leaf_prob,
+                                                          const uint32_t* __restrict__ pool_counts,
+                                                          const int32_t* __restrict__ node_tree, int64_t n, int T, int C,
+                                                          int dt_mode, const int32_t* __restrict__ local,
+                                                          const int32_t* __restrict__ ord, const int32_t* __restrict__ cnt,
+                                                          const int64_t* __restrict__ tree_off, uint2* layout) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const int t = node_tree[i];
+    if (t < 0 || t >= T) return;
+    uint2* blk = layout + tree_off[t];
+    const int4 nd = nodes[i];
+    const uint32_t n_t = (uint32_t)cnt[3 * t], c_t = (uint32_t)cnt[3 * t + 2];
+    uint2 rec;
+    if (nd.x < 0) {
+        const uint32_t vo = n_t + c_t * kLayoutCatWords + (uint32_t)ord[i] * (uint32_t)C;
+        rec = make_uint2(kLayoutLeaf, vo);
+        double* v = (double*)(blk + vo);
+        if (dt_mode) { for (int k = 0; k < C; ++k) v[k] = (double)pool_counts[i * C + k]; }
+        else { for (int k = 0; k < C; ++k) v[k] = leaf_prob[i * C + k]; }
+    } else if ((uint32_t)nd.y >= 65536u) {
+        const uint32_t co = n_t + (uint32_t)ord[i] * kLayoutCatWords;
+        rec = make_uint2((uint32_t)nd.x | kLayoutCat, co);
+        blk[co] = make_uint2((uint32_t)local[nd.z], 0u);
+        unsigned long long* m = (unsigned long long*)(blk + co + 1);
+        for (int q = 0; q < 4; ++q) m[q] = node_mask ? node_mask[i * 4 + q] : 0ull;
+    } else {
+        const uint32_t thr = (uint32_t)nd.y < 255u ? (uint32_t)nd.y : 255u;   // bins are bytes: a threshold >= 255 sends all left
+        rec = make_uint2((uint32_t)nd.x | (thr << 16), (uint32_t)local[nd.z]);
+    }
+    blk[local[i]] = rec;
+}
+
+// A CTA owns a block of rows (one per thread; bins transposed in shared memory as in predict_kernel) and walks them
+// through the trees in order.  Tree t's block is staged with cp.async into one of two buffers while tree t-1 is walked; a
+// word at offset o of the block is read from shared memory when o < cap (the buffer size) and from global memory otherwise,
+// so a tree larger than the buffer keeps its first (top-level) nodes in shared memory.  A tree that fits is walked by the
+// same code compiled without the bound check, which saves the compare and select on every load.  The last tree of a round
+// stages tree 0 of the next.  Votes add in fp64, in tree order, from 0.0: predict_kernel's adds, bit for bit.
+// kRegC > 0 (C <= kRegC): the votes accumulate in registers, not in shared memory: no shared-memory read-modify-write per
+// class and leaf, and 8·C more bytes per row for the tree buffers (every KDD99 tree then fits).  The bin of feature f is one
+// byte load from the thread's column: byte f & 3 of word f >> 2, at (f >> 2)·4·bd + (f & 3) = (f & ~3)·bd + (f & 3).
+template <int kRegC>
+__global__ void __launch_bounds__(kRegC ? kPredForestRegThreads : 1024, 1)
+predict_forest_kernel(const uint8_t* __restrict__ tp, int stride, int fwords, int64_t n, const uint2* __restrict__ layout,
+                      const int64_t* __restrict__ tree_off, int T, int C, int cap, double* raw, double* prob, double* pred) {
+    extern __shared__ __align__(16) uint8_t sm[];
+    const int bd = blockDim.x, tid = threadIdx.x;
+    uint32_t* binw = (uint32_t*)sm;                                           // [fwords][bd]
+    double* votes = (double*)(sm + (size_t)fwords * bd * 4);                  // [C][bd] (kRegC == 0)
+    uint2* tbuf = (uint2*)(votes + (kRegC ? 0 : (size_t)C * bd));             // [2][cap]
+    auto stage = [&](int t, int buf) {
+        if (t >= 0) {
+            const int64_t o = tree_off[t];
+            const int64_t w = tree_off[t + 1] - o < cap ? tree_off[t + 1] - o : cap;
+            const uint4* src = (const uint4*)(layout + o);
+            uint4* dst = (uint4*)(tbuf + (size_t)buf * cap);
+            for (int i = tid; i < (int)(w >> 1); i += bd) cp_async16(dst + i, src + i);
+        }
+        cp_async_commit();
+    };
+    const int64_t round_rows = (int64_t)gridDim.x * bd;
+    const uint8_t* bb = (const uint8_t*)(binw + tid);                         // this thread's column of the transposed bins
+    double* vt = votes + tid;
+    int g = 0;                                                                // trees walked by this CTA: buffer parity
+    if ((int64_t)blockIdx.x * bd < n) stage(0, 0);
+    for (int64_t base = (int64_t)blockIdx.x * bd; base < n; base += round_rows) {
+        const int64_t row = base + tid;
+        const bool live = row < n;
+        if (live) {
+            const uint4* src = (const uint4*)(tp + row * stride);
+            for (int q = 0; q < fwords / 4; ++q) {
+                const uint4 v = ld_stream_u4(src + q);
+                binw[(4 * q + 0) * bd + tid] = v.x; binw[(4 * q + 1) * bd + tid] = v.y;
+                binw[(4 * q + 2) * bd + tid] = v.z; binw[(4 * q + 3) * bd + tid] = v.w;
+            }
+        }
+        double acc[kRegC > 0 ? kRegC : 1];
+#pragma unroll
+        for (int k = 0; k < (kRegC > 0 ? kRegC : 1); ++k) acc[k] = 0.0;
+        if (!kRegC) for (int k = 0; k < C; ++k) vt[k * bd] = 0.0;
+        for (int t = 0; t < T; ++t, ++g) {
+            cp_async_wait_all();
+            __syncthreads();                                                // tree t landed; everybody left tree t-1
+            stage(t + 1 < T ? t + 1 : (base + round_rows < n ? 0 : -1), (g + 1) & 1);
+            const uint2* tb = tbuf + (size_t)(g & 1) * cap;
+            const uint2* gb = layout + tree_off[t];
+            const bool whole = tree_off[t + 1] - tree_off[t] <= cap;
+            auto walk = [&](auto whole_tag) {
+                constexpr bool kWhole = decltype(whole_tag)::value;
+                auto word = [&](uint32_t o) -> uint2 { return (kWhole || o < (uint32_t)cap) ? tb[o] : __ldg(gb + o); };
+                if (!live) return;
+                uint2 nd = word(0);
+                while (!(nd.x & kLayoutLeaf)) {
+                    const uint32_t f = nd.x & 0xffff;
+                    const uint32_t bin = bb[(f & ~3u) * bd + (f & 3u)];
+                    uint32_t next;
+                    if (nd.x & kLayoutCat) {
+                        const uint2 m = word(nd.y + 1 + (bin >> 6));
+                        next = word(nd.y).x + !((((bin & 32) ? m.y : m.x) >> (bin & 31)) & 1u);
+                    } else {
+                        next = nd.y + (bin > ((nd.x >> 16) & 0xff));
+                    }
+                    nd = word(next);
+                }
+                if (kRegC) {
+#pragma unroll
+                    for (int k = 0; k < kRegC; ++k)
+                        if (k < C) { const uint2 w = word(nd.y + k); acc[k] += __hiloint2double((int)w.y, (int)w.x); }
+                } else {
+                    for (int k0 = 0; k0 < C; k0 += kVoteBatch) {                // the batch's loads issue before its adds
+                        uint2 w[kVoteBatch];
+#pragma unroll
+                        for (int j = 0; j < kVoteBatch; ++j) if (k0 + j < C) w[j] = word(nd.y + k0 + j);
+#pragma unroll
+                        for (int j = 0; j < kVoteBatch; ++j)
+                            if (k0 + j < C) vt[(k0 + j) * bd] += __hiloint2double((int)w[j].y, (int)w[j].x);
+                    }
+                }
+            };
+            if (whole) walk(std::integral_constant<bool, true>()); else walk(std::integral_constant<bool, false>());
+        }
+        if (!live) continue;
+        if (kRegC) {
+            double s = 0.0; int arg = 0; double best = acc[0];
+#pragma unroll
+            for (int k = 0; k < kRegC; ++k) if (k < C) { s += acc[k]; if (acc[k] > best) { best = acc[k]; arg = k; } }
+#pragma unroll
+            for (int k = 0; k < kRegC; ++k) if (k < C) {
+                if (raw) raw[row * C + k] = acc[k];
+                if (prob) prob[row * C + k] = s != 0.0 ? acc[k] / s : 0.0;
+            }
+            pred[row] = (double)arg;
+        } else {
+            double s = 0.0; int arg = 0; double best = vt[0];
+            for (int k = 0; k < C; ++k) { const double v = vt[k * bd]; s += v; if (v > best) { best = v; arg = k; } }
+            for (int k = 0; k < C; ++k) {
+                const double v = vt[k * bd];
+                if (raw) raw[row * C + k] = v;
+                if (prob) prob[row * C + k] = s != 0.0 ? v / s : 0.0;
+            }
+            pred[row] = (double)arg;
+        }
+    }
+    cp_async_wait_all();                                                    // nothing in flight when the CTA exits
 }
 
 // ------------------------------------------------------------------ row gather (predictions of unique records -> rows)
@@ -368,6 +605,69 @@ extern "C" int b200flow_predict(const uint8_t* tp, int32_t tp_stride, int64_t n_
     }
     if (e != cudaSuccess) { set_error("predict: %s", cudaGetErrorString(e)); return B200FLOW_ERR_CUDA; }
     return check_launch("predict");
+}
+
+extern "C" int b200flow_forest_layout_size(const b200flow_node* nodes, const int32_t* node_tree, int64_t n_nodes, int32_t T,
+                                           int32_t C, int32_t* scratch, int64_t* tree_off, void* stream) {
+    B2F_REQUIRE(nodes && node_tree && scratch && tree_off && T > 0 && C > 0 && n_nodes >= T, "forest_layout_size: bad arguments");
+    // every offset in a tree's block is 32-bit and the rank kernel counts at most 2^21 per chunk field: bound the words
+    B2F_REQUIRE(n_nodes * ((int64_t)C + kLayoutCatWords + 1) < ((int64_t)1 << 31), "forest_layout_size: forest too large for 32-bit offsets");
+    cudaStream_t st = (cudaStream_t)stream;
+    int32_t* local = scratch; int32_t* ord = scratch + n_nodes; int32_t* cnt = ord + n_nodes; int32_t* words = cnt + 3 * (int64_t)T;
+    layout_rank_kernel<<<T, kLayoutRankBlock, 0, st>>>((const int4*)nodes, node_tree, n_nodes, C, local, ord, cnt, words);
+    const int rc = check_launch("forest_layout_size");
+    if (rc) return rc;
+    return b200flow_exclusive_scan_i32_to_i64(words, T, tree_off, tree_off + T, stream);
+}
+
+extern "C" int b200flow_build_forest_layout(const b200flow_node* nodes, const uint64_t* node_mask, const double* leaf_prob,
+                                            const uint32_t* pool_counts, const int32_t* node_tree, int64_t n_nodes, int32_t T,
+                                            int32_t C, int32_t dt_mode, const int32_t* scratch, const int64_t* tree_off,
+                                            uint64_t* layout, void* stream) {
+    B2F_REQUIRE(nodes && node_tree && scratch && tree_off && layout && T > 0 && C > 0 && n_nodes >= T && ((uintptr_t)layout & 15) == 0,
+                "build_forest_layout: bad arguments");
+    B2F_REQUIRE(dt_mode ? pool_counts != nullptr : leaf_prob != nullptr, "build_forest_layout: missing leaf payload");
+    const int32_t* local = scratch; const int32_t* ord = scratch + n_nodes; const int32_t* cnt = ord + n_nodes;
+    layout_fill_kernel<<<(unsigned)((n_nodes + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
+        (const int4*)nodes, (const unsigned long long*)node_mask, leaf_prob, pool_counts, node_tree, n_nodes, T, C, dt_mode,
+        local, ord, cnt, tree_off, (uint2*)layout);
+    return check_launch("build_forest_layout");
+}
+
+// shared memory of predict_forest_kernel: the rows take at most half of kPredForestSmem, the two tree buffers the rest
+constexpr size_t kPredForestSmem = 227 * 1024;              // the H100's opt-in maximum per CTA
+
+extern "C" int b200flow_predict_forest(const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows, const uint64_t* layout,
+                                       const int64_t* tree_off, int32_t T, int32_t C, double* raw, double* prob, double* pred,
+                                       void* stream) {
+    if (n_rows <= 0) return B200FLOW_OK;            // empty batch: nothing to do (pointers may be NULL)
+    B2F_REQUIRE(tp && layout && tree_off && pred && T > 0 && C > 0 && F > 0 && F < 65536 && F <= tp_stride && (tp_stride & 15) == 0,
+                "predict_forest: bad arguments");
+    B2F_REQUIRE(((uintptr_t)tp & 15) == 0 && ((uintptr_t)layout & 15) == 0, "predict_forest: tp and layout must be 16-byte aligned");
+    const bool reg = C <= kPredForestRegC;          // votes in registers
+    const int fwords = (F + 15) / 16 * 4;           // bin words a row keeps (whole 16-byte loads; <= tp_stride / 4)
+    const size_t row_bytes = (size_t)fwords * 4 + (reg ? 0 : (size_t)C * 8);
+    const int64_t max_bd = reg ? kPredForestRegThreads : 1024;
+    int64_t bd = (int64_t)(kPredForestSmem / 2 / row_bytes) / 32 * 32;
+    if (bd > max_bd) bd = max_bd;
+    if (bd < 32) bd = 32;
+    B2F_REQUIRE((size_t)bd * row_bytes + 16 <= kPredForestSmem, "predict_forest: too many classes/features for shared memory");
+    // as few rounds as the widest block allows, with the rows spread evenly over them and the SMs
+    const int64_t rounds = (n_rows + (int64_t)kNumSMs * bd - 1) / ((int64_t)kNumSMs * bd);
+    const int64_t want = (n_rows + (int64_t)kNumSMs * rounds - 1) / ((int64_t)kNumSMs * rounds);
+    bd = (want + 31) / 32 * 32 < bd ? (want + 31) / 32 * 32 : bd;
+    const int grid = grid_for(n_rows, (int)bd, kNumSMs);
+    const size_t rows_smem = (size_t)bd * row_bytes;
+    const int cap = (int)((kPredForestSmem - rows_smem) / 16) & ~1;   // words per tree buffer, even
+    const size_t smem = rows_smem + (size_t)2 * cap * 8;
+    const void* fn = reg ? (const void*)predict_forest_kernel<kPredForestRegC> : (const void*)predict_forest_kernel<0>;
+    cudaError_t e = cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { set_error("predict_forest: %s", cudaGetErrorString(e)); return B200FLOW_ERR_CUDA; }
+    if (reg) predict_forest_kernel<kPredForestRegC><<<grid, (int)bd, smem, (cudaStream_t)stream>>>(tp, tp_stride, fwords, n_rows,
+                                                                  (const uint2*)layout, tree_off, T, C, cap, raw, prob, pred);
+    else predict_forest_kernel<0><<<grid, (int)bd, smem, (cudaStream_t)stream>>>(tp, tp_stride, fwords, n_rows,
+                                                                  (const uint2*)layout, tree_off, T, C, cap, raw, prob, pred);
+    return check_launch("predict_forest");
 }
 
 extern "C" int b200flow_gather_rows(const void* src, int32_t row_bytes, const int32_t* idx, int64_t n_rows, void* out, void* stream) {
