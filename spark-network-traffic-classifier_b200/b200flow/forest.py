@@ -88,6 +88,25 @@ def poisson_cdf_table(rate=1.0):
     return out
 
 
+def bag_weights(rows, T, cdf_host, cdf_dev, by_record, seed, row_offset):
+    """W int32 [T][U]: the summed weights of every (weight row, unique record) of read _TrainingRows, drawn per (row t, global
+    row) from the 32-threshold inverse CDF cdf_host (cdf_dev: its device copy, staged by the caller).  cdf_host None: every
+    record weighs its multiplicity.  by_record: draw over the rows grouped by unique record (one RED per warp run and weight
+    row instead of one per row), when there are draws and records repeat."""
+    n, U, uid, dev = rows.n, rows.U, rows.uid, rows.src.device
+    W = torch.zeros(max(T * U, 1), dtype=torch.int32, device=dev)
+    if n > 0:
+        perm = uperm = None
+        if by_record and cdf_host is not None and uid is not None and U < n:
+            gsize = torch.empty(U, dtype=torch.int32, device=dev); cursor = torch.empty(U, dtype=torch.int32, device=dev)
+            goff = torch.empty(U + 1, dtype=torch.int64, device=dev)
+            perm = torch.empty(n, dtype=torch.int32, device=dev); uperm = torch.empty(n, dtype=torch.int32, device=dev)
+            _timed("group_rows", "b200flow_group_rows", ptr(uid), n, U, ptr(gsize), ptr(goff), ptr(cursor), ptr(perm), ptr(uperm))
+        _timed("bag_weights", "b200flow_bag_weights", seed, T, int(row_offset), n, ptr(cdf_dev),
+               cdf_host.ctypes.data if cdf_host is not None else None, ptr(uperm if perm is not None else uid), ptr(perm), U, ptr(W))
+    return W
+
+
 def build_metadata(n_rows, F, num_classes, arity, max_bins, num_trees, strategy="auto"):
     """DecisionTreeMetadata.buildMetadata (A.1): (maxPossibleBins, feat_kind[F], numFeaturesPerNode)."""
     arity = np.asarray(arity, np.int32)
@@ -570,6 +589,109 @@ class _TrainingRows:
         return self
 
 
+class Bag:
+    """the entries {unique record, weight} of T weight rows W [T][U]: the non-zero weights, tree-major and in unique-id order.
+    count() enqueues bag_count (the non-zeros of every 1024-record block) and its scan into the block offsets, whose total
+    (the entry count) stays on the device; fill() writes the entries.  Tree t's entries are [blk_off[t·nb], blk_off[(t+1)·nb])."""
+
+    def __init__(self, T, U, dev):
+        self.T, self.U, self.nb = T, U, (U + 1023) // 1024
+        self.blk_cnt = torch.zeros(max(T * self.nb, 1), dtype=torch.int32, device=dev)
+        self.blk_off = torch.zeros(T * self.nb + 1, dtype=torch.int64, device=dev)
+        self.total = torch.zeros(1, dtype=torch.int64, device=dev)
+
+    def count(self, W):
+        if self.U > 0:
+            call("b200flow_bag_count", ptr(W), self.T, self.U, ptr(self.blk_cnt))
+        call("b200flow_exclusive_scan_i32_to_i64", ptr(self.blk_cnt), self.T * self.nb, ptr(self.blk_off), ptr(self.total))
+
+    def fill(self, W, ent):
+        if self.U > 0:
+            call("b200flow_bag_fill", ptr(W), self.T, self.U, ptr(self.blk_off), ptr(ent))
+
+    def segments(self):
+        """-> (seg_begin, seg_end) int64 [T]: every tree's entry range, one level-0 slot per tree"""
+        idx = torch.arange(self.T, dtype=torch.int64, device=self.blk_off.device) * self.nb
+        return self.blk_off[idx].contiguous(), self.blk_off[idx + self.nb].contiguous()
+
+
+def chunk_table(lens):
+    """(device offsets int64 [ns + 1], their host copy) of the CHUNK_ROWS-entry chunks of slots holding lens [ns] entries: the
+    chunk table of hist_level, partition_level and their variance-tree forms (one host read)"""
+    nch = ((lens + (CHUNK_ROWS - 1)) // CHUNK_ROWS).to(torch.int32).contiguous()
+    off = torch.empty(nch.shape[0] + 1, dtype=torch.int64, device=lens.device)
+    call("b200flow_exclusive_scan_i32_to_i64", ptr(nch), nch.shape[0], ptr(off), None)
+    return off, off.cpu()
+
+
+class NodePool:
+    """the growing node pool of a fit: roots 0..n_roots-1, and per node the statistics grow_level copies from the scored
+    slots — int32 [cap, C] class counts for the forest, int64 [cap, 3] {Σw, Σw·q, Σw·q2} for the variance trees.  grow_level
+    sees them as opaque 32-bit words."""
+
+    def __init__(self, n_roots, cap, with_mask, stat_width, stat_dtype, dev):
+        self.dev, self.cap, self.size = dev, cap, n_roots
+        self.nodes = torch.zeros((cap, 16), dtype=torch.uint8, device=dev)
+        self.node_mask = torch.zeros((cap, 4), dtype=torch.int64, device=dev) if with_mask else None
+        self.stats = torch.zeros((cap, stat_width), dtype=stat_dtype, device=dev)
+        self.node_tree = torch.zeros(cap, dtype=torch.int32, device=dev)
+        self.node_gain = torch.zeros(cap, dtype=torch.float64, device=dev)
+        root = np.zeros(n_roots, NODE_DTYPE); root["feat"] = -1; root["left"] = -1; root["nid"] = 1
+        self.nodes[:n_roots] = _lib.h2d(root.view(np.uint8).reshape(n_roots, 16), dev)
+        self.node_tree[:n_roots] = torch.arange(n_roots, dtype=torch.int32, device=dev)
+        self.counters = None
+
+    def grow(self, need):
+        if need <= self.cap:
+            return
+        new_cap = self.cap
+        while new_cap < need:
+            new_cap *= 2
+
+        def ext(t):
+            nt = torch.zeros((new_cap,) + tuple(t.shape[1:]), dtype=t.dtype, device=self.dev)
+            nt[:self.cap] = t
+            return nt
+        self.nodes, self.stats, self.node_tree, self.node_gain = ext(self.nodes), ext(self.stats), ext(self.node_tree), ext(self.node_gain)
+        if self.node_mask is not None:
+            self.node_mask = ext(self.node_mask)
+        self.cap = new_cap
+
+    def grow_level(self, n_slots, slot_tree, slot_nid, slot_node, split, node_st, left_st, right_st, next_tree, next_nid,
+                   next_node, next_parent, child_slot=None):
+        """enqueue grow_level: the slots' nodes are written and their children appended (the pool first grows to hold them).
+        The counters [pool size, n_next, overflow, pool size before, route chunks, ...] + per-block scratch live across levels:
+        the pool size carries over on the device, everything else is rewritten by grow_level / the scans, so they are only
+        re-allocated when a level needs more scratch (no per-level fill launches).  commit() takes their host copy."""
+        self.grow(self.size + 2 * n_slots)
+        nblk = (n_slots + 255) // 256
+        if self.counters is None or self.counters.numel() < 8 + nblk + 1:
+            fresh = torch.zeros(8 + 2 * nblk + 1024, dtype=torch.int64, device=self.dev)
+            if self.counters is None:
+                fresh[0:1].fill_(self.size)
+            else:
+                fresh[:8] = self.counters[:8]
+            self.counters = fresh
+        words = self.stats.shape[1] * self.stats.element_size() // 4
+        _timed("grow_level", "b200flow_grow_level", n_slots, ptr(slot_tree), ptr(slot_nid), ptr(slot_node), ptr(split), ptr(node_st),
+               ptr(left_st), ptr(right_st), words, ptr(self.nodes), ptr(self.node_mask), ptr(self.stats), ptr(self.node_tree),
+               self.cap, ptr(next_tree), ptr(next_nid), ptr(next_node), ptr(next_parent), ptr(child_slot), ptr(self.counters))
+
+    def commit(self, cnt):
+        """cnt: the host copy of counters[:3] after grow_level -> the number of next-level slots (the pool size moves on)"""
+        if int(cnt[2]) != 0:
+            raise B200FlowError("node pool overflow (capacity %d)" % self.cap)
+        self.size = int(cnt[0])
+        return int(cnt[1])
+
+    def model(self, rows, T, leaf, class_counts=False, dt_mode=False):
+        """the ForestModel of trees 0..T-1 of this pool, binned as rows, with leaf table leaf [size, C]; class_counts: the
+        stats are the class counts the forest's grid predictors and export read"""
+        return ForestModel(T, leaf.shape[1], rows.F, rows.arity, rows.mpb, rows.thresholds, rows.n_thr, self.nodes,
+                           self.node_mask, self.stats if class_counts else None, self.node_tree, leaf, self.node_gain,
+                           self.size, dt_mode)
+
+
 def fit_forest(x, labels, num_classes, arity, params, row_offset=0, group=None):
     """RandomForest.run (R4-R8) on a dense CUDA feature matrix x [n, F] (f32/f64) and int32 labels [n].
 
@@ -604,47 +726,17 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
     T = int(p.num_trees)
     seed = int(p.seed) & 0xFFFFFFFFFFFFFFFF
     rows = _TrainingRows(src, C, arity, p.max_bins, T, p.feature_subset_strategy, seed, row_offset, group)
-    mpb, kind, m, arity = rows.mpb, rows.kind, rows.m, rows.arity
-    thresholds, n_thr, feat_bins, feat_kind, uid, dedup = rows.thresholds, rows.n_thr, rows.feat_bins, rows.feat_kind, rows.uid, rows.dedup
+    kind, m, feat_bins, feat_kind = rows.kind, rows.m, rows.feat_bins, rows.feat_kind
     stride = tp_stride(F)
-    total = torch.zeros(1, dtype=torch.int64, device=dev)
     # host-side preparation that does not depend on the counts runs BEFORE the read, while the GPU works through the queue
     bagging = p.bootstrap and T > 1
     cdf_host = np.ascontiguousarray(poisson_cdf_table(p.subsampling_rate)) if bagging else None
     cdf = _lib.h2d(cdf_host.view(np.int32), dev) if bagging else None
-    # node pool
-    cap_nodes = max(4096, 4 * T, min(T << (min(p.max_depth, 18) + 1), 1 << 20))   # sized so that typical forests never re-allocate
-    nodes = torch.zeros((cap_nodes, 16), dtype=torch.uint8, device=dev)
-    use_mask = bool((kind > 0).any())
-    node_mask = torch.zeros((cap_nodes, 4), dtype=torch.int64, device=dev) if use_mask else None
-    pool_counts = torch.zeros((cap_nodes, C), dtype=torch.int32, device=dev)
-    node_tree = torch.zeros(cap_nodes, dtype=torch.int32, device=dev)
-    node_gain = torch.zeros(cap_nodes, dtype=torch.float64, device=dev)
-    root = np.zeros(T, NODE_DTYPE); root["feat"] = -1; root["left"] = -1; root["nid"] = 1
-    nodes[:T] = _lib.h2d(root.view(np.uint8).reshape(T, 16), dev)
-    node_tree[:T] = torch.arange(T, dtype=torch.int32, device=dev)
-    pool_size = T
-
-    def grow_pool(need):
-        nonlocal nodes, node_mask, pool_counts, node_tree, node_gain, cap_nodes
-        if need <= cap_nodes:
-            return
-        new_cap = cap_nodes
-        while new_cap < need:
-            new_cap *= 2
-        def ext(t, shape_tail):
-            nt = torch.zeros((new_cap,) + shape_tail, dtype=t.dtype, device=dev)
-            nt[:cap_nodes] = t
-            return nt
-        nodes = ext(nodes, (16,)); pool_counts = ext(pool_counts, (C,)); node_tree = ext(node_tree, ())
-        node_gain = ext(node_gain, ())
-        if node_mask is not None:
-            node_mask = ext(node_mask, (4,))
-        cap_nodes = new_cap
-
+    # node pool, sized so that typical forests never re-allocate
+    pool = NodePool(T, max(4096, 4 * T, min(T << (min(p.max_depth, 18) + 1), 1 << 20)), bool((kind > 0).any()), C, torch.int32,
+                    dev)
     rows.read()
     n_bins, U, tp, head = rows.n_bins, rows.U, rows.tp, rows.head
-    del rows
     # launch shape of the fused kernel: entries per routing chunk and subset features per pass (wide nodes — many classes,
     # or a DecisionTree's all-feature histograms — are accumulated in several feature passes, the first of which routes)
     desc_host, rec_bytes = _lib.packed_layout(head[5:5 + F].numpy(), C) if FUSED else (None, 0)
@@ -660,39 +752,22 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
         field_desc = _lib.h2d(desc_host, dev)
         rec_tp, rec_stride = pack_records(tp, F, field_desc, rec_bytes), rec_bytes
     # ---- R6 bagging: W[tree][unique] = summed Poisson weights; entries = non-zero (unique, weight) pairs per tree
-    nb = (U + 1023) // 1024
-    W = torch.zeros(max(T * U, 1), dtype=torch.int32, device=dev)
-    if n > 0:
-        perm = uperm = None
-        if uid is not None and bagging and U < n:           # group the rows by unique id: one RED per (warp run, tree)
-            gsize = torch.empty(U, dtype=torch.int32, device=dev); cursor = torch.empty(U, dtype=torch.int32, device=dev)
-            goff = torch.empty(U + 1, dtype=torch.int64, device=dev)
-            perm = torch.empty(n, dtype=torch.int32, device=dev); uperm = torch.empty(n, dtype=torch.int32, device=dev)
-            _timed("group_rows", "b200flow_group_rows", ptr(uid), n, U, ptr(gsize), ptr(goff), ptr(cursor), ptr(perm), ptr(uperm))
-        _timed("bag_weights", "b200flow_bag_weights", seed, T, int(row_offset), n, ptr(cdf),
-               cdf_host.ctypes.data if bagging else None, ptr(uperm if perm is not None else uid), ptr(perm), U, ptr(W))
-    blk_cnt = torch.zeros(max(T * nb, 1), dtype=torch.int32, device=dev)
-    blk_off = torch.zeros(T * nb + 1, dtype=torch.int64, device=dev)
-    if U > 0:
-        call("b200flow_bag_count", ptr(W), T, U, ptr(blk_cnt))
-    call("b200flow_exclusive_scan_i32_to_i64", ptr(blk_cnt), T * nb, ptr(blk_off), ptr(total))
+    W = bag_weights(rows, T, cdf_host, cdf, True, seed, row_offset)
+    bag = Bag(T, U, dev)
+    bag.count(W)
     # the entry count E stays on the device when its upper bound T * U (every record drawn by every tree) is affordable:
     # one host round trip less; the exact count is read with the last level's counters
-    e_dev = total.clone()
-    E = T * U if T * U * 16 <= ENTRY_BOUND_BYTES else int(total.item())
+    E = T * U if T * U * 16 <= ENTRY_BOUND_BYTES else int(bag.total.item())
     ent = torch.empty((max(E, 1), 2), dtype=torch.int32, device=dev)     # {unique record index, weight}
     ent2 = torch.empty_like(ent)
-    if U > 0:
-        call("b200flow_bag_fill", ptr(W), T, U, ptr(blk_off), ptr(ent))
-    del W, uid
-
+    bag.fill(W, ent)
+    del W
+    rows.uid = None                    # the row -> record map is not needed past the bag weights
     # ---- level 0 slots: one per tree
     slot_tree = torch.arange(T, dtype=torch.int32, device=dev)
     slot_nid = torch.ones(T, dtype=torch.int32, device=dev)
     slot_node = torch.arange(T, dtype=torch.int32, device=dev)
-    idx = torch.arange(T, dtype=torch.int64, device=dev) * nb
-    seg_begin = blk_off[idx].contiguous()
-    seg_end = blk_off[idx + nb].contiguous()
+    seg_begin, seg_end = bag.segments()
     n_slots = T
     level = 0
     per_slot_hist = m * n_bins * C * 4
@@ -701,11 +776,6 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
 
     stats["route_chunk"], stats["route_passes"] = route_ch if fused else 0, route_passes if fused else 0
     stats["record_format"], stats["record_bytes"] = ("packed", rec_bytes) if field_desc is not None else ("bytes", stride)
-
-    def chunk_table(nch):
-        off = torch.empty(nch.shape[0] + 1, dtype=torch.int64, device=dev)
-        call("b200flow_exclusive_scan_i32_to_i64", ptr(nch), nch.shape[0], ptr(off), ptr(total))
-        return off, int(total.item())
 
     def level_subsets(ns, s_tree, s_nid):
         sub = torch.empty((ns, m), dtype=torch.int16, device=dev)
@@ -791,7 +861,6 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
     host_cnt = torch.empty(5, dtype=torch.int64).pin_memory() if _PIN else None
     subset = level_subsets(n_slots, slot_tree, slot_nid)
     hist_ready = None                  # histogram of the CURRENT level when the fused kernel already built it
-    counters = None
     if fused and n_slots * hsz * 4 <= HIST_BUDGET_BYTES:        # (not on E: every rank must take the same collective path)
         # level 0 through the same kernel: T pseudo-parents whose split sends every entry "left" into the tree's root
         pseudo = np.zeros(T, SPLIT_DTYPE); pseudo["bin_thr"] = 255; pseudo["flags"] = 4
@@ -799,11 +868,11 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
         child0 = torch.stack([torch.arange(T, dtype=torch.int32, device=dev),
                               torch.full((T,), -1, dtype=torch.int32, device=dev)], 1).contiguous().view(-1)
         cursors0 = torch.zeros(2 * T, dtype=torch.int32, device=dev)
-        roff0 = plan_route(T, pseudo_t, seg_begin, seg_end, total)
-        hist_full = run_route(roff0, total, T, pseudo_t, child0, cursors0, subset, T, route=False)
+        rch0 = torch.zeros(1, dtype=torch.int64, device=dev)
+        roff0 = plan_route(T, pseudo_t, seg_begin, seg_end, rch0)
+        hist_full = run_route(roff0, rch0, T, pseudo_t, child0, cursors0, subset, T, route=False)
         hist_ready = hist_full[:T * hsz]
     while n_slots > 0:
-        grow_pool(pool_size + 2 * n_slots)
         lens = (seg_end - seg_begin) if hist_ready is None else None   # only the unfused kernels need the lengths on the host side
         n_alloc = n_slots + world - 1                        # room for the padded node blocks of the sharded scoring
         split = torch.empty((n_alloc, 64), dtype=torch.uint8, device=dev)
@@ -812,8 +881,7 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
         right_counts = torch.empty((n_alloc, C), dtype=torch.int32, device=dev)
         chunk_off = None
         if hist_ready is None:
-            nch = ((lens + (CHUNK_ROWS - 1)) // CHUNK_ROWS).to(torch.int32).contiguous()
-            chunk_off, n_chunks = chunk_table(nch)
+            chunk_off, chunk_h = chunk_table(lens)
         groups = [(0, n_slots)] if hist_ready is not None else \
             [(g0, min(n_slots, g0 + group_slots)) for g0 in range(0, n_slots, group_slots)]
         for g0, g1 in groups:
@@ -822,11 +890,8 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
                 h = hist_ready
             else:
                 h = torch.zeros(gs * hsz, dtype=torch.int32, device=dev)
-                if g0 == 0 and g1 == n_slots:
-                    coff, gch = chunk_off, n_chunks
-                else:
-                    coff = (chunk_off[g0:g1 + 1] - chunk_off[g0]).contiguous()
-                    gch = int((chunk_off[g1] - chunk_off[g0]).item())
+                gch = int(chunk_h[g1] - chunk_h[g0])
+                coff = chunk_off if g0 == 0 and g1 == n_slots else (chunk_off[g0:g1 + 1] - chunk_off[g0]).contiguous()
                 # R7 HOT LOOP A (unfused form: level 0, and levels whose histograms exceed the fused budget)
                 _timed("hist_level", "b200flow_hist_level", ptr(tp), stride, F, ptr(ent), gs,
                        ptr(seg_begin[g0:g1]), ptr(seg_end[g0:g1]), ptr(coff), gch, CHUNK_ROWS, ptr(subset[g0:g1]), m, n_bins, C, ptr(h))
@@ -852,34 +917,24 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
         split, node_counts, left_counts, right_counts = split[:n_slots], node_counts[:n_slots], left_counts[:n_slots], right_counts[:n_slots]
         hist_ready = None
         # grow the pool by this level's children and emit the next level's slots
-        nblk = (n_slots + 255) // 256
-        if counters is None or counters.numel() < 8 + nblk + 1:
-            # [pool, n_next, overflow, pool_before, route chunks, ...] + per-block scratch; lives across levels: the pool size carries
-            # over on the device, everything else is rewritten by grow_level / the scans (no per-level fill launches)
-            fresh = torch.zeros(8 + 2 * nblk + 1024, dtype=torch.int64, device=dev)
-            if counters is None:
-                fresh[0:1].fill_(pool_size)
-            else:
-                fresh[:8] = counters[:8]
-            counters = fresh
         next_tree = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
         next_nid = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
         next_node = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
         next_parent = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
         child_slot = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
-        _timed("grow_level", "b200flow_grow_level", n_slots, ptr(slot_tree), ptr(slot_nid), ptr(slot_node), ptr(split), ptr(node_counts),
-               ptr(left_counts), ptr(right_counts), C, ptr(nodes), ptr(node_mask), ptr(pool_counts), ptr(node_tree),
-               cap_nodes, ptr(next_tree), ptr(next_nid), ptr(next_node), ptr(next_parent), ptr(child_slot), ptr(counters))
+        pool.grow_level(n_slots, slot_tree, slot_nid, slot_node, split, node_counts, left_counts, right_counts, next_tree, next_nid,
+                        next_node, next_parent, child_slot)
+        counters = pool.counters
         n_cap = 2 * n_slots                              # upper bound on the number of next-level slots
         # (the deepest level has only leaf children: nothing to route, nothing to enqueue ahead)
         speculative = fused and n_cap * hsz * 4 <= HIST_BUDGET_BYTES and level + 1 < p.max_depth
         if not speculative:
-            node_gain[slot_node.long()] = split.view(torch.float64)[:, 2]
+            pool.node_gain[slot_node.long()] = split.view(torch.float64)[:, 2]
         if speculative:
             # Everything the next level needs is enqueued NOW with device-side counts (children created, routing chunks);
             # the host reads the counts on a side stream while the routing pass runs, so the GPU never waits for Python.
             cursors = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)       # zeroed by plan_route
-            roff = plan_route(n_slots, split, seg_begin, seg_end, counters[4:5], slot_node, node_gain, cursors)
+            roff = plan_route(n_slots, split, seg_begin, seg_end, counters[4:5], slot_node, pool.node_gain, cursors)
             ev_planned = torch.cuda.Event(); ev_planned.record()
             with torch.cuda.stream(side_stream):
                 side_stream.wait_event(ev_planned)
@@ -896,9 +951,7 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
             ev_read.synchronize()
         else:
             cnt = counters[:5].cpu()
-        if int(cnt[2]) != 0:
-            raise B200FlowError("node pool overflow (capacity %d)" % cap_nodes)
-        pool_size, n_next = int(cnt[0]), int(cnt[1])
+        n_next = pool.commit(cnt)
         stats["levels"] += 1; stats["slots"] += n_slots
         if n_next == 0:
             break
@@ -911,11 +964,9 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
             next_subset = level_subsets(n_next, next_tree, next_nid)
             cursors = torch.zeros(2 * n_slots, dtype=torch.int32, device=dev)
             if chunk_off is None:
-                lens = seg_end - seg_begin
-                nch = ((lens + (CHUNK_ROWS - 1)) // CHUNK_ROWS).to(torch.int32).contiguous()
-                chunk_off, n_chunks = chunk_table(nch)
+                chunk_off, chunk_h = chunk_table(seg_end - seg_begin)
             _timed("partition_level", "b200flow_partition_level", ptr(tp), stride, ptr(ent), ptr(ent2),
-                   n_slots, ptr(seg_begin), ptr(seg_end), ptr(chunk_off), n_chunks, CHUNK_ROWS, ptr(split), ptr(cursors))
+                   n_slots, ptr(seg_begin), ptr(seg_end), ptr(chunk_off), int(chunk_h[-1]), CHUNK_ROWS, ptr(split), ptr(cursors))
             next_begin = torch.empty(n_next, dtype=torch.int64, device=dev)
             next_end = torch.empty(n_next, dtype=torch.int64, device=dev)
             call("b200flow_next_segments", n_next, None, ptr(next_parent), ptr(seg_begin), ptr(seg_end), ptr(cursors),
@@ -926,11 +977,10 @@ def _fit(src, num_classes, arity, params, row_offset=0, group=None):
         n_slots = n_next
         level += 1
 
-    leaf_prob = torch.empty((pool_size, C), dtype=torch.float64, device=dev)
-    call("b200flow_finalize_forest", pool_size, ptr(pool_counts), C, ptr(leaf_prob))
-    stats["entries"] = int(e_dev.item())
-    model = ForestModel(T, C, F, arity, mpb, thresholds, n_thr, nodes, node_mask, pool_counts, node_tree, leaf_prob,
-                        node_gain, pool_size, dt_mode=(T == 1 and not p.bootstrap))
+    leaf_prob = torch.empty((pool.size, C), dtype=torch.float64, device=dev)
+    call("b200flow_finalize_forest", pool.size, ptr(pool.stats), C, ptr(leaf_prob))
+    stats["entries"] = int(bag.total.item())
+    model = pool.model(rows, T, leaf_prob, class_counts=True, dt_mode=(T == 1 and not p.bootstrap))
     model.train_stats = stats
     model.feat_kind, model.feat_bins, model.n_bins, model.m = kind, feat_bins, n_bins, m
     return model

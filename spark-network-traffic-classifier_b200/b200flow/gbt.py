@@ -17,19 +17,8 @@ import torch
 
 from . import _lib
 from . import forest as fr
-from ._lib import NODE_DTYPE, B200FlowError, call, ptr
-
-PROFILE = None                     # set to a dict to collect per-phase CUDA-event timings (tools/bench_gbt.py)
-
-
-def _timed(name, fn, *args):
-    if PROFILE is None:
-        return call(fn, *args)
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    call(fn, *args)
-    e1.record()
-    PROFILE.setdefault(name, []).append((e0, e1))
+from ._lib import NODE_DTYPE, call, ptr
+from .forest import _timed
 
 
 @dataclass
@@ -178,39 +167,6 @@ class OvRGBTModel:
         return raw, pred
 
 
-class NodePool:
-    """the growing node pool of a variance-tree fit: roots 0..n_roots-1; a node's stats are 3 int64 {Σw, Σw·q, Σw·q2} = the
-    6 opaque words grow_level copies per node"""
-
-    def __init__(self, n_roots, cap, with_mask, dev):
-        self.dev, self.cap, self.size = dev, cap, n_roots
-        self.nodes = torch.zeros((cap, 16), dtype=torch.uint8, device=dev)
-        self.node_mask = torch.zeros((cap, 4), dtype=torch.int64, device=dev) if with_mask else None
-        self.stats = torch.zeros((cap, 3), dtype=torch.int64, device=dev)
-        self.node_tree = torch.zeros(cap, dtype=torch.int32, device=dev)
-        self.node_gain = torch.zeros(cap, dtype=torch.float64, device=dev)
-        root = np.zeros(n_roots, NODE_DTYPE); root["feat"] = -1; root["left"] = -1; root["nid"] = 1
-        self.nodes[:n_roots] = _lib.h2d(root.view(np.uint8).reshape(n_roots, 16), dev)
-        self.node_tree[:n_roots] = torch.arange(n_roots, dtype=torch.int32, device=dev)
-        self.counters = torch.zeros(8 + 2 * 64 + 1024, dtype=torch.int64, device=dev)
-
-    def grow(self, need):
-        if need <= self.cap:
-            return
-        new_cap = self.cap
-        while new_cap < need:
-            new_cap *= 2
-
-        def ext(t):
-            nt = torch.zeros((new_cap,) + tuple(t.shape[1:]), dtype=t.dtype, device=self.dev)
-            nt[:self.cap] = t
-            return nt
-        self.nodes, self.stats, self.node_tree, self.node_gain = ext(self.nodes), ext(self.stats), ext(self.node_tree), ext(self.node_gain)
-        if self.node_mask is not None:
-            self.node_mask = ext(self.node_mask)
-        self.cap = new_cap
-
-
 class LevelLoop:
     """the level loop of the variance trees, shared by GBTClassifier, OneVsRest(GBTClassifier) and the regressors
     (b200flow/regression.py): every level builds the slots' {Σw, Σw·q, Σw·q2} histograms (gbt_hist_level, in slot groups
@@ -226,15 +182,6 @@ class LevelLoop:
         self.per_slot = m * n_bins * 3
         self.group_slots = max(1, fr.HIST_BUDGET_BYTES // (self.per_slot * 8))
 
-    def _chunk_table(self, lens, dev):
-        """(device chunk offsets, their host copy) of the slots' entry ranges"""
-        CH = fr.CHUNK_ROWS
-        nch = ((lens + (CH - 1)) // CH).to(torch.int32).contiguous()
-        off = torch.empty(nch.shape[0] + 1, dtype=torch.int64, device=dev)
-        total = torch.zeros(1, dtype=torch.int64, device=dev)
-        call("b200flow_exclusive_scan_i32_to_i64", ptr(nch), nch.shape[0], ptr(off), ptr(total))
-        return off, off.cpu()
-
     def grow(self, pool, ent, ent2, seg_begin, seg_end, slot_tree):
         """grow the trees rooted at pool nodes slot_tree (one level-0 slot each, whose entries are ent[seg_begin:seg_end])
         to the end; -> (ent, ent2), swapped as the partitions left them"""
@@ -244,17 +191,13 @@ class LevelLoop:
         n_slots, level = int(slot_tree.numel()), 0
         slot_nid = torch.ones(n_slots, dtype=torch.int32, device=dev)
         slot_node = slot_tree.clone()
-        pool.counters[0] = pool.size
         while n_slots > 0:
-            pool.grow(pool.size + 2 * n_slots)
-            if pool.counters.numel() < 8 + 2 * ((n_slots + 255) // 256):
-                pool.counters = torch.cat([pool.counters, torch.zeros(2 * n_slots, dtype=torch.int64, device=dev)])
             subset = torch.empty((n_slots, m), dtype=torch.int16, device=dev)
             # the feature subsets are keyed by the iteration, as in the K separate fits: class k's tree t draws tree t's
             slot_iter = torch.remainder(slot_tree, T) if ovr else slot_tree
             call("b200flow_feature_subsets", self.seed, n_slots, ptr(slot_iter), ptr(slot_nid), self.F, m, ptr(subset))
             slot_class = torch.div(slot_tree, T, rounding_mode="floor") if ovr else None
-            chunk_off, off_h = self._chunk_table(seg_end - seg_begin, dev)
+            chunk_off, off_h = fr.chunk_table(seg_end - seg_begin)
             n_chunks = int(off_h[-1])
             split = torch.empty((n_slots, 64), dtype=torch.uint8, device=dev)
             st = torch.empty((3, n_slots, 3), dtype=torch.int64, device=dev)   # node, left, right
@@ -282,14 +225,10 @@ class LevelLoop:
             next_nid = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
             next_node = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
             next_parent = torch.empty(2 * n_slots, dtype=torch.int32, device=dev)
-            _timed("grow_level", "b200flow_grow_level", n_slots, ptr(slot_tree), ptr(slot_nid), ptr(slot_node), ptr(split), ptr(st[0]),
-                   ptr(st[1]), ptr(st[2]), 6, ptr(pool.nodes), ptr(pool.node_mask), ptr(pool.stats), ptr(pool.node_tree), pool.cap,
-                   ptr(next_tree), ptr(next_nid), ptr(next_node), ptr(next_parent), None, ptr(pool.counters))
+            pool.grow_level(n_slots, slot_tree, slot_nid, slot_node, split, st[0], st[1], st[2], next_tree, next_nid, next_node,
+                            next_parent)
             pool.node_gain[slot_node.long()] = split.view(torch.float64)[:, 2]
-            cnt = pool.counters[:3].cpu()
-            if int(cnt[2]) != 0:
-                raise B200FlowError("node pool overflow (capacity %d)" % pool.cap)
-            pool.size, n_next = int(cnt[0]), int(cnt[1])
+            n_next = pool.commit(pool.counters[:3].cpu())
             self.stats["levels"] += 1; self.stats["slots"] += n_slots
             if n_next == 0:
                 break
@@ -309,13 +248,8 @@ class LevelLoop:
         return ent, ent2
 
 
-def _fit(src, arity, params, row_offset=0, group=None, n_classes=None):
-    """the boosting loop.  n_classes None: the binary problem of the label byte.  n_classes = K: the K problems (label == k)
-    side by side — the pool holds K·T trees, class-major (tree k·T + t), margin and rq are [K][U], every iteration's entries
-    are repeated in K segments (one per class root) and one level loop grows all K trees."""
-    from . import dist as bdist
-    _lib.require_cuda()
-    p = params
+def check_boosting_params(p):
+    """the parameter checks GBTClassifier and GBTRegressor share"""
     if not (0 <= p.max_depth <= 30):
         raise ValueError("maxDepth must be in [0, 30], got %d" % p.max_depth)
     if int(p.max_iter) < 1:
@@ -324,6 +258,16 @@ def _fit(src, arity, params, row_offset=0, group=None, n_classes=None):
         raise ValueError("stepSize must be in (0, 1], got %r" % p.step_size)
     if not (0.0 < p.subsampling_rate <= 1.0):
         raise ValueError("subsamplingRate must be in (0, 1], got %r" % p.subsampling_rate)
+
+
+def _fit(src, arity, params, row_offset=0, group=None, n_classes=None):
+    """the boosting loop.  n_classes None: the binary problem of the label byte.  n_classes = K: the K problems (label == k)
+    side by side — the pool holds K·T trees, class-major (tree k·T + t), margin and rq are [K][U], every iteration's entries
+    are repeated in K segments (one per class root) and one level loop grows all K trees."""
+    from . import dist as bdist
+    _lib.require_cuda()
+    p = params
+    check_boosting_params(p)
     ovr = n_classes is not None
     K = int(n_classes) if ovr else 1
     if not (1 <= K <= 256):
@@ -336,7 +280,7 @@ def _fit(src, arity, params, row_offset=0, group=None, n_classes=None):
     # num_classes = 2 only shapes the metadata, so the bins are the binary fit's; de-duplication keys on (bins, label byte), and
     # with K classes those records refine each relabelled problem's records: the trees see the same integer histogram sums
     rows = fr._TrainingRows(src, 2, arity, p.max_bins, 1, strategy, seed, row_offset, group).read()
-    tp, uid, U, m, n_bins = rows.tp, rows.uid, rows.U, rows.m, rows.n_bins
+    tp, U, m, n_bins = rows.tp, rows.U, rows.m, rows.n_bins
     feat_bins, feat_kind, stride = rows.feat_bins, rows.feat_kind, fr.tp_stride(F)
     S, S2 = grid_shift(rows.n_global)
     # labels must be 0 or 1 (OneVsRest: below K) on EVERY rank: the flag is summed over the ranks first, so that all of them
@@ -354,16 +298,12 @@ def _fit(src, arity, params, row_offset=0, group=None, n_classes=None):
     # iteration sees each unique record with its multiplicity
     sub = p.subsampling_rate < 1.0
     TW = T if sub else 1
-    W = torch.zeros(max(TW * U, 1), dtype=torch.int32, device=dev)
-    if n > 0:
-        cdf_host = subsample_cdf(p.subsampling_rate) if sub else None
-        call("b200flow_bag_weights", seed, TW, int(row_offset), n, ptr(_lib.h2d(cdf_host.view(np.int32), dev)) if sub else None,
-             cdf_host.ctypes.data if sub else None, ptr(uid), None, U, ptr(W))
-    del uid
+    cdf_host = subsample_cdf(p.subsampling_rate) if sub else None
+    W = fr.bag_weights(rows, TW, cdf_host, _lib.h2d(cdf_host.view(np.int32), dev) if sub else None, False, seed, row_offset)
 
     # node pool: roots 0..K·T-1
     TK = K * T
-    pool = NodePool(TK, max(1024, TK * min(1 << (p.max_depth + 1), 64)), bool((rows.kind > 0).any()), dev)
+    pool = fr.NodePool(TK, max(1024, TK * min(1 << (p.max_depth + 1), 64)), bool((rows.kind > 0).any()), 3, torch.int64, dev)
 
     weights = [1.0] + [float(p.step_size)] * (T - 1)
     tree_weight = _lib.h2d(np.asarray(weights * K, np.float64), dev)
@@ -375,10 +315,7 @@ def _fit(src, arity, params, row_offset=0, group=None, n_classes=None):
     else:
         call("b200flow_gbt_update", ptr(tp), stride, F, U, None, None, None, -1, S, S2, ptr(margin), ptr(rq))
 
-    nb = (U + 1023) // 1024
-    blk_cnt = torch.zeros(max(nb, 1), dtype=torch.int32, device=dev)
-    blk_off = torch.zeros(nb + 1, dtype=torch.int64, device=dev)
-    total = torch.zeros(1, dtype=torch.int64, device=dev)
+    bag = fr.Bag(1, U, dev)
     ent = torch.empty((max(K * U, 1), 2), dtype=torch.int32, device=dev)        # class k's segment starts at k·U
     ent2 = torch.empty_like(ent)
     stats_t = dict(levels=0, slots=0, rows=n, unique_rows=U, S=S)
@@ -391,20 +328,17 @@ def _fit(src, arity, params, row_offset=0, group=None, n_classes=None):
     for t in range(T):
         # ---- this iteration's entries {unique record, weight}: the non-zero weights, in unique-id order
         Wt = W[(t if sub else 0) * U:(t if sub else 0) * U + max(U, 1)]
-        if U > 0:
-            call("b200flow_bag_count", ptr(Wt), 1, U, ptr(blk_cnt))
-        call("b200flow_exclusive_scan_i32_to_i64", ptr(blk_cnt), nb, ptr(blk_off), ptr(total))
-        if U > 0:
-            call("b200flow_bag_fill", ptr(Wt), 1, U, ptr(blk_off), ptr(ent))
+        bag.count(Wt)
+        bag.fill(Wt, ent)
         if ovr:             # the same entries for every class: one segment per class root k·T + t
             if K > 1 and U > 0:
                 ent[:K * U].view(K, U, 2)[1:] = ent[:U]
             seg_begin = cls_base.clone()
-            seg_end = cls_base + total
+            seg_end = cls_base + bag.total
             slot_tree = cls_root + t
         else:
             seg_begin = torch.zeros(1, dtype=torch.int64, device=dev)
-            seg_end = total.clone()
+            seg_end = bag.total.clone()
             slot_tree = torch.full((1,), t, dtype=torch.int32, device=dev)
         ent, ent2 = loop.grow(pool, ent, ent2, seg_begin, seg_end, slot_tree)
         # ---- leaf values of the pool so far, then F and the next residuals of every unique record
@@ -418,14 +352,9 @@ def _fit(src, arity, params, row_offset=0, group=None, n_classes=None):
             _timed("gbt_update", "b200flow_gbt_update", ptr(tp), stride, F, U, ptr(pool.nodes), ptr(pool.node_mask), ptr(payload), t,
                    S, S2, ptr(margin), ptr(rq))
 
-    nodes, node_mask, stats, node_tree, node_gain, pool_size = (pool.nodes, pool.node_mask, pool.stats, pool.node_tree,
-                                                                pool.node_gain, pool.size)
     if ovr:
-        return _ovr_model(rows, K, T, weights, S, stats_t, nodes, node_mask, stats, node_tree, node_gain, payload, pool_size,
-                          margin, U)
-    forest = fr.ForestModel(T, 1, F, rows.arity, rows.mpb, rows.thresholds, rows.n_thr, nodes, node_mask, None, node_tree,
-                            payload[:pool_size].reshape(pool_size, 1).contiguous(), node_gain, pool_size, dt_mode=False)
-    model = GBTModel(forest, weights, stats, S)
+        return _ovr_model(rows, K, T, weights, S, stats_t, pool, payload, margin, U)
+    model = GBTModel(pool.model(rows, T, payload[:pool.size].reshape(pool.size, 1).contiguous()), weights, pool.stats, S)
     model.train_stats = stats_t
     model.train_margin = margin[:U]                      # F of every unique training record (rows: train_margin[train_uid])
     model.train_uid = rows.uid
@@ -433,12 +362,13 @@ def _fit(src, arity, params, row_offset=0, group=None, n_classes=None):
     return model
 
 
-def _ovr_model(rows, K, T, weights, S, stats_t, nodes, node_mask, stats, node_tree, node_gain, payload, pool_size, margin, U):
+def _ovr_model(rows, K, T, weights, S, stats_t, pool, payload, margin, U):
     """the K·T-tree pool -> OvRGBTModel: each class's nodes compacted into their own pool (pool order kept, so its roots
     k·T..k·T+T-1 become 0..T-1 and sibling pairs stay adjacent; left indices remapped), and the combined C = K forest."""
+    nodes, node_mask, stats, node_tree, node_gain = pool.nodes, pool.node_mask, pool.stats, pool.node_tree, pool.node_gain
+    n = pool.size
     dev = nodes.device
     F = rows.F
-    n = pool_size
     tree = node_tree[:n]
     cls = torch.div(tree, T, rounding_mode="floor").long()
     sels = [torch.nonzero(cls == k).view(-1) for k in range(K)]
@@ -466,8 +396,6 @@ def _ovr_model(rows, K, T, weights, S, stats_t, nodes, node_mask, stats, node_tr
     leaf = torch.zeros((max(n, 1), K), dtype=torch.float64, device=dev)
     if n > 0:
         leaf[torch.arange(n, device=dev), cls] = payload[:n]
-    forest = fr.ForestModel(K * T, K, F, rows.arity, rows.mpb, rows.thresholds, rows.n_thr, nodes, node_mask, None, node_tree,
-                            leaf, node_gain, n, dt_mode=False)
-    model = OvRGBTModel(models, forest)
+    model = OvRGBTModel(models, pool.model(rows, K * T, leaf))
     model.train_stats = stats_t
     return model

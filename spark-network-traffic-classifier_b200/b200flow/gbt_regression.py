@@ -137,43 +137,24 @@ def fit_gbt_regressor(x, y, arity, params, row_offset=0, group=None):
     import torch.distributed as dist
     _lib.require_cuda()
     p = params
-    if not (0 <= p.max_depth <= 30):
-        raise ValueError("maxDepth must be in [0, 30], got %d" % p.max_depth)
-    if int(p.max_iter) < 1:
-        raise ValueError("maxIter must be >= 1, got %d" % p.max_iter)
-    if not (0.0 < p.step_size <= 1.0):
-        raise ValueError("stepSize must be in (0, 1], got %r" % p.step_size)
-    if not (0.0 < p.subsampling_rate <= 1.0):
-        raise ValueError("subsamplingRate must be in (0, 1], got %r" % p.subsampling_rate)
+    bg.check_boosting_params(p)
     if p.loss not in LOSSES:
         raise ValueError("lossType must be one of %s, got %r" % (sorted(LOSSES), p.loss))
     loss = LOSSES[p.loss]
-    dev = x.device
-    n, F = x.shape
-    if y.shape[0] != n:
-        raise ValueError("%d labels for %d rows" % (y.shape[0], n))
-    y = y.to(device=dev, dtype=torch.float64).contiguous()
     T = int(p.max_iter)
     seed = int(p.seed) & 0xFFFFFFFFFFFFFFFF
     strategy = "all" if str(p.feature_subset_strategy) == "auto" else p.feature_subset_strategy
+    src, rows = rg._labelled_rows(x, y, arity, p.max_bins, 1, strategy, seed, row_offset, group)
+    dev = x.device
+    n, F = x.shape
     stride = fr.tp_stride(F)
-    # as for the regressors: the label bits ride in the record's padding when there is room, so records merge only when bins
-    # AND label are equal — such rows share F and r at every iteration; without room every row stays its own record
-    in_record = stride - (F + 1) >= 8
-    src = rg._LabelledSource(x, y, in_record)
-    rows = fr._TrainingRows(src, 2, arity, p.max_bins, 1, strategy, seed, row_offset, group, key_bytes=F + 9,
-                            dedup=None if in_record else False).read()
-    tp, uid, U, m, n_bins = rows.tp, rows.uid, rows.U, rows.m, rows.n_bins
+    tp, U, m, n_bins = rows.tp, rows.U, rows.m, rows.n_bins
 
     # subsampling weights W[iteration][unique record] (GBTClassifier's Bernoulli draws per (iteration, global row))
     sub = p.subsampling_rate < 1.0
     TW = T if sub else 1
-    W = torch.zeros(max(TW * U, 1), dtype=torch.int32, device=dev)
-    if n > 0:
-        cdf_host = bg.subsample_cdf(p.subsampling_rate) if sub else None
-        call("b200flow_bag_weights", seed, TW, int(row_offset), n, ptr(_lib.h2d(cdf_host.view(np.int32), dev)) if sub else None,
-             cdf_host.ctypes.data if sub else None, ptr(uid), None, U, ptr(W))
-    del uid
+    cdf_host = bg.subsample_cdf(p.subsampling_rate) if sub else None
+    W = fr.bag_weights(rows, TW, cdf_host, _lib.h2d(cdf_host.view(np.int32), dev) if sub else None, False, seed, row_offset)
 
     # ---- the label check and max |y| on every rank; S = S2 = 61 - ceil(log2 n): a tree's weights never exceed n
     head = torch.cat([(src.flags[0:1] > 0).to(torch.int64), src.flags[1:2]])
@@ -184,25 +165,22 @@ def fit_gbt_regressor(x, y, arity, params, row_offset=0, group=None):
         raise ValueError("a label is NaN or infinite: regression labels must be finite")
     E, S, S2 = rg.label_grid(float(np.array([max_bits], np.int64).view(np.float64)[0]), rows.n_global)
 
-    pool = bg.NodePool(T, max(1024, T * min(1 << (p.max_depth + 1), 64)), bool((rows.kind > 0).any()), dev)
+    pool = fr.NodePool(T, max(1024, T * min(1 << (p.max_depth + 1), 64)), bool((rows.kind > 0).any()), 3, torch.int64, dev)
     weights = [1.0] + [float(p.step_size)] * (T - 1)
     payload = torch.zeros(pool.cap, dtype=torch.float64, device=dev)
     margin = torch.zeros(max(U, 1), dtype=torch.float64, device=dev)
     resid = torch.zeros(max(U, 1), dtype=torch.float64, device=dev)
     rq = torch.zeros((max(U, 1), 2), dtype=torch.int64, device=dev)
     mx = torch.zeros(1, dtype=torch.int64, device=dev)
-    y_vec = None if in_record else y                    # else the label is read from the record's bytes [F + 1, F + 9)
+    y_vec = None if src.in_record else src.y                    # else the label is read from the record's bytes [F + 1, F + 9)
 
     def update(tree):
         mx.zero_()
-        bg._timed("gbr_update", "b200flow_gbr_update", ptr(tp), stride, F + 1, ptr(y_vec), U, ptr(pool.nodes),
+        fr._timed("gbr_update", "b200flow_gbr_update", ptr(tp), stride, F + 1, ptr(y_vec), U, ptr(pool.nodes),
                   ptr(pool.node_mask), ptr(payload), tree, loss, ptr(margin), ptr(resid), ptr(mx))
     update(-1)                                          # F = +0.0, r = y
 
-    nb = (U + 1023) // 1024
-    blk_cnt = torch.zeros(max(nb, 1), dtype=torch.int32, device=dev)
-    blk_off = torch.zeros(nb + 1, dtype=torch.int64, device=dev)
-    total = torch.zeros(1, dtype=torch.int64, device=dev)
+    bag = fr.Bag(1, U, dev)
     ent = torch.empty((max(U, 1), 2), dtype=torch.int32, device=dev)
     ent2 = torch.empty_like(ent)
     Es = []
@@ -216,16 +194,13 @@ def fit_gbt_regressor(x, y, arity, params, row_offset=0, group=None):
             E = residual_exponent(float(np.array([_read(mx)], np.int64).view(np.float64)[0]))
         Es.append(E)
         if U > 0:
-            bg._timed("gbr_grid", "b200flow_reg_grid", None, stride, F + 1, ptr(resid), U, E, S, S2, ptr(rq))
+            fr._timed("gbr_grid", "b200flow_reg_grid", None, stride, F + 1, ptr(resid), U, E, S, S2, ptr(rq))
         loop.S, loop.S2 = S - E, S2 - 2 * E
         # ---- this iteration's entries {unique record, weight}: the non-zero weights, in unique-id order
         Wt = W[(t if sub else 0) * U:(t if sub else 0) * U + max(U, 1)]
-        if U > 0:
-            call("b200flow_bag_count", ptr(Wt), 1, U, ptr(blk_cnt))
-        call("b200flow_exclusive_scan_i32_to_i64", ptr(blk_cnt), nb, ptr(blk_off), ptr(total))
-        if U > 0:
-            call("b200flow_bag_fill", ptr(Wt), 1, U, ptr(blk_off), ptr(ent))
-        ent, ent2 = loop.grow(pool, ent, ent2, torch.zeros(1, dtype=torch.int64, device=dev), total.clone(),
+        bag.count(Wt)
+        bag.fill(Wt, ent)
+        ent, ent2 = loop.grow(pool, ent, ent2, torch.zeros(1, dtype=torch.int64, device=dev), bag.total.clone(),
                               torch.full((1,), t, dtype=torch.int32, device=dev))
         if payload.shape[0] < pool.cap:                 # earlier trees' payloads are kept: they are not recomputed
             grown = torch.zeros(pool.cap, dtype=torch.float64, device=dev)
@@ -234,10 +209,7 @@ def fit_gbt_regressor(x, y, arity, params, row_offset=0, group=None):
         call("b200flow_gbr_leaf_values", pool.size, ptr(pool.stats), ptr(pool.node_tree), t, weights[t], S - E, ptr(payload))
         update(t)
 
-    n_nodes = pool.size
-    forest = fr.ForestModel(T, 1, F, rows.arity, rows.mpb, rows.thresholds, rows.n_thr, pool.nodes, pool.node_mask, None,
-                            pool.node_tree, payload[:n_nodes].reshape(n_nodes, 1).contiguous(), pool.node_gain, n_nodes,
-                            dt_mode=False)
+    forest = pool.model(rows, T, payload[:pool.size].reshape(pool.size, 1).contiguous())
     model = GBTRegressionModel(forest, weights, pool.stats, Es, S, S2)
     model.train_stats = stats_t
     model.train_margin = margin[:U]                      # F of every unique training record (rows: train_margin[train_uid])
@@ -247,13 +219,13 @@ def fit_gbt_regressor(x, y, arity, params, row_offset=0, group=None):
 
 
 def _read(mx):
-    """host copy of the device scalar mx.  With gbt.PROFILE set, the device time from the read's start until the stream
+    """host copy of the device scalar mx.  With forest.PROFILE set, the device time from the read's start until the stream
     resumes after it (the copy and the host round trip the GPU waits through) is recorded as 'gbr_sync'."""
-    if bg.PROFILE is None:
+    if fr.PROFILE is None:
         return int(mx.item())
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     e0.record()
     v = int(mx.item())
     e1.record()
-    bg.PROFILE.setdefault("gbr_sync", []).append((e0, e1))
+    fr.PROFILE.setdefault("gbr_sync", []).append((e0, e1))
     return v

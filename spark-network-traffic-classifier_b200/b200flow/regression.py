@@ -78,6 +78,21 @@ class _LabelledSource(fr._DenseSource):
         return tp, None
 
 
+def _labelled_rows(x, y, arity, max_bins, num_trees, strategy, seed, row_offset, group):
+    """the front half of a regression fit on a dense feature matrix x [n, F] and labels y [n]: -> (the _LabelledSource, whose y
+    holds the labels as f64 on x's device, the read forest._TrainingRows).  The label bits ride in the record's padding when
+    there is room, so records merge only when bins AND label are equal — such rows also share every boosting residual; without
+    room every row stays its own record.  num_classes = 2: every categorical feature is ordered by centroid, as for GBT's
+    regression trees."""
+    n, F = x.shape
+    if y.shape[0] != n:
+        raise ValueError("%d labels for %d rows" % (y.shape[0], n))
+    src = _LabelledSource(x, y.to(device=x.device, dtype=torch.float64).contiguous(), fr.tp_stride(F) - (F + 1) >= 8)
+    rows = fr._TrainingRows(src, 2, arity, max_bins, num_trees, strategy, seed, row_offset, group, key_bytes=F + 9,
+                            dedup=None if src.in_record else False).read()
+    return src, rows
+
+
 class RegressionModel:
     """Device-resident regression trees: one node pool (roots = nodes 0..T-1), payload[node] = the node's mean label.
     prediction = (Σ over the trees, in tree order from +0.0, of the reached leaf's payload) / T."""
@@ -162,35 +177,18 @@ def _fit(x, y, arity, p, row_offset=0, group=None, want_variance=False):
         raise ValueError("numTrees must be >= 1, got %d" % T)
     if not (0.0 < p.subsampling_rate <= 1.0):
         raise ValueError("subsamplingRate must be in (0, 1], got %r" % p.subsampling_rate)
+    seed = int(p.seed) & 0xFFFFFFFFFFFFFFFF
+    src, rows = _labelled_rows(x, y, arity, p.max_bins, T, resolve_strategy(p.feature_subset_strategy, T), seed, row_offset,
+                               group)
     dev = x.device
     n, F = x.shape
-    if y.shape[0] != n:
-        raise ValueError("%d labels for %d rows" % (y.shape[0], n))
-    y = y.to(device=dev, dtype=torch.float64).contiguous()
-    seed = int(p.seed) & 0xFFFFFFFFFFFFFFFF
     stride = fr.tp_stride(F)
-    # the label bits ride in the record's padding when there is room: rows merge only when bins AND label are equal; without
-    # room every row stays its own record
-    in_record = stride - (F + 1) >= 8
-    src = _LabelledSource(x, y, in_record)
-    # num_classes = 2: every categorical feature is ordered by centroid, as for GBT's regression trees
-    rows = fr._TrainingRows(src, 2, arity, p.max_bins, T, resolve_strategy(p.feature_subset_strategy, T), seed, row_offset,
-                            group, key_bytes=F + 9, dedup=None if in_record else False).read()
-    tp, uid, U, m, n_bins = rows.tp, rows.uid, rows.U, rows.m, rows.n_bins
+    tp, U, m, n_bins = rows.tp, rows.U, rows.m, rows.n_bins
     # ---- bag weights W[tree][unique record] (the forest classifier's draws); a decision tree weighs each record by its
     # multiplicity
     bagging = p.bootstrap and T > 1
     cdf_host = np.ascontiguousarray(fr.poisson_cdf_table(p.subsampling_rate)) if bagging else None
-    W = torch.zeros(max(T * U, 1), dtype=torch.int32, device=dev)
-    if n > 0:
-        perm = uperm = None
-        if uid is not None and bagging and U < n:           # group the rows by unique id: one RED per (warp run, tree)
-            gsize = torch.empty(U, dtype=torch.int32, device=dev); cursor = torch.empty(U, dtype=torch.int32, device=dev)
-            goff = torch.empty(U + 1, dtype=torch.int64, device=dev)
-            perm = torch.empty(n, dtype=torch.int32, device=dev); uperm = torch.empty(n, dtype=torch.int32, device=dev)
-            call("b200flow_group_rows", ptr(uid), n, U, ptr(gsize), ptr(goff), ptr(cursor), ptr(perm), ptr(uperm))
-        call("b200flow_bag_weights", seed, T, int(row_offset), n, ptr(_lib.h2d(cdf_host.view(np.int32), dev)) if bagging else None,
-             cdf_host.ctypes.data if bagging else None, ptr(uperm if perm is not None else uid), ptr(perm), U, ptr(W))
+    W = fr.bag_weights(rows, T, cdf_host, _lib.h2d(cdf_host.view(np.int32), dev) if bagging else None, True, seed, row_offset)
     # ---- the label check, max |y| and the largest tree weight: one all-reduce (MAX) of [bad flag, max |y| bits, totals]
     totals = torch.zeros(T, dtype=torch.int64, device=dev)
     call("b200flow_reg_tree_weights", ptr(W), T, U, ptr(totals))
@@ -206,43 +204,30 @@ def _fit(x, y, arity, p, row_offset=0, group=None, want_variance=False):
     E, S, S2 = label_grid(max_abs, w_max)
     rq = torch.zeros((max(U, 1), 2), dtype=torch.int64, device=dev)
     if U > 0:
-        call("b200flow_reg_grid", ptr(tp) if in_record else None, stride, F + 1, None if in_record else ptr(y), U, E, S, S2,
-             ptr(rq))
-    del uid
+        call("b200flow_reg_grid", ptr(tp) if src.in_record else None, stride, F + 1, None if src.in_record else ptr(src.y), U, E,
+             S, S2, ptr(rq))
 
     # ---- entries {unique record, weight} of every tree, tree-major: one level-0 segment per tree root
-    nb = (U + 1023) // 1024
-    blk_cnt = torch.zeros(max(T * nb, 1), dtype=torch.int32, device=dev)
-    blk_off = torch.zeros(T * nb + 1, dtype=torch.int64, device=dev)
-    total = torch.zeros(1, dtype=torch.int64, device=dev)
-    if U > 0:
-        call("b200flow_bag_count", ptr(W), T, U, ptr(blk_cnt))
-    call("b200flow_exclusive_scan_i32_to_i64", ptr(blk_cnt), T * nb, ptr(blk_off), ptr(total))
-    n_ent = int(total.item())
+    bag = fr.Bag(T, U, dev)
+    bag.count(W)
+    n_ent = int(bag.total.item())
     ent = torch.empty((max(n_ent, 1), 2), dtype=torch.int32, device=dev)
     ent2 = torch.empty_like(ent)
-    if U > 0:
-        call("b200flow_bag_fill", ptr(W), T, U, ptr(blk_off), ptr(ent))
+    bag.fill(W, ent)
     del W
-    idx = torch.arange(T, dtype=torch.int64, device=dev) * nb
-    seg_begin, seg_end = blk_off[idx].contiguous(), blk_off[idx + nb].contiguous()
+    seg_begin, seg_end = bag.segments()
 
-    pool = bg.NodePool(T, max(1024, T * min(1 << (p.max_depth + 1), 64)), bool((rows.kind > 0).any()), dev)
+    pool = fr.NodePool(T, max(1024, T * min(1 << (p.max_depth + 1), 64)), bool((rows.kind > 0).any()), 3, torch.int64, dev)
     stats_t = dict(levels=0, slots=0, rows=n, unique_rows=U, entries=n_ent, E=E, S=S, S2=S2)
     loop = bg.LevelLoop(tp, stride, rq, U, F, m, n_bins, rows.feat_bins, rows.feat_kind, S - E, S2 - 2 * E, seed, p, group,
                         stats_t)
     loop.grow(pool, ent, ent2, seg_begin, seg_end, torch.arange(T, dtype=torch.int32, device=dev))
 
-    n_nodes = pool.size
     width = 2 if want_variance else 1
-    table = torch.zeros((max(n_nodes, 1), width), dtype=torch.float64, device=dev)
-    call("b200flow_reg_leaf_table", n_nodes, ptr(pool.stats), S - E, S2 - 2 * E, ptr(table), width)
-
-    def forest_of(leaf):
-        return fr.ForestModel(T, leaf.shape[1], F, rows.arity, rows.mpb, rows.thresholds, rows.n_thr, pool.nodes, pool.node_mask,
-                              None, pool.node_tree, leaf, pool.node_gain, n_nodes, dt_mode=False)
-    forest = forest_of(table[:, 0:1].contiguous())
-    model = RegressionModel(forest, pool.stats, E, S, S2, forest_of(table.contiguous()) if want_variance else None)
+    table = torch.zeros((max(pool.size, 1), width), dtype=torch.float64, device=dev)
+    call("b200flow_reg_leaf_table", pool.size, ptr(pool.stats), S - E, S2 - 2 * E, ptr(table), width)
+    model = RegressionModel(pool.model(rows, T, table[:, 0:1].contiguous()), pool.stats, E, S, S2,
+                            pool.model(rows, T, table.contiguous()) if want_variance else None)
     model.train_stats = stats_t
     model.feat_kind, model.feat_bins, model.n_bins, model.m = rows.kind, rows.feat_bins, n_bins, m
     return model

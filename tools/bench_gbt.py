@@ -106,7 +106,7 @@ def main():
     ap.add_argument("--oracle-rows", type=int, default=0, help="rows for the numpy restatement (0: all of them)")
     ap.add_argument("--repeats", type=int, default=10)
     a = ap.parse_args()
-    from b200flow import gbt as bg
+    from b200flow import forest as fr, gbt as bg
     torch.cuda.set_device(0)
     out = dict(card=card(), rows=a.rows)
     x, y, arity = features(a.rows, 2019)
@@ -118,11 +118,11 @@ def main():
     torch.cuda.synchronize()
     out["fit_s"] = time.perf_counter() - t0
     out["train_stats"] = model.train_stats
-    bg.PROFILE = {}
+    fr.PROFILE = {}
     bg.fit_gbt(x, y, arity, p)
     torch.cuda.synchronize()
-    out["phases_ms"] = {k: round(sum(e0.elapsed_time(e1) for e0, e1 in v), 3) for k, v in bg.PROFILE.items()}
-    bg.PROFILE = None
+    out["phases_ms"] = {k: round(sum(e0.elapsed_time(e1) for e0, e1 in v), 3) for k, v in fr.PROFILE.items()}
+    fr.PROFILE = None
     out["transform_ms"] = events(lambda: model.predict(x), a.repeats)
     pred = model.predict(x)[2]
     out["train_accuracy"] = float((pred == y.to(torch.float64)).to(torch.float64).mean().item())

@@ -64,12 +64,13 @@ def event_ms(fn):
     return e0.elapsed_time(e1)
 
 
-def phases(bg, fn):
-    bg.PROFILE = {}
+def phases(fn):
+    from b200flow import forest as fr
+    fr.PROFILE = {}
     fn()
     torch.cuda.synchronize()
-    out = {k: round(sum(e0.elapsed_time(e1) for e0, e1 in v), 3) for k, v in bg.PROFILE.items()}
-    bg.PROFILE = None
+    out = {k: round(sum(e0.elapsed_time(e1) for e0, e1 in v), 3) for k, v in fr.PROFILE.items()}
+    fr.PROFILE = None
     return out
 
 
@@ -97,7 +98,7 @@ def one(K_req, rows, repeats, bg):
         equal = equal and a.tree_weights == b.tree_weights and torch.equal(a.forest.thresholds, b.forest.thresholds)
     out = dict(classes=K, fit_batched_s=summary(t_b), fit_generic_s=summary(t_g),
                speedup=float(np.median(t_g) / np.median(t_b)), models_equal=bool(equal),
-               train_stats=ovr.train_stats, phases_batched_ms=phases(bg, batched), phases_generic_ms=phases(bg, generic))
+               train_stats=ovr.train_stats, phases_batched_ms=phases(batched), phases_generic_ms=phases(generic))
 
     def joint():
         return ovr.predict(x)

@@ -71,12 +71,13 @@ def events(fn, repeats):
     return float(np.median(ts))
 
 
-def phases(module, fn):
-    module.PROFILE = {}
+def phases(fn):
+    from b200flow import forest as fr
+    fr.PROFILE = {}
     fn()
     torch.cuda.synchronize()
-    out = {k: round(sum(a.elapsed_time(b) for a, b in v), 2) for k, v in module.PROFILE.items()}
-    module.PROFILE = None
+    out = {k: round(sum(a.elapsed_time(b) for a, b in v), 2) for k, v in fr.PROFILE.items()}
+    fr.PROFILE = None
     return out
 
 
@@ -96,7 +97,7 @@ def main():
         model, ms = timed_fit(lambda: br.fit_rf_regressor(x, y, arity, p))
         r = dict(fit_ms=round(ms, 1), nodes=model.n_nodes, unique_rows=model.train_stats["unique_rows"],
                  levels=model.train_stats["levels"], E=model.E, S=model.S)
-        r["phases_ms"] = phases(bg, lambda: br.fit_rf_regressor(x, y, arity, p))
+        r["phases_ms"] = phases(lambda: br.fit_rf_regressor(x, y, arity, p))
         r["transform_ms"] = round(events(lambda: model.predict(x), a.repeats), 2)
         pred = model.predict(x)
         r["evaluator_ms"] = round(events(lambda: bm.regression_metrics(y, pred), a.repeats), 2)
