@@ -585,6 +585,60 @@ int b200flow_isotonic_fit(const void* feature, int32_t feature_dtype, int64_t fe
 int b200flow_isotonic_predict(const void* x, int32_t x_dtype, int64_t stride, int64_t n, const double* boundaries,
                               const double* predictions, int64_t K, double* out, void* stream);
 
+/* ------------------------------------------------------------ column statistics, quantiles, transforms ---
+ * Imputer, RobustScaler, MinMaxScaler, MaxAbsScaler, QuantileDiscretizer and Bucketizer, DESIGN.md §5s.  Every call reads
+ * D >= 1 columns of n rows: value (r, c) is at base + r * row_bytes + cols[2c] with dtype cols[2c + 1] (B200FLOW_F32,
+ * B200FLOW_F64 or B200FLOW_I32), cols int32 [2 D] on the device; row_bytes and the offsets are multiples of 4 (an f64
+ * field needs only 4-byte alignment, as in a raw record).  Values are widened to f64.  A value is missing when it is NaN or,
+ * with has_missing, == missing.
+ * b200flow_column_stats: stats int64 [6][D] (device) = per column the count of non-missing values, of +inf and of -inf;
+ * the smallest and largest ordered key (Java's Double.compare order, -0.0 < 0.0, stored as key ^ 2^63 so that int64 order
+ * is key order; INT64_MAX / INT64_MIN without values); the bits of the largest finite |x| (0 without one).  Sum the first
+ * three rows, min the fourth and max the last two over ranks.
+ * b200flow_column_sums: limbs int64 [D][4] (device, caller zeroes) += the 32-bit limbs (top one signed) of
+ * rint(x 2^shift[c]) over column c's finite non-missing values, shift int32 [D] on the device; n < 2^31.
+ * b200flow_quantile_hist / b200flow_quantile_step: exact rank select over T targets, ordered by column then rank.  state
+ * int64 [6 T + 2 D + 1] (device): ranks [T] (1-based, among the column's non-missing values in Double.compare order),
+ * then T words the library owns, then the values [T] (f64, written by the last step), then the columns [T], then T + 2 D + 1
+ * words the library owns.  The caller fills ranks and columns, calls step(select = 0), then for pass = 0 .. 7: hist (which
+ * zeroes hist int64 [group_bound][256] and counts the pass's digits of every group; group_bound >= the groups of the pass,
+ * at most min(T, active columns 256^pass); at most 48 groups count in shared memory, more in global memory), sums hist over
+ * ranks, and step(select = 1).
+ * b200flow_bucketize: out [n][D] f64 = Spark's Bucketizer.binarySearchForBuckets of value (r, c) over column c's splits
+ * splits[split_off[c] .. split_off[c + 1]) (device, strictly increasing, K >= 3 each): NaN -> K - 1 and flags[r] = 0
+ * (flags uint8 [n], else 1); x == the last split -> the last bucket, K - 2; else
+ * java.util.Arrays.binarySearch's hit or insertion point - 1.  checks int64 [2] (device) = NaN values, values outside the
+ * splits (their output is meaningless and the caller must raise).
+ * b200flow_impute_fill: column c is copied to outs[c] (a device pointer to n contiguous values of the column's own dtype,
+ * outs uint64 [D] on the device) with every missing value replaced by the bits fill_bits[c] (device uint64 [D]; the low 32
+ * bits for f32 / i32 columns).
+ * b200flow_min_max: out [n][D] f64 = (x - emin[c]) * scale[c] + lo when scale[c] != 0, else constant, and NaN for NaN
+ * (emin, scale f64 [D] device), no FMA.
+ * b200flow_mode_keys: keys [n] (device) = the ordered keys of the non-missing values of one column col = {offset, dtype}
+ * (host int32 [2]), -0.0 counted as 0.0, in any order; *count (device int64) = their number.
+ * b200flow_mode: out f64 [2] (device) = the most frequent value among keys [M] (device, M >= 1, overwritten; the padding
+ * key 0xFFFFFFFFFFFFFFFF is ignored) with the smallest one on ties, and its count; NaN and 0 when every key is padding.
+ * scratch: device, 256-byte aligned, b200flow_mode_scratch(M) bytes (host-only query). */
+#define B200FLOW_I32 2
+int b200flow_column_stats(const void* base, int64_t row_bytes, int64_t n, int32_t D, const int32_t* cols, int32_t has_missing,
+                          double missing, int64_t* stats, void* stream);
+int b200flow_column_sums(const void* base, int64_t row_bytes, int64_t n, int32_t D, const int32_t* cols, int32_t has_missing,
+                         double missing, const int32_t* shift, int64_t* limbs, void* stream);
+int b200flow_quantile_hist(const void* base, int64_t row_bytes, int64_t n, int32_t D, const int32_t* cols,
+                           int32_t has_missing, double missing, int64_t T, int64_t* state, int32_t pass, int64_t group_bound,
+                           int64_t* hist, void* stream);
+int b200flow_quantile_step(int64_t T, int32_t D, int64_t* state, const int64_t* hist, int32_t select, void* stream);
+int b200flow_bucketize(const void* base, int64_t row_bytes, int64_t n, int32_t D, const int32_t* cols, const double* splits,
+                       const int32_t* split_off, double* out, uint8_t* flags, int64_t* checks, void* stream);
+int b200flow_impute_fill(const void* base, int64_t row_bytes, int64_t n, int32_t D, const int32_t* cols, int32_t has_missing,
+                         double missing, const uint64_t* fill_bits, const uint64_t* outs, void* stream);
+int b200flow_min_max(const void* base, int64_t row_bytes, int64_t n, int32_t D, const int32_t* cols, const double* emin,
+                     const double* scale, double lo, double constant, double* out, void* stream);
+int b200flow_mode_keys(const void* base, int64_t row_bytes, int64_t n, const int32_t* col, int32_t has_missing, double missing,
+                       uint64_t* keys, int64_t* count, void* stream);
+int b200flow_mode_scratch(int64_t M, int64_t* scratch_bytes);
+int b200flow_mode(uint64_t* keys, int64_t M, void* scratch, int64_t scratch_bytes, double* out, void* stream);
+
 /* ------------------------------------------------------------ factorization machines ---
  * FMClassifier and OneVsRest(FMClassifier), DESIGN.md §5k.  Features x [n_rows][ld] are f32 (x_dtype B200FLOW_F32) or
  * f64 (B200FLOW_F64), converted to f64 before any arithmetic; 1 <= D <= 255, factor_size F >= 1, K >= 1 class columns.

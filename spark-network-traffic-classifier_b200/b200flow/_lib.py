@@ -12,7 +12,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libb200flow.so")
 
-F32, F64 = 0, 1
+F32, F64, I32 = 0, 1, 2
 SRC_F32, SRC_F64, SRC_I32, SRC_INDEX, SRC_ONEHOT = 0, 1, 2, 3, 4
 
 SLOT_DTYPE = np.dtype([("kind", "<i4"), ("src_off", "<i4"), ("lut_off", "<i4"), ("lut_len", "<i4"),
@@ -91,6 +91,15 @@ _SIGNATURES = {
                           _P],
     "b200flow_isotonic_fit": [_P, _I32, _I64, _P, _I64, _P, _I64, _I64, _I32, _I64, _P, _I64, _P, _P, _P, _P, _P],
     "b200flow_isotonic_predict": [_P, _I32, _I64, _I64, _P, _P, _I64, _P, _P],
+    "b200flow_column_stats": [_P, _I64, _I64, _I32, _P, _I32, _F64, _P, _P],
+    "b200flow_column_sums": [_P, _I64, _I64, _I32, _P, _I32, _F64, _P, _P, _P],
+    "b200flow_quantile_hist": [_P, _I64, _I64, _I32, _P, _I32, _F64, _I64, _P, _I32, _I64, _P, _P],
+    "b200flow_quantile_step": [_I64, _I32, _P, _P, _I32, _P],
+    "b200flow_bucketize": [_P, _I64, _I64, _I32, _P, _P, _P, _P, _P, _P, _P],
+    "b200flow_impute_fill": [_P, _I64, _I64, _I32, _P, _I32, _F64, _P, _P, _P],
+    "b200flow_min_max": [_P, _I64, _I64, _I32, _P, _P, _P, _F64, _F64, _P, _P],
+    "b200flow_mode_keys": [_P, _I64, _I64, _P, _I32, _F64, _P, _P, _P],
+    "b200flow_mode": [_P, _I64, _P, _I64, _P, _P],
     "b200flow_fm_loss_grad": [_P, _I32, _I64, _I64, _I32, _I32, _P, _P, _I64, _P, _F64, _U64, _I64, _P, _P],
     "b200flow_fm_regression_loss_grad": [_P, _I32, _I64, _I64, _I32, _I32, _P, _P, _F64, _U64, _I64, _P, _P],
     "b200flow_fm_raw": [_P, _I32, _I64, _I64, _I32, _I32, _I64, _P, _P, _P],
@@ -131,7 +140,7 @@ EXPORTS = sorted(list(_SIGNATURES) + ["b200flow_last_error", "b200flow_version",
                                        "b200flow_packed_layout", "b200flow_binary_counts_scratch",
                                        "b200flow_group_sums_chunks", "b200flow_mlp_config",
                                        "b200flow_svc_config", "b200flow_fm_config",
-                                       "b200flow_isotonic_scratch"])
+                                       "b200flow_isotonic_scratch", "b200flow_mode_scratch"])
 
 _lib = None
 launches = 0   # kernels of OURS launched so far (counted per C-ABI call); bench.py reads the delta over the timed region
@@ -169,6 +178,8 @@ def load():
         lib.b200flow_fm_config.restype = C.c_int
         lib.b200flow_isotonic_scratch.argtypes = [_I64, C.POINTER(_I64)]
         lib.b200flow_isotonic_scratch.restype = C.c_int
+        lib.b200flow_mode_scratch.argtypes = [_I64, C.POINTER(_I64)]
+        lib.b200flow_mode_scratch.restype = C.c_int
         _lib = lib
     return _lib
 
@@ -208,6 +219,15 @@ def isotonic_scratch(n):
     lib = load()
     if lib.b200flow_isotonic_scratch(int(n), C.byref(out)) != 0:
         raise B200FlowError("b200flow_isotonic_scratch failed: %s" % lib.b200flow_last_error().decode())
+    return int(out.value)
+
+
+def mode_scratch(M):
+    """bytes of device scratch b200flow_mode needs for M keys (host-only call)."""
+    out = _I64(0)
+    lib = load()
+    if lib.b200flow_mode_scratch(int(M), C.byref(out)) != 0:
+        raise B200FlowError("b200flow_mode_scratch failed: %s" % lib.b200flow_last_error().decode())
     return int(out.value)
 
 

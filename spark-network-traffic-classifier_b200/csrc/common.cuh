@@ -187,6 +187,53 @@ template <> __device__ __forceinline__ double load_as_double<double>(const void*
     return __ldg((const double*)base + idx);
 }
 
+// ------------------------------------------------------------------ Java double order, exact fixed-point sums
+// (shared by isotonic.cu, quantile.cu and regression.cu)
+// ascending order of x as a uint64, Java's Double.compare: -0.0 sorts before 0.0
+__device__ __forceinline__ unsigned long long asc_key(double x) {
+    const unsigned long long b = (unsigned long long)__double_as_longlong(x);
+    return (b >> 63) ? ~b : (b | (1ull << 63));
+}
+
+// java.util.Arrays.binarySearch(double[], double) on b [K]: the index of a hit, else -(insertion point) - 1.  Equal values
+// order by Double.doubleToLongBits (NaN canonical) as signed longs, so -0.0 < 0.0 and NaN is above everything.
+__device__ __forceinline__ int64_t java_binary_search(const double* __restrict__ b, int64_t K, double key) {
+    const long long kb = key != key ? 0x7ff8000000000000ll : __double_as_longlong(key);
+    int64_t low = 0, high = K - 1;
+    while (low <= high) {
+        const int64_t mid = (low + high) >> 1;
+        const double m = b[mid];
+        if (m < key) low = mid + 1;
+        else if (m > key) high = mid - 1;
+        else {
+            const long long mb = m != m ? 0x7ff8000000000000ll : __double_as_longlong(m);
+            if (mb == kb) return mid;
+            if (mb < kb) low = mid + 1;
+            else high = mid - 1;
+        }
+    }
+    return -(low + 1);
+}
+
+// rint(t 2^sh) (|.| < 2^126) as a two's-complement 128-bit integer: 32-bit limbs, the top one signed
+__device__ __forceinline__ void fixed_limbs(double t, int sh, long long* limb) {
+    const double v = rint(ldexp(t, sh));
+    const double a = fabs(v);
+    unsigned __int128 u;
+    if (a < 9223372036854775808.0) {
+        u = (unsigned __int128)(unsigned long long)a;
+    } else {
+        int e;
+        const double mnt = frexp(a, &e);                               // a = mnt 2^e, 2^63 <= a < 2^126: e - 53 >= 11
+        u = (unsigned __int128)(unsigned long long)ldexp(mnt, 53) << (e - 53);
+    }
+    if (v < 0.0) u = ~u + 1;
+    limb[0] = (long long)(u & 0xffffffffull);
+    limb[1] = (long long)((u >> 32) & 0xffffffffull);
+    limb[2] = (long long)((u >> 64) & 0xffffffffull);
+    limb[3] = (long long)(int)(unsigned)(u >> 96);
+}
+
 // chunk id -> (slot, chunk-in-slot) by binary search over the exclusive scan chunk_off[n_slots+1]
 __device__ __forceinline__ int find_slot(const int64_t* __restrict__ chunk_off, int n_slots, int64_t c) {
     int lo = 0, hi = n_slots;                          // last s with chunk_off[s] <= c

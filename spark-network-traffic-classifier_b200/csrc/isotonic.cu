@@ -24,12 +24,6 @@ constexpr int kIsoChunk = 64;
 constexpr int kIsoThreads = 256;
 constexpr unsigned long long kIsoDropped = ~0ull;       // zero-weight or refused rows: sorted last (no finite key equals it)
 
-// ascending order of x as a uint64, Java's Double.compare: -0.0 sorts before 0.0
-__device__ __forceinline__ unsigned long long asc_key(double x) {
-    const unsigned long long b = (unsigned long long)__double_as_longlong(x);
-    return (b >> 63) ? ~b : (b | (1ull << 63));
-}
-
 template <typename T>
 __global__ void __launch_bounds__(kIsoThreads) iso_keys_kernel(const void* __restrict__ feat, int64_t fstride,
                                                                const double* __restrict__ label, int64_t lstride,
@@ -194,26 +188,6 @@ __global__ void __launch_bounds__(kIsoThreads) iso_emit_kernel(const double* __r
             if (out_w) out_w[o] = v.x;
         }
     }
-}
-
-// java.util.Arrays.binarySearch(double[], double) on b [K]: the index of a hit, else -(insertion point) - 1.  Equal values
-// order by Double.doubleToLongBits (NaN canonical) as signed longs, so -0.0 < 0.0 and NaN is above everything.
-__device__ __forceinline__ int64_t java_binary_search(const double* __restrict__ b, int64_t K, double key) {
-    const long long kb = key != key ? 0x7ff8000000000000ll : __double_as_longlong(key);
-    int64_t low = 0, high = K - 1;
-    while (low <= high) {
-        const int64_t mid = (low + high) >> 1;
-        const double m = b[mid];
-        if (m < key) low = mid + 1;
-        else if (m > key) high = mid - 1;
-        else {
-            const long long mb = m != m ? 0x7ff8000000000000ll : __double_as_longlong(m);
-            if (mb == kb) return mid;
-            if (mb < kb) low = mid + 1;
-            else high = mid - 1;
-        }
-    }
-    return -(low + 1);
 }
 
 template <typename T>

@@ -199,25 +199,6 @@ __global__ void reg_eval_max_kernel(const double* __restrict__ y, const double* 
     }
 }
 
-// rint(t 2^sh) (|.| < 2^126) as a two's-complement 128-bit integer: 32-bit limbs, the top one signed
-__device__ __forceinline__ void fixed_limbs(double t, int sh, long long* limb) {
-    const double v = rint(ldexp(t, sh));
-    const double a = fabs(v);
-    unsigned __int128 u;
-    if (a < 9223372036854775808.0) {
-        u = (unsigned __int128)(unsigned long long)a;
-    } else {
-        int e;
-        const double mnt = frexp(a, &e);                               // a = mnt 2^e, 2^63 <= a < 2^126: e - 53 >= 11
-        u = (unsigned __int128)(unsigned long long)ldexp(mnt, 53) << (e - 53);
-    }
-    if (v < 0.0) u = ~u + 1;
-    limb[0] = (long long)(u & 0xffffffffull);
-    limb[1] = (long long)((u >> 32) & 0xffffffffull);
-    limb[2] = (long long)((u >> 64) & 0xffffffffull);
-    limb[3] = (long long)(int)(unsigned)(u >> 96);
-}
-
 // limbs[k][j] += Σ over the rows of limb j of term k on its grid 2^sh[k]; rows with a non-finite input or term are skipped
 // (the caller has already counted them and returns NaN)
 __global__ void __launch_bounds__(kRegThreads) reg_eval_sums_kernel(const double* __restrict__ y, const double* __restrict__ p,

@@ -1,7 +1,9 @@
 """pyspark.ml.feature shim: StringIndexer, VectorAssembler (used by the reference scripts: kdd99.py:34-35,45-46;
 cicids17.py:41-46) and OneHotEncoder, StandardScaler (named by the north star) — all executed by the fused
 b200flow encode kernel — PCA on the PCA kernels (b200flow/pca.py), and the feature selectors (UnivariateFeatureSelector,
-ChiSqSelector, VarianceThresholdSelector) on the selection kernels (b200flow/selection.py).  Each output column remembers how it derives from the raw record fields
+ChiSqSelector, VarianceThresholdSelector) on the selection kernels (b200flow/selection.py), and the imputer, scalers and
+discretizers (Imputer, RobustScaler, MinMaxScaler, MaxAbsScaler, QuantileDiscretizer, Bucketizer) on the quantile kernels
+(b200flow/quantile.py).  Each output column remembers how it derives from the raw record fields
 (ColumnData.prov), so VectorAssembler / StandardScaler re-run ONE fused kernel over the raw AoS records
 instead of chaining per-stage passes (StringIndexer lookup + one-hot expand + scale + assemble).
 """
@@ -13,12 +15,13 @@ import torch
 from b200flow import dist as bdist
 from b200flow import encode as enc
 from b200flow import pca as _pca
+from b200flow import quantile as _q
 from b200flow import selection as _sel
 from b200flow._lib import SRC_F32, SRC_INDEX, SRC_ONEHOT, B200FlowError
 from b200flow.encode import EncodePlan, RecordSchema
 
 from . import Estimator, Model, Transformer
-from ..sql import ColumnData, DataFrame
+from ..sql import ColumnData, DataFrame, LocalFrame
 from .linalg import DenseMatrix, DenseVector
 
 
@@ -373,34 +376,41 @@ class StandardScalerModel(Model):
         self.mean, self.std = np.asarray(mean, np.float64), np.asarray(std, np.float64)
 
     def _transform(self, df):
-        name, out = self.getOrDefault("inputCol"), self.getOrDefault("outputCol")
-        if out in df._cols:
-            raise IllegalArgumentException("Output column %s already exists." % out)
-        c = df._cols[name]
         D = len(self.mean)
         mean = self.mean if self.getOrDefault("withMean") else np.zeros(D)
         scale = (np.where(self.std != 0, 1.0 / np.where(self.std != 0, self.std, 1.0), 0.0)
                  if self.getOrDefault("withStd") else np.ones(D))
+        return _scale_column(df, self.getOrDefault("inputCol"), self.getOrDefault("outputCol"), mean, scale)
+
+
+def _scale_column(df, name, out, mean, scale):
+    """df with column `out` = (x - mean) * scale of the vector column `name` (StandardScalerModel, RobustScalerModel,
+    MaxAbsScalerModel).  A column with raw-record provenance is re-encoded from the records with the scaling fused into
+    the plan, and keeps that provenance; otherwise the encode kernel scales the dense vector."""
+    if out in df._cols:
+        raise IllegalArgumentException("Output column %s already exists." % out)
+    c = df._cols[name]
+    D = len(mean)
+    plan = None
+    if c.prov is not None and c.prov[0] == "plan" and df._rec is not None:
+        src = c.prov[1]
+        if src.n_out == D and all(s[5] == 0.0 and s[6] == 1.0 for s in src.slots):
+            plan = copy.copy(src); plan.slots = list(src.slots); plan.luts = list(src.luts); plan._dev = None
+            plan.label = None
+            plan.set_scaling(mean, scale)              # fused: index + one-hot + scale + assemble from raw records
+            vec, _, _ = plan.run(df._rec, torch.float64, want_valid=False)
+    if plan is None:
+        x = _materialize(df, name)
+        if x.shape[1] != D:
+            raise IllegalArgumentException("vector size %d does not match the fitted size %d" % (x.shape[1], D))
+        plan = EncodePlan(_dense_schema(D))
+        for i in range(D):
+            plan.add_numeric("v%d" % i, mean[i], scale[i])
+        vec, _, _ = plan.run(x.view(torch.uint8).reshape(x.shape[0], -1), torch.float64, want_valid=False)
         plan = None
-        if c.prov is not None and c.prov[0] == "plan" and df._rec is not None:
-            src = c.prov[1]
-            if src.n_out == D and all(s[5] == 0.0 and s[6] == 1.0 for s in src.slots):
-                plan = copy.copy(src); plan.slots = list(src.slots); plan.luts = list(src.luts); plan._dev = None
-                plan.label = None
-                plan.set_scaling(mean, scale)              # fused: index + one-hot + scale + assemble from raw records
-                vec, _, _ = plan.run(df._rec, torch.float64, want_valid=False)
-        if plan is None:
-            x = _materialize(df, name)
-            if x.shape[1] != D:
-                raise IllegalArgumentException("vector size %d does not match the fitted size %d" % (x.shape[1], D))
-            plan = EncodePlan(_dense_schema(D))
-            for i in range(D):
-                plan.add_numeric("v%d" % i, mean[i], scale[i])
-            vec, _, _ = plan.run(x.view(torch.uint8).reshape(x.shape[0], -1), torch.float64, want_valid=False)
-            plan = None
-        cols = dict(df._cols)
-        cols[out] = ColumnData("vector", vec, "f64", {"attrs": [{"type": "numeric"}] * D}, ("plan", plan) if plan else None)
-        return df._with(cols=cols)
+    cols = dict(df._cols)
+    cols[out] = ColumnData("vector", vec, "f64", {"attrs": [{"type": "numeric"}] * D}, ("plan", plan) if plan else None)
+    return df._with(cols=cols)
 
 
 # ----------------------------------------------------------------------------------- PCA
@@ -621,3 +631,371 @@ class VarianceThresholdSelector(Estimator):
 
 class VarianceThresholdSelectorModel(_SelectorModel):
     _defaults = dict(VarianceThresholdSelector._defaults)
+
+
+# ----------------------------------------------------------------------------------- imputer, scalers, discretizers
+def _check_relative_error(v):
+    if not 0.0 <= v <= 1.0:
+        raise IllegalArgumentException("relativeError must be in [0, 1], got %r" % (v,))
+    return float(v)
+
+
+def _io_cols(stage, single_in="inputCol", multi_in="inputCols", single_out="outputCol", multi_out="outputCols"):
+    """(input columns, output columns) of a stage with inputCol(s) / outputCol(s)"""
+    if stage.getOrDefault(multi_in):
+        if stage.getOrDefault(single_in):
+            raise IllegalArgumentException("%s and %s cannot both be set" % (single_in, multi_in))
+        ins, outs = list(stage.getOrDefault(multi_in)), list(stage.getOrDefault(multi_out) or [])
+    else:
+        ins = [stage.getOrDefault(single_in)] if stage.getOrDefault(single_in) else []
+        outs = [stage.getOrDefault(single_out)] if stage.getOrDefault(single_out) else []
+    if not ins:
+        raise IllegalArgumentException("%s or %s must be set" % (single_in, multi_in))
+    if len(ins) != len(outs):
+        raise IllegalArgumentException("The number of input and output columns must match (%d vs %d)" % (len(ins), len(outs)))
+    return ins, outs
+
+
+def _check_numeric(df, names):
+    for c in names:
+        if c not in df._cols:
+            raise IllegalArgumentException("Field \"%s\" does not exist." % c)
+        col = df._cols[c]
+        if col.kind == "vector" or (col.kind == "field" and df._schema.type_of[c] == "code"):
+            raise IllegalArgumentException("Column %s must be of a numeric type" % c)
+
+
+def _numeric_columns(df, names):
+    """the numeric columns `names` as one Columns: raw record fields read in place through their offsets, one derived
+    column as its tensor; a mix is stacked as f64, which widens exactly, so this serves fits and outputs that are f64
+    whatever the input type (statistics, quantiles, buckets).  Transforms that keep each input's type use _column_groups."""
+    _check_numeric(df, names)
+    if df._rec is not None and all(df._cols[c].kind == "field" for c in names):
+        return _q.record_columns(df._rec, df._schema, names)
+    if len(names) == 1:
+        return _q.columns(df._column_tensor(names[0]))
+    return _q.columns(torch.stack([_materialize(df, c)[:, 0] for c in names], 1))
+
+
+def _column_groups(df, names):
+    """the numeric columns `names` as [(positions in names, Columns)], each column in its own type: every raw record field
+    in one Columns over the records, every derived column in a Columns of its own tensor"""
+    _check_numeric(df, names)
+    fields = [i for i, c in enumerate(names) if df._rec is not None and df._cols[c].kind == "field"]
+    groups = [(fields, _q.record_columns(df._rec, df._schema, [names[i] for i in fields]))] if fields else []
+    for i, c in enumerate(names):
+        if i not in fields:
+            t = df._column_tensor(c)
+            groups.append(([i], _q.columns(t if t.dtype in (torch.float32, torch.float64, torch.int32) else t.to(torch.float64))))
+    return groups
+
+
+def _vector_input(df, name):
+    """a vector column's values [n, D] for a fit: a lazy column is computed without being kept (_peek)"""
+    if name not in df._cols:
+        raise IllegalArgumentException("Field \"%s\" does not exist." % name)
+    c = df._cols[name]
+    if c.kind != "vector":
+        raise IllegalArgumentException("Column %s must be of type vector" % name)
+    if not c.lazy and c.data is not None and c.data.dtype in (torch.float32, torch.float64):
+        return c.data
+    return _peek(df, name)
+
+
+class Imputer(Estimator):
+    """pyspark.ml.feature.Imputer (b200flow/quantile.py, DESIGN.md §5s): mean, median or mode surrogates of numeric columns
+    computed from the values that are neither NaN nor missingValue; the model is the same for any number of ranks."""
+    _defaults = {"inputCol": None, "inputCols": None, "outputCol": None, "outputCols": None, "strategy": "mean",
+                 "missingValue": float("nan"), "relativeError": 0.001}
+
+    def __init__(self, strategy=None, missingValue=None, inputCols=None, outputCols=None, inputCol=None, outputCol=None,
+                 relativeError=None):
+        super().__init__(strategy=strategy, missingValue=missingValue, inputCols=inputCols, outputCols=outputCols,
+                         inputCol=inputCol, outputCol=outputCol, relativeError=relativeError)
+
+    def _fit(self, df):
+        ins, _ = _io_cols(self)
+        strategy = self.getOrDefault("strategy")
+        if strategy not in ("mean", "median", "mode"):
+            raise IllegalArgumentException("strategy must be one of ['mean', 'median', 'mode'], got %r" % (strategy,))
+        _check_relative_error(self.getOrDefault("relativeError"))
+        mv = float(self.getOrDefault("missingValue"))
+        cs = _numeric_columns(df, ins)
+        grp = bdist.group()
+        if strategy == "mean":
+            st = _q.column_stats(cs, mv, grp, with_mean=True)
+            count, sur = st.count, st.mean
+        elif strategy == "median":
+            count = _q.column_stats(cs, mv, grp).count
+            q = _q.select_ranks(cs, [[_q.target_rank(0.5, count[c])] if count[c] else [] for c in range(cs.D)], mv, grp)
+            sur = np.array([v[0] if len(v) else np.nan for v in q])
+        else:
+            sur = _q.mode(cs, mv, grp)
+            count = np.where(np.isnan(sur), 0, 1)
+        for c, name in enumerate(ins):
+            if count[c] == 0:
+                raise SparkException("surrogate cannot be computed. All the values in %s are Null, Nan or missingValue(%r)"
+                                     % (name, mv))
+        m = ImputerModel(dict(zip(ins, (float(v) for v in sur))))
+        m._paramMap = dict(self._paramMap)
+        return m
+
+
+class ImputerModel(Model):
+    _defaults = dict(Imputer._defaults)
+
+    def __init__(self, surrogates):
+        super().__init__()
+        self._surrogates = dict(surrogates)            # input column -> surrogate (f64, before the cast to the column type)
+
+    @property
+    def surrogateDF(self):
+        import pandas as pd
+        return LocalFrame(pd.DataFrame({k: [v] for k, v in self._surrogates.items()}))
+
+    def _transform(self, df):
+        ins, outs = _io_cols(self)
+        for o in outs:
+            if o in df._cols:
+                raise IllegalArgumentException("Output column %s already exists." % o)
+        names = {_q.F32: "f32", _q.F64: "f64", _q.I32: "i32"}
+        mv = float(self.getOrDefault("missingValue"))
+        cols = dict(df._cols)
+        for pos, cs in _column_groups(df, ins):            # one launch per group; every output keeps its input's type
+            filled = _q.fill(cs, [self._surrogates[ins[i]] for i in pos], mv)
+            for i, t, code in zip(pos, filled, cs.dtypes):
+                cols[outs[i]] = ColumnData("numeric", t, names[code], {}, None)
+        return df._with(cols=cols)
+
+
+class RobustScaler(Estimator):
+    """pyspark.ml.feature.RobustScaler (Spark 3.0): per feature the median and the range q(upper) - q(lower) of its
+    non-NaN values, exact quantiles (b200flow/quantile.py); the transform is (x - median) * (1 / range) on the encode plan."""
+    _defaults = {"inputCol": None, "outputCol": None, "lower": 0.25, "upper": 0.75, "withCentering": False,
+                 "withScaling": True, "relativeError": 0.001}
+
+    def __init__(self, lower=None, upper=None, withCentering=None, withScaling=None, inputCol=None, outputCol=None,
+                 relativeError=None):
+        super().__init__(lower=lower, upper=upper, withCentering=withCentering, withScaling=withScaling, inputCol=inputCol,
+                         outputCol=outputCol, relativeError=relativeError)
+
+    def _fit(self, df):
+        lo, hi = self.getOrDefault("lower"), self.getOrDefault("upper")
+        if not 0.0 <= lo <= 1.0 or not 0.0 <= hi <= 1.0:
+            raise IllegalArgumentException("lower and upper must be in [0, 1], got %r and %r" % (lo, hi))
+        if not lo < hi:
+            raise IllegalArgumentException("lower must be less than upper, got %r and %r" % (lo, hi))
+        _check_relative_error(self.getOrDefault("relativeError"))
+        q = _q.quantiles(_vector_input(df, self.getOrDefault("inputCol")), [lo, 0.5, hi], group=bdist.group())
+        median = np.array([v[1] if len(v) else np.nan for v in q])
+        rng = np.array([v[2] - v[0] if len(v) else np.nan for v in q])
+        m = RobustScalerModel(median, rng)
+        m._paramMap = dict(self._paramMap)
+        return m
+
+
+class RobustScalerModel(Model):
+    _defaults = dict(RobustScaler._defaults)
+
+    def __init__(self, median, range_):
+        super().__init__()
+        self._median, self._range = np.asarray(median, np.float64), np.asarray(range_, np.float64)
+
+    @property
+    def median(self):
+        return DenseVector(self._median.copy())
+
+    @property
+    def range(self):
+        return DenseVector(self._range.copy())
+
+    def _transform(self, df):
+        D = len(self._median)
+        shift = self._median if self.getOrDefault("withCentering") else np.zeros(D)
+        if self.getOrDefault("withScaling"):
+            scale = np.array([0.0 if v == 0.0 else 1.0 / v for v in self._range])
+        else:
+            scale = np.ones(D)
+        return _scale_column(df, self.getOrDefault("inputCol"), self.getOrDefault("outputCol"), shift, scale)
+
+
+class MaxAbsScaler(Estimator):
+    """pyspark.ml.feature.MaxAbsScaler: x * (1 / max |x|) per feature (1 for a feature whose max |x| is 0), NaN skipped by
+    the fit; the transform runs on the encode plan."""
+    _defaults = {"inputCol": None, "outputCol": None}
+
+    def __init__(self, inputCol=None, outputCol=None):
+        super().__init__(inputCol=inputCol, outputCol=outputCol)
+
+    def _fit(self, df):
+        st = _q.column_stats(_vector_input(df, self.getOrDefault("inputCol")), group=bdist.group())
+        m = MaxAbsScalerModel(st.max_abs)
+        m._paramMap = dict(self._paramMap)
+        return m
+
+
+class MaxAbsScalerModel(Model):
+    _defaults = dict(MaxAbsScaler._defaults)
+
+    def __init__(self, max_abs):
+        super().__init__()
+        self._max_abs = np.asarray(max_abs, np.float64)
+
+    @property
+    def maxAbs(self):
+        return DenseVector(self._max_abs.copy())
+
+    def _transform(self, df):
+        scale = np.array([1.0 if v == 0.0 else 1.0 / v for v in self._max_abs])
+        return _scale_column(df, self.getOrDefault("inputCol"), self.getOrDefault("outputCol"), np.zeros(len(scale)), scale)
+
+
+class MinMaxScaler(Estimator):
+    """pyspark.ml.feature.MinMaxScaler: (x - E_min) * (max - min) / (E_max - E_min) + min per feature, NaN skipped by the fit
+    and kept by the transform (b200flow_min_max)."""
+    _defaults = {"min": 0.0, "max": 1.0, "inputCol": None, "outputCol": None}
+
+    def __init__(self, min=None, max=None, inputCol=None, outputCol=None):      # noqa: A002 (Spark's parameter names)
+        super().__init__(min=min, max=max, inputCol=inputCol, outputCol=outputCol)
+
+    def _fit(self, df):
+        lo, hi = self.getOrDefault("min"), self.getOrDefault("max")
+        if not lo < hi:
+            raise IllegalArgumentException("min (%r) must be less than max (%r)" % (lo, hi))
+        st = _q.column_stats(_vector_input(df, self.getOrDefault("inputCol")), group=bdist.group())
+        m = MinMaxScalerModel(st.min, st.max)
+        m._paramMap = dict(self._paramMap)
+        return m
+
+
+class MinMaxScalerModel(Model):
+    _defaults = dict(MinMaxScaler._defaults)
+
+    def __init__(self, original_min, original_max):
+        super().__init__()
+        self._omin, self._omax = np.asarray(original_min, np.float64), np.asarray(original_max, np.float64)
+
+    @property
+    def originalMin(self):
+        return DenseVector(self._omin.copy())
+
+    @property
+    def originalMax(self):
+        return DenseVector(self._omax.copy())
+
+    def _transform(self, df):
+        name, out = self.getOrDefault("inputCol"), self.getOrDefault("outputCol")
+        if out in df._cols:
+            raise IllegalArgumentException("Output column %s already exists." % out)
+        lo, hi = float(self.getOrDefault("min")), float(self.getOrDefault("max"))
+        x = _vector_input(df, name)
+        if x.shape[1] != len(self._omin):
+            raise IllegalArgumentException("vector size %d does not match the fitted size %d" % (x.shape[1], len(self._omin)))
+        span = hi - lo
+        rng = self._omax - self._omin
+        scale = np.array([span / r if r != 0.0 else 0.0 for r in rng])
+        vec = _q.min_max(x, self._omin, scale, lo, 0.5 * span + lo)
+        cols = dict(df._cols)
+        cols[out] = ColumnData("vector", vec, "f64", {"attrs": [{"type": "numeric"}] * vec.shape[1]}, None)
+        return df._with(cols=cols)
+
+
+def _check_splits(splits):
+    s = [float(v) for v in splits]
+    if len(s) < 3:
+        raise IllegalArgumentException("Bucketizer splits should have at least 3 split points, got %d" % len(s))
+    if not all(a < b for a, b in zip(s, s[1:])):
+        raise IllegalArgumentException("Bucketizer splits should be strictly increasing, got %r" % (s,))
+    return s
+
+
+class Bucketizer(Transformer):
+    """pyspark.ml.feature.Bucketizer: Spark's binarySearchForBuckets per value (b200flow_bucketize), one launch over every
+    input column.  NaN raises (error), gets index len(splits) - 1 (keep) or drops the row (skip); a value outside the splits
+    raises under every handleInvalid."""
+    _defaults = {"splits": None, "splitsArray": None, "inputCol": None, "inputCols": None, "outputCol": None,
+                 "outputCols": None, "handleInvalid": "error"}
+
+    def __init__(self, splits=None, inputCol=None, outputCol=None, handleInvalid=None, splitsArray=None, inputCols=None,
+                 outputCols=None):
+        super().__init__(splits=splits, inputCol=inputCol, outputCol=outputCol, handleInvalid=handleInvalid,
+                         splitsArray=splitsArray, inputCols=inputCols, outputCols=outputCols)
+
+    def _splits(self, n_in):
+        if self.getOrDefault("inputCols"):
+            arr = self.getOrDefault("splitsArray")
+            if arr is None or len(arr) != n_in:
+                raise IllegalArgumentException("splitsArray must hold one split list per input column")
+            return [_check_splits(s) for s in arr]
+        if self.getOrDefault("splits") is None:
+            raise IllegalArgumentException("splits must be set")
+        return [_check_splits(self.getOrDefault("splits"))]
+
+    def _transform(self, df):
+        ins, outs = _io_cols(self)
+        splits = self._splits(len(ins))
+        hi = _check_handle_invalid(self.getOrDefault("handleInvalid"))
+        for o in outs:
+            if o in df._cols:
+                raise IllegalArgumentException("Output column %s already exists." % o)
+        out, flags, nan, oob = _q.bucketize(_numeric_columns(df, ins), splits)
+        if oob:
+            raise SparkException("Feature value out of Bucketizer bounds (%d values). Check your features, or loosen the "
+                                 "lower/upper bound constraints." % oob)
+        if nan and hi == "error":
+            raise SparkException("Bucketizer encountered NaN value. To handle or skip NaNs, try setting "
+                                 "Bucketizer.handleInvalid.")
+        cols = dict(df._cols)
+        for c, o in enumerate(outs):
+            cols[o] = ColumnData("numeric", out[:, c].contiguous(), "f64", {}, None)
+        res = df._with(cols=cols)
+        return res._compact(flags) if nan and hi == "skip" else res
+
+
+class QuantileDiscretizer(Estimator):
+    """pyspark.ml.feature.QuantileDiscretizer: splits at the exact i / numBuckets quantiles of the non-NaN values, the ends
+    replaced by -inf / +inf, -0.0 normalised to 0.0 and duplicates removed (getDistinctSplits); fit returns a Bucketizer."""
+    _defaults = {"numBuckets": 2, "numBucketsArray": None, "inputCol": None, "inputCols": None, "outputCol": None,
+                 "outputCols": None, "relativeError": 0.001, "handleInvalid": "error"}
+
+    def __init__(self, numBuckets=None, inputCol=None, outputCol=None, relativeError=None, handleInvalid=None,
+                 numBucketsArray=None, inputCols=None, outputCols=None):
+        super().__init__(numBuckets=numBuckets, inputCol=inputCol, outputCol=outputCol, relativeError=relativeError,
+                         handleInvalid=handleInvalid, numBucketsArray=numBucketsArray, inputCols=inputCols,
+                         outputCols=outputCols)
+
+    def _fit(self, df):
+        ins, outs = _io_cols(self)
+        hi = _check_handle_invalid(self.getOrDefault("handleInvalid"))
+        _check_relative_error(self.getOrDefault("relativeError"))
+        if self.getOrDefault("inputCols") and self.getOrDefault("numBucketsArray") is not None:
+            nb = [int(v) for v in self.getOrDefault("numBucketsArray")]
+            if len(nb) != len(ins):
+                raise IllegalArgumentException("numBucketsArray must hold one value per input column")
+        else:
+            nb = [int(self.getOrDefault("numBuckets"))] * len(ins)
+        for k in nb:
+            if k < 2:
+                raise IllegalArgumentException("numBuckets must be >= 2, got %d" % k)
+        q = _q.quantiles(_numeric_columns(df, ins), [[i / k for i in range(1, k)] for k in nb], group=bdist.group())
+        splits = []
+        for name, v in zip(ins, q):
+            if len(v) == 0:
+                raise SparkException("QuantileDiscretizer: column %s has no non-NaN value to compute splits from" % name)
+            try:                                          # an all +-inf column leaves only [-inf, +inf]
+                splits.append(_check_splits(distinct_splits([-np.inf] + list(v) + [np.inf])))
+            except IllegalArgumentException as e:
+                raise IllegalArgumentException("QuantileDiscretizer: the splits of column %s are invalid: %s" % (name, e))
+        b = Bucketizer(handleInvalid=hi)
+        if self.getOrDefault("inputCols"):
+            b._set(inputCols=ins, outputCols=outs, splitsArray=splits)
+        else:
+            b._set(inputCol=ins[0], outputCol=outs[0], splits=splits[0])
+        return b
+
+
+def distinct_splits(splits):
+    """Spark's QuantileDiscretizer.getDistinctSplits: ends -inf / +inf, -0.0 -> 0.0, duplicates removed in order"""
+    s = [float(v) for v in splits]
+    s[0], s[-1] = -np.inf, np.inf
+    return list(dict.fromkeys(0.0 if v == 0.0 else v for v in s))

@@ -447,6 +447,41 @@ class DataFrame:
     def rdd(self):
         return _RDD(self.collect())
 
+    def approxQuantile(self, col, probabilities, relativeError):
+        """DataFrameStatFunctions.approxQuantile over numeric columns (b200flow/quantile.py): the exact element of rank
+        ceil(q n) among the non-NaN values, which is within any relativeError of the target; [] for a column without a
+        value.  col: a name (-> list of floats) or a list of names (-> one list per column)."""
+        from b200flow import dist as bdist
+        from b200flow import quantile as q
+        if not relativeError >= 0.0:
+            raise ValueError("Relative Error must be non-negative but got %r" % (relativeError,))
+        names = [col] if isinstance(col, str) else list(col)
+        probs = q.check_probabilities(probabilities)
+        for c in names:
+            if c not in self._cols or self._cols[c].kind == "vector" or \
+                    (self._cols[c].kind == "field" and self._schema.type_of[c] == "code"):
+                raise ValueError("approxQuantile needs numeric columns, got %r" % c)
+        if self._rec is not None and all(self._cols[c].kind == "field" for c in names):
+            cs = q.record_columns(self._rec, self._schema, names)
+        else:
+            cs = q.columns(torch.stack([self._column_tensor(c).to(torch.float64) for c in names], 1))
+        res = [[float(v) for v in r] for r in q.quantiles(cs, probs, group=bdist.group())]
+        return res[0] if isinstance(col, str) else res
+
+    @property
+    def stat(self):
+        return _StatFunctions(self)
+
+
+class _StatFunctions:
+    """df.stat (pyspark.sql.DataFrameStatFunctions): approxQuantile"""
+
+    def __init__(self, df):
+        self._df = df
+
+    def approxQuantile(self, col, probabilities, relativeError):
+        return self._df.approxQuantile(col, probabilities, relativeError)
+
 
 def _java_repl(r):
     return re.sub(r"\$(\d+)", r"\\\1", r)
