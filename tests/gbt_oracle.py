@@ -193,7 +193,7 @@ def walk(nodes, bins):
 def leaf_value(nd, weight, S):
     st = nd["stats"]
     with np.errstate(all="ignore"):
-        return weight * ((float(st[1]) * 2.0 ** -S) / float(st[0]))
+        return weight * ((np.float64(st[1]) * 2.0 ** -S) / np.float64(st[0]))      # 0/0 = NaN for an empty node
 
 
 def boost(bins, labels, W, feat_bins, feat_kind, m, max_iter, step_size, max_depth, min_inst, min_gain, seed, n_global=None):
