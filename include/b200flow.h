@@ -335,23 +335,7 @@ int b200flow_finalize_forest(int64_t n_nodes, const uint32_t* pool_counts, int32
                              double* leaf_prob, void* stream);
 
 /* ----------------------------------------------------------------- predict ---
- * R9  RandomForestClassificationModel.transform (kdd99.py:82, cicids17.py:86) — HOT LOOP C.  Walks all T trees for every
- * binned row; raw[n][C] = Σ_t leaf_prob (tree order, fp64), prob = raw/Σraw, pred = first argmax.
- * dt_mode != 0 (DecisionTreeClassifier): raw = leaf class counts.  raw/prob may be NULL. */
-int b200flow_predict(const uint8_t* tp, int32_t tp_stride, int64_t n_rows,
-                     const b200flow_node* nodes, const uint64_t* node_mask,
-                     const double* leaf_prob, const uint32_t* pool_counts,
-                     int32_t T, int32_t C, int32_t dt_mode,
-                     const void* top_nodes /* NULL or the table of b200flow_build_top_nodes */, int32_t top_levels,
-                     double* raw, double* prob, double* pred, void* stream);
-
-/* shared-memory table for predict: top[tree][nid] (16-byte b200flow_node, [T][2^top_levels], entry 0 unused) = the tree's
- * node with MLlib node id nid < 2^top_levels.  Built once per model; the walk of the first top_levels levels then reads
- * shared memory instead of issuing one L1 request per lane and level. */
-int b200flow_build_top_nodes(const b200flow_node* nodes, const int32_t* node_tree, int64_t n_nodes, int32_t T,
-                             int32_t top_levels, void* top, void* stream);
-
-/* per-tree compact layout for b200flow_predict_forest, built once per model in two calls.  Tree t (t < T; pool nodes of
+ * per-tree compact layout for b200flow_predict_forest, built once per model in two calls.  Tree t (t < T; pool nodes of
  * other trees are ignored) owns the 8-byte words [tree_off[t], tree_off[t+1]) of `layout`: its nodes in pool order (8-byte
  * records, child and payload offsets local to the tree), the C fp64 votes of its leaves (leaf_prob, or pool_counts as fp64
  * when dt_mode != 0) and the left-set masks of its categorical splits.
@@ -363,9 +347,11 @@ int b200flow_build_forest_layout(const b200flow_node* nodes, const uint64_t* nod
                                  const uint32_t* pool_counts, const int32_t* node_tree, int64_t n_nodes, int32_t T, int32_t C,
                                  int32_t dt_mode, const int32_t* scratch, const int64_t* tree_off, uint64_t* layout, void* stream);
 
-/* R9 over the compact layout: what b200flow_predict computes (raw, prob, pred bit for bit; raw/prob may be NULL), with each
- * tree staged whole in shared memory (the first words of a tree larger than the buffer; the rest read from global).
- * F = features (bins tp[row][0..F-1]). */
+/* R9  RandomForestClassificationModel.transform (kdd99.py:82, cicids17.py:86) — HOT LOOP C.  Walks all T trees of the
+ * compact layout for every binned row; raw[n][C] = Σ_t leaf votes (tree order, fp64, from 0.0), prob = raw/Σraw,
+ * pred = first argmax.  The votes are leaf_prob, or the leaf class counts when the layout was built with dt_mode != 0
+ * (DecisionTreeClassifier).  raw/prob may be NULL.  Each tree is staged whole in shared memory (the first words of a tree
+ * larger than the buffer; the rest read from global).  F = features (bins tp[row][0..F-1]). */
 int b200flow_predict_forest(const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows, const uint64_t* layout,
                             const int64_t* tree_off, int32_t T, int32_t C, double* raw, double* prob, double* pred, void* stream);
 
@@ -378,13 +364,20 @@ int b200flow_gather_rows(const void* src, int32_t row_bytes, const int32_t* idx,
 int b200flow_confusion(const double* pred, const double* label, int64_t n_rows, int32_t C,
                        int64_t* cm, void* stream);
 
+/* shared-memory table for b200flow_predict_grid_confusion / _scores: top[tree][nid] (16-byte b200flow_node,
+ * [T][2^top_levels], entry 0 unused) = the tree's node with MLlib node id nid < 2^top_levels.  Built once per model; the
+ * walk of the first top_levels levels then reads shared memory instead of issuing one L1 request per lane and level. */
+int b200flow_build_top_nodes(const b200flow_node* nodes, const int32_t* node_tree, int64_t n_nodes, int32_t T,
+                             int32_t top_levels, void* top, void* stream);
+
 /* Model selection (CrossValidator / TrainValidationSplit over numTrees x maxDepth, DESIGN.md §5a): confusion matrices of
  * every truncated forest (first T_i trees, cut at depth d_j) on the validation records, from ONE walk of each tree.
  * tp[n_rows][tp_stride] = UNIQUE binned records with the label at byte F; mult[n_rows] = rows per unique record.
  * tree_cuts_host: 1 <= T_1 < ... < T_I <= T (I <= 256); depth_cuts_host: 0 <= d_1 < ... < d_J <= 30.
  * cm int64 [I][J][cm_side][cm_side] (cm_side >= C, caller zeroes): cm[i][j][label][pred] += mult, where pred is what
- * b200flow_predict gives for the truncated forest; labels >= cm_side are not counted.  max_depth_cuts_per_launch: 0 = as many
- * as shared memory holds (the result does not depend on it). */
+ * b200flow_predict_forest gives for the truncated forest; labels >= cm_side are not counted.  max_depth_cuts_per_launch: 0 = as many
+ * as shared memory holds (the result does not depend on it).
+ * top_nodes: NULL or the table of b200flow_build_top_nodes with top_levels levels. */
 int b200flow_predict_grid_confusion(const uint8_t* tp, int32_t tp_stride, int32_t F, int64_t n_rows, const int32_t* mult,
                                     const b200flow_node* nodes, const uint64_t* node_mask, const double* leaf_prob,
                                     const uint32_t* pool_counts, int32_t T, int32_t C, int32_t dt_mode,

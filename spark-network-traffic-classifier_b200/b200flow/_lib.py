@@ -62,7 +62,6 @@ _SIGNATURES = {
     "b200flow_plan_route": [_I32, _P, _P, _P, _I32, _P, _P, _P, _P, _P],
     "b200flow_next_segments": [_I32, _P, _P, _P, _P, _P, _P, _P, _P],
     "b200flow_finalize_forest": [_I64, _P, _I32, _P, _P],
-    "b200flow_predict": [_P, _I32, _I64, _P, _P, _P, _P, _I32, _I32, _I32, _P, _I32, _P, _P, _P, _P],
     "b200flow_build_top_nodes": [_P, _P, _I64, _I32, _I32, _P, _P],
     "b200flow_forest_layout_size": [_P, _P, _I64, _I32, _I32, _P, _P, _P],
     "b200flow_build_forest_layout": [_P, _P, _P, _P, _P, _I64, _I32, _I32, _I32, _P, _P, _P, _P],

@@ -21,7 +21,7 @@ from ._lib import NODE_DTYPE, SPLIT_DTYPE, B200FlowError, UnsupportedParamError,
 import os as _os
 CHUNK_ROWS = 2048                  # entries per CTA in hist_level / partition_level (<= 2048)
 FUSED = True                       # use route_hist_level (partition + next-level histogram in one pass) when it fits
-TOP_LEVELS = int(_os.environ.get("B200FLOW_TOP_LEVELS", "8"))   # tree levels the predict kernel walks in shared memory (0 = none)
+TOP_LEVELS = int(_os.environ.get("B200FLOW_TOP_LEVELS", "8"))   # tree levels the grid predict kernel walks in shared memory (0 = none)
 DEDUP = True                       # run the level loop on unique binned records (flow records repeat massively)
 _PIN = True                        # read the per-level counts into pinned host memory
 PROFILE = None                     # set to a dict to collect per-kernel CUDA-event timings (bench.py)
@@ -264,8 +264,8 @@ class ForestModel:
         return tp, bad[0:1]
 
     def _top_table(self):
-        """the first TOP_LEVELS levels of every tree, heap-indexed by node id, for the predict kernel's shared-memory stage
-        (built once per model)."""
+        """the first TOP_LEVELS levels of every tree, heap-indexed by node id, for the grid predict kernel's shared-memory
+        stage (built once per model)."""
         if TOP_LEVELS <= 0:
             return None, 0
         if getattr(self, "_top", None) is None:

@@ -147,7 +147,7 @@ def fit_gbt_ovr_records(rec, plan, K, arity, params, row_offset=0, group=None, r
 class OvRGBTModel:
     """OneVsRest over K binary GBT models trained together.  models[k] is class k's GBTModel on its own node pool; `forest`
     is the combined pool (K·T trees, tree k·T + t = class k's tree t) with C = K, whose leaf_prob[node] is one-hot on the class
-    of the node's tree and carries the node's payload.  One b200flow_predict over it gives every class's margin — class k's
+    of the node's tree and carries the node's payload.  One b200flow_predict_forest over it gives every class's margin — class k's
     column adds its own payloads and +0.0 for the other classes' trees, in tree order from +0.0, so it has the bits of
     models[k].margin — and the first argmax under Spark's `>` rule."""
 

@@ -76,9 +76,6 @@ class GBTRegressionModel:
         fo = self.forest
         pre = fr.ForestModel(k, 1, fo.F, fo.arity, fo.max_bins, fo.thresholds, fo.n_thr, fo.nodes, fo.node_mask, None,
                              fo.node_tree, fo.leaf_prob, fo.node_gain, fo.n_nodes, dt_mode=False)
-        top, _ = fo._top_table()
-        if top is not None:                              # heap-indexed per tree: the first k trees' rows are the prefix's
-            pre._top = top
         pre._layout = fo._forest_layout()                # per-tree blocks in tree order: the first k are the prefix's
         return pre
 

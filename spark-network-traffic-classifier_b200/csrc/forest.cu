@@ -12,7 +12,6 @@
 // with sparse global REDs, so the multi-GPU all-reduce sees one dense uint32 buffer per level.
 #include <float.h>
 #include <stdlib.h>
-#include <string.h>
 
 #include "common.cuh"
 
@@ -574,7 +573,7 @@ struct RouteArgs {
     int route;                                  // 1: write the routed entries + cursors (first pass of a routed level)
 };
 
-// M = compile-time number of subset features of the pass (merged shared atomics); M = 0: generic path.
+// M = compile-time number of subset features of the pass (rotated shared atomics); M = 0: generic path (passes wider than 12).
 // Barrier-free inner loop: a chunk is NW sub-chunks of KS * 32 entries, one per warp.  Per warp and step t:
 //     entries(t+2) -> registers (prefetch) | record gather(t) -> private tile (LDGSTS; hidden by the other resident warps)
 //     write-out of step t-1 (its cursor reservation, a global atomic issued one step earlier, has landed by now)
@@ -587,13 +586,12 @@ struct RouteArgs {
 // (side, j) histogram << 16.  The lane-major layout keeps every table read conflict-free.
 __host__ __device__ inline size_t route_tab_bytes(int mp, bool packed) { return packed && mp <= 12 ? (size_t)2 * mp * 32 * 8 : 0; }
 
-template <int M, int NW, int KS, int MERGE, int NQ>   // MERGE: 0 plain shared atomics (runtime m), 1 top-group merge,
-                                                      // 2 rotated features; NQ: 16-byte granules of a bit-packed record
-                                                      // (a.field_desc, a.stride == 16 * NQ), 0: byte records
+template <int M, int NW, int KS, int NQ>   // M > 0: rotated features, M = 0: plain shared atomics (runtime m); NQ: 16-byte
+                                          // granules of a bit-packed record (a.field_desc, a.stride == 16 * NQ), 0: byte records
 __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) route_hist_level_kernel(const RouteArgs a) {
     extern __shared__ __align__(16) uint32_t sm_u32[];
     constexpr bool PACKED = NQ > 0;
-    constexpr bool kTab = PACKED && M > 0 && MERGE == 2;     // histogram update through the per-lane descriptor table
+    constexpr bool kTab = PACKED && M > 0;                   // histogram update through the per-lane descriptor table
     constexpr int kThreads = NW * 32, kSub = KS * 32;
     constexpr int gran = PACKED ? 16 : kGran;
     const int m = M > 0 ? M : a.m;
@@ -761,30 +759,12 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) rou
                 const uint32_t mL = __ballot_sync(0xffffffffu, d == 1), mR = __ballot_sync(0xffffffffu, d == 2);
                 nL += __popc(mL); nR += __popc(mR);
                 if (d != 0) {
-                    const uint32_t active = mL | mR;
                     const int side = d - 1;
                     const int* fpos = sh_fpos + side * m;
                     uint32_t* hist = sh_hist + side * hsz;
                     const uint32_t lab = field(i, lab_pos);
                     const uint32_t w = e[k].y;
-                    if (M > 0 && MERGE == 1) {
-                        // top-group merge: per feature, the lanes that share the first active lane's (bin, label, child) counter are
-                        // summed with ONE redux over the whole active mask (the others contribute 0: no divergence) and issue one
-                        // shared atomic; the other lanes add alone.  A per-feature match.any merge would issue one redux per
-                        // distinct mask, which serialises.
-                        const uint32_t tag = (lab << 8) | ((uint32_t)side << 16);
-#pragma unroll
-                        for (int j = 0; j < M; ++j) {
-                            const int fp = fpos[j];
-                            const uint32_t bin = field(i, fp);
-                            const uint32_t key = bin | tag;
-                            uint32_t* addr = &hist[j * nbC + bin * a.C + lab];
-                            const int l0 = __ffs(active) - 1;
-                            const bool top = key == __shfl_sync(active, key, l0);          // same counter as the first active lane
-                            const uint32_t sum = __reduce_add_sync(active, top ? w : 0u);  // no divergence: the others contribute 0
-                            if (!top || lane == l0) atomicAdd(addr, top ? sum : w);
-                        }
-                    } else if (kTab) {
+                    if (kTab) {
                         // rotated features through the descriptor table: one table read, one tile read, one shared atomic
                         const uint2* tab = sh_tab + side * (M * 32) + lane;
                         const uint8_t* rec = (const uint8_t*)tile + i * rs;
@@ -796,7 +776,7 @@ __global__ void __launch_bounds__(NW * 32, NW == 8 ? 3 : (NW == 16 ? 2 : 1)) rou
                             const uint32_t bin = __funnelshift_r(v, 0u, dd.y) & ((dd.y >> 8) & 0xffu);
                             atomicAdd(hl + (dd.y >> 16) + bin * a.C, w);
                         }
-                    } else if (M > 0 && MERGE == 2) {
+                    } else if (M > 0) {
                         // rotated features: lane i walks the subset positions in the order (i + t) % M, so that one warp
                         // instruction spreads over all M features — the lanes 8 apart (same bank for a 48-byte pitch) read
                         // different record words, and only ~32 / M lanes can meet on one hot counter.  Integer sums: same result.
@@ -886,17 +866,9 @@ static bool route_cfg(int F, int rs, bool packed, int m, int n_bins, int C, Rout
     return true;
 }
 
-// histogram update of the fused kernel: 2 = rotated features (default), 1 = top-group merge, 0 = generic runtime loop.
-// Tuning knob B200FLOW_ROUTE_VARIANT, read per call: "merge" / "generic".
-static int route_hist_variant() {
-    const char* e = getenv("B200FLOW_ROUTE_VARIANT");
-    if (e && !strcmp(e, "merge")) return 1;
-    if (e && !strcmp(e, "generic")) return 0;
-    return 2;
-}
-
+// M = 1..12: the rotated histogram update compiled for that pass width; any other M: the generic runtime loop
 template <int NW, int KS, int NQ>
-static cudaError_t route_launch(int M, int merge, unsigned grid_cap, size_t smem, int per_sm_hint, int waves, int64_t n_chunks_max,
+static cudaError_t route_launch(int M, unsigned grid_cap, size_t smem, int per_sm_hint, int waves, int64_t n_chunks_max,
                                 const RouteArgs& a, cudaStream_t st) {
     cudaError_t e = cudaSuccess;
 #define B2F_ROUTE_GO(KERNEL)                                                                                                   \
@@ -912,16 +884,11 @@ static cudaError_t route_launch(int M, int merge, unsigned grid_cap, size_t smem
         if (grid_cap && grid > grid_cap) grid = grid_cap;                                                                      \
         KERNEL<<<grid, NW * 32, smem, st>>>(a);                                                                                \
     }
-#define B2F_ROUTE_CASE(MM)                                                                                                     \
-    case MM:                                                                                                                   \
-        if (merge == 1) B2F_ROUTE_GO((route_hist_level_kernel<MM, NW, KS, 1, NQ>))                                         \
-        else if (merge == 2) B2F_ROUTE_GO((route_hist_level_kernel<MM, NW, KS, 2, NQ>))                                    \
-        else B2F_ROUTE_GO((route_hist_level_kernel<0, NW, KS, 0, NQ>))                                                     \
-        break;
+#define B2F_ROUTE_CASE(MM) case MM: B2F_ROUTE_GO((route_hist_level_kernel<MM, NW, KS, NQ>)) break;
     switch (M) {
         B2F_ROUTE_CASE(1) B2F_ROUTE_CASE(2) B2F_ROUTE_CASE(3) B2F_ROUTE_CASE(4) B2F_ROUTE_CASE(5) B2F_ROUTE_CASE(6)
         B2F_ROUTE_CASE(7) B2F_ROUTE_CASE(8) B2F_ROUTE_CASE(9) B2F_ROUTE_CASE(10) B2F_ROUTE_CASE(11) B2F_ROUTE_CASE(12)
-        default: B2F_ROUTE_GO((route_hist_level_kernel<0, NW, KS, 0, NQ>)) break;
+        default: B2F_ROUTE_GO((route_hist_level_kernel<0, NW, KS, NQ>)) break;
     }
 #undef B2F_ROUTE_CASE
 #undef B2F_ROUTE_GO
@@ -929,13 +896,13 @@ static cudaError_t route_launch(int M, int merge, unsigned grid_cap, size_t smem
 }
 
 template <int NQ>
-static cudaError_t route_shape(const RouteCfg& cfg, int M, int merge, size_t smem, int waves, int64_t n_chunks_max, const RouteArgs& a,
+static cudaError_t route_shape(const RouteCfg& cfg, int M, size_t smem, int waves, int64_t n_chunks_max, const RouteArgs& a,
                                cudaStream_t st) {
-    if (cfg.nw == 8 && cfg.ks == 2) return route_launch<8, 2, NQ>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
-    if (cfg.nw == 8) return route_launch<8, 1, NQ>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
-    if (cfg.nw == 16 && cfg.ks == 2) return route_launch<16, 2, NQ>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
-    if (cfg.nw == 16) return route_launch<16, 1, NQ>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
-    return route_launch<32, 1, NQ>(M, merge, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+    if (cfg.nw == 8 && cfg.ks == 2) return route_launch<8, 2, NQ>(M, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+    if (cfg.nw == 8) return route_launch<8, 1, NQ>(M, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+    if (cfg.nw == 16 && cfg.ks == 2) return route_launch<16, 2, NQ>(M, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+    if (cfg.nw == 16) return route_launch<16, 1, NQ>(M, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
+    return route_launch<32, 1, NQ>(M, 0, smem, cfg.per_sm, waves, n_chunks_max, a, st);
 }
 
 __global__ void next_segments_kernel(int n_next, const int64_t* __restrict__ n_next_dev, const int32_t* __restrict__ next_parent,
@@ -1142,19 +1109,17 @@ extern "C" int b200flow_route_hist_level(const uint8_t* tp, int32_t tp_stride, i
     a.subset_next = subset_next; a.m_total = m; a.n_bins = n_bins; a.C = C; a.hist_next = hist_next;
     static int waves = -1;                                    // CTAs per resident slot: > 1 lets the block scheduler even out the tail
     if (waves < 0) { const char* e = getenv("B200FLOW_ROUTE_WAVES"); waves = e ? atoi(e) : 2; if (waves < 1) waves = 1; }
-    int merge = route_hist_variant();
-    if (merge == 1 && C > 128) merge = 2;                      // the merge key packs the label into 8 bits
     for (int j0 = 0, pass = 0; j0 < m; j0 += cfg.m_pass, ++pass) {
         a.j0 = j0; a.m = m - j0 < cfg.m_pass ? m - j0 : cfg.m_pass; a.route = (route && pass == 0) ? 1 : 0;
         const int M = a.m <= 12 ? a.m : 0;
         const size_t smem = route_hist_smem(rs, field_desc != nullptr, a.m, n_bins, C, cfg.nw, cfg.ks);
         cudaError_t e;
         switch (field_desc ? tp_stride / 16 : 0) {               // packed: granules per record, a compile-time gather geometry
-            case 1: e = route_shape<1>(cfg, M, merge, smem, waves, n_chunks_max, a, st); break;
-            case 2: e = route_shape<2>(cfg, M, merge, smem, waves, n_chunks_max, a, st); break;
-            case 3: e = route_shape<3>(cfg, M, merge, smem, waves, n_chunks_max, a, st); break;
-            case 4: e = route_shape<4>(cfg, M, merge, smem, waves, n_chunks_max, a, st); break;
-            default: e = route_shape<0>(cfg, M, merge, smem, waves, n_chunks_max, a, st); break;
+            case 1: e = route_shape<1>(cfg, M, smem, waves, n_chunks_max, a, st); break;
+            case 2: e = route_shape<2>(cfg, M, smem, waves, n_chunks_max, a, st); break;
+            case 3: e = route_shape<3>(cfg, M, smem, waves, n_chunks_max, a, st); break;
+            case 4: e = route_shape<4>(cfg, M, smem, waves, n_chunks_max, a, st); break;
+            default: e = route_shape<0>(cfg, M, smem, waves, n_chunks_max, a, st); break;
         }
         if (e != cudaSuccess) { set_error("route_hist_level: %s", cudaGetErrorString(e)); return B200FLOW_ERR_CUDA; }
     }

@@ -5,8 +5,8 @@
 // S = 60 - ceil(log2 n), S2 = 58 - ceil(log2 n)), so every histogram cell {Σw, Σw·q, Σw·q2} is an exact int64 sum below 2^62:
 // the all-reduce over ranks, the shared- and global-memory atomics and the order of the entries cannot change a bit.
 // The tree structure reuses the forest's: b200flow_split records, b200flow_partition_level, b200flow_next_segments,
-// b200flow_grow_level (the three int64 stats travel as 6 opaque words per node) and b200flow_predict (C = 1 over the
-// payloads).  OneVsRest(GBTClassifier) grows the K binary problems' trees side by side (DESIGN.md §5f): the _classes entry
+// b200flow_grow_level (the three int64 stats travel as 6 opaque words per node) and b200flow_predict_forest (C = 1
+// over the payloads).  OneVsRest(GBTClassifier) grows the K binary problems' trees side by side (DESIGN.md §5f): the _classes entry
 // points read each slot's residuals from its class's block and update every (class, record) pair.  Compiled with -fmad=false: every fp64 expression below is restated operation for operation by the test oracle.
 #include <float.h>
 

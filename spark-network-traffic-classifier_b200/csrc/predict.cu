@@ -3,130 +3,17 @@
 // randomSplit and stable row compaction.
 // Reference call sites: model.transform(test_set) kdd99.py:82 / cicids17.py:86; evaluator.evaluate
 // kdd99.py:86-91; randomSplit kdd99.py:52; where / handleInvalid="skip" cicids17.py:30-35,41.
-#include <stdlib.h>
 #include <type_traits>
 
 #include "common.cuh"
 
 namespace b200flow {
 
-// ------------------------------------------------------------------ R9 predict
-// A thread owns kPredRows rows and walks them through each tree TOGETHER: the walk is a chain of dependent 16-byte node
-// loads (L1/L2 hits: the pool of a 100-tree depth-16 forest is a few MB), so two independent chains per thread double the
-// memory-level parallelism.  A row's bins live in transposed smem (word k of thread t at [k*blockDim + t], conflict-free);
-// votes accumulate in fp64, in tree order, in smem ([class*blockDim + t]).
-//
-// What bounds the walk is the L1: below the first few levels every lane of a warp is at a different node, so each level costs
-// 32 separate sector requests per warp and row (long-scoreboard stalls: the t-stage serialises them).  The top `top_levels` levels of the CURRENT tree (2^K - 1 nodes, heap-indexed by MLlib's node id) are therefore
-// staged in shared memory, double-buffered with cp.async one tree ahead: a scattered LDS.128 costs a handful of bank
-// wavefronts instead of 32 tag lookups, and only the levels below K go to the L1/L2.
-
-// top[tree][nid] = the tree's node with MLlib id nid, for nid < 2^K (entry 0 unused)
-__global__ void __launch_bounds__(256) build_top_kernel(const int4* __restrict__ nodes, const int32_t* __restrict__ node_tree,
-                                                        int64_t n_nodes, int K, int4* top) {
-    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n_nodes) return;
-    const int4 nd = nodes[i];
-    if ((uint32_t)nd.w < (1u << K)) top[((int64_t)node_tree[i] << K) + nd.w] = nd;
-}
-
-template <int kPredRows>
-__global__ void __launch_bounds__(128) predict_kernel(const uint8_t* __restrict__ tp, int stride, int64_t n,
-                                                      const b200flow_node* __restrict__ nodes,
-                                                      const unsigned long long* __restrict__ node_mask,
-                                                      const double* __restrict__ leaf_prob,
-                                                      const uint32_t* __restrict__ pool_counts, int T, int C, int dt_mode,
-                                                      const int4* __restrict__ top, int K,
-                                                      double* raw, double* prob, double* pred) {
-    extern __shared__ __align__(16) uint8_t sm[];
-    const int bd = blockDim.x, tid = threadIdx.x;
-    const int words = stride / 4;
-    uint32_t* binw = (uint32_t*)sm;                                           // [kPredRows][words][bd]
-    double* votes = (double*)(sm + (size_t)kPredRows * words * bd * 4);       // [kPredRows][C][bd]
-    const int topn = top ? (1 << K) : 0;
-    int4* topbuf = (int4*)(votes + (size_t)kPredRows * C * bd);               // [2][topn] when the top table is given
-    auto stage_top = [&](int t, int buf) {                                    // asynchronous copy of tree t's table
-        if (t < T) for (int i = tid; i < topn; i += bd) cp_async16(topbuf + (size_t)buf * topn + i, top + ((int64_t)t << K) + i);
-        cp_async_commit();
-    };
-    for (int64_t base = (int64_t)blockIdx.x * bd * kPredRows; base < n; base += (int64_t)gridDim.x * bd * kPredRows) {
-        int64_t row[kPredRows]; bool live[kPredRows];
-#pragma unroll
-        for (int r = 0; r < kPredRows; ++r) {
-            row[r] = base + (int64_t)r * bd + tid; live[r] = row[r] < n;
-            uint32_t* bw = binw + (size_t)r * words * bd;
-            if (live[r]) {
-                const uint4* src = (const uint4*)(tp + row[r] * stride);
-                for (int q = 0; q < words / 4; ++q) {
-                    const uint4 v = ld_stream_u4(src + q);
-                    bw[(4 * q + 0) * bd + tid] = v.x; bw[(4 * q + 1) * bd + tid] = v.y;
-                    bw[(4 * q + 2) * bd + tid] = v.z; bw[(4 * q + 3) * bd + tid] = v.w;
-                }
-            }
-            for (int k = 0; k < C; ++k) votes[((size_t)r * C + k) * bd + tid] = 0.0;
-        }
-        const uint32_t* bw0 = binw + tid;                                   // this thread's column of the transposed bins
-        const int4* nodes4 = (const int4*)nodes;                            // {feat, kind<<16|bin, left, nid}
-        if (top) stage_top(0, 0);
-        for (int t = 0; t < T; ++t) {
-            const int4* tb = topbuf + (size_t)(t & 1) * topn;
-            if (top) {
-                cp_async_wait_all();
-                __syncthreads();                                            // table of tree t landed; everybody left tree t-1
-                stage_top(t + 1, (t + 1) & 1);
-            }
-            int idx[kPredRows]; uint32_t nid[kPredRows]; int4 nd[kPredRows];
-#pragma unroll
-            for (int r = 0; r < kPredRows; ++r) { idx[r] = t; nid[r] = 1u; nd[r] = top ? tb[1] : __ldg(nodes4 + t); if (!live[r]) nd[r].x = -1; }
-            while (true) {
-                bool any = false;
-#pragma unroll
-                for (int r = 0; r < kPredRows; ++r) {
-                    if (nd[r].x >= 0) {
-                        const int f = nd[r].x;
-                        const int bin = (bw0[(r * words + (f >> 2)) * bd] >> ((f & 3) * 8)) & 0xff;
-                        const int right = nd[r].y < 65536 ? (bin > nd[r].y)
-                                                          : !((node_mask[(int64_t)idx[r] * 4 + (bin >> 6)] >> (bin & 63)) & 1ull);
-                        idx[r] = nd[r].z + right;
-                        nid[r] = 2u * nid[r] + (uint32_t)right;
-                        any = true;
-                    }
-                }
-                if (!any) break;
-#pragma unroll
-                for (int r = 0; r < kPredRows; ++r)
-                    if (nd[r].x >= 0) nd[r] = nid[r] < (uint32_t)topn ? tb[nid[r]] : __ldg(nodes4 + idx[r]);
-            }
-#pragma unroll
-            for (int r = 0; r < kPredRows; ++r) {
-                if (!live[r]) continue;
-                double* vt = votes + (size_t)r * C * bd + tid;
-                if (dt_mode) { for (int k = 0; k < C; ++k) vt[k * bd] += (double)pool_counts[(int64_t)idx[r] * C + k]; }
-                else { for (int k = 0; k < C; ++k) vt[k * bd] += leaf_prob[(int64_t)idx[r] * C + k]; }
-            }
-        }
-#pragma unroll
-        for (int r = 0; r < kPredRows; ++r) {
-            if (!live[r]) continue;
-            const double* vt = votes + (size_t)r * C * bd + tid;
-            double s = 0.0; int arg = 0; double best = vt[0];
-            for (int k = 0; k < C; ++k) { const double v = vt[k * bd]; s += v; if (v > best) { best = v; arg = k; } }
-            for (int k = 0; k < C; ++k) {
-                const double v = vt[k * bd];
-                if (raw) raw[row[r] * C + k] = v;
-                if (prob) prob[row[r] * C + k] = s != 0.0 ? v / s : 0.0;
-            }
-            pred[row[r]] = (double)arg;
-        }
-        if (top) { cp_async_wait_all(); __syncthreads(); }                  // the look-ahead copy of the last tree is a no-op commit
-    }
-}
-
 // ------------------------------------------------------------------ R9 predict over the per-tree compact layout
-// predict_kernel's walk is bound by L1 tag lookups: below the heap-indexed top table every lane's node load (and, at the
-// leaf, each of its C vote loads) is a separate request.  A KDD tree is small once compacted (~1,900 nodes: ~15 KB of
-// 8-byte nodes plus ~37 KB of C = 5 fp64 leaf votes), so the whole tree is staged in shared memory and every walk step and
-// vote add becomes a scattered LDS.
+// A walk through the pool is bound by L1 tag lookups: below the first few levels every lane of a warp is at a different
+// node, so every node load (and, at the leaf, each of its C vote loads) is a separate request.  A KDD tree is small once
+// compacted (~1,900 nodes: ~15 KB of 8-byte nodes plus ~37 KB of C = 5 fp64 leaf votes), so the whole tree is staged in
+// shared memory and every walk step and vote add becomes a scattered LDS.
 //
 // Layout (8-byte words), built once per model: tree t owns words [tree_off[t], tree_off[t+1]), padded to an even count.
 //   [0, n_t)            node records in pool order (the pool is level-major, so this is the tree's BFS order), uint2 {a, b}:
@@ -244,12 +131,12 @@ __global__ void __launch_bounds__(256) layout_fill_kernel(const int4* __restrict
     blk[local[i]] = rec;
 }
 
-// A CTA owns a block of rows (one per thread; bins transposed in shared memory as in predict_kernel) and walks them
-// through the trees in order.  Tree t's block is staged with cp.async into one of two buffers while tree t-1 is walked; a
+// A CTA owns a block of rows (one per thread; bins transposed in shared memory, word k of thread t at [k*blockDim + t],
+// conflict-free) and walks them through the trees in order.  Tree t's block is staged with cp.async into one of two buffers while tree t-1 is walked; a
 // word at offset o of the block is read from shared memory when o < cap (the buffer size) and from global memory otherwise,
 // so a tree larger than the buffer keeps its first (top-level) nodes in shared memory.  A tree that fits is walked by the
 // same code compiled without the bound check, which saves the compare and select on every load.  The last tree of a round
-// stages tree 0 of the next.  Votes add in fp64, in tree order, from 0.0: predict_kernel's adds, bit for bit.
+// stages tree 0 of the next.  Votes add in fp64, in tree order, from 0.0.
 // kRegC > 0 (C <= kRegC): the votes accumulate in registers, not in shared memory: no shared-memory read-modify-write per
 // class and leaf, and 8·C more bytes per row for the tree buffers (every KDD99 tree then fits).  The bin of feature f is one
 // byte load from the thread's column: byte f & 3 of word f >> 2, at (f >> 2)·4·bd + (f & 3) = (f & ~3)·bd + (f & 3).
@@ -387,11 +274,28 @@ __global__ void __launch_bounds__(256) confusion_kernel(const double* __restrict
 
 // ------------------------------------------------------------------ grid prediction -> confusion matrices (model selection)
 // For fixed other params, the forest fitted with (T, d) is the first T trees of the (T_max, d_max) forest cut at depth d
-// (DESIGN.md §5a).  One thread owns one UNIQUE validation record (label at byte F, multiplicity mult[row]) and walks each
-// tree once, down to a leaf or to the deepest depth cut of this launch.  The node met at depth cut j (or the leaf the walk
-// ended on above it) adds its payload to votes[j] in tree order, from 0.0: the fp64 adds predict_kernel performs for the
-// truncated forest.  After tree T_i - 1 the first argmax of every votes[j] (predict_kernel's `v > best` rule) is counted
-// into cm[i][j][label][pred].  A launch covers depth cuts [j0, j0 + jn) of J.
+// (DESIGN.md §5a).  One thread owns one UNIQUE validation record (label at byte F, multiplicity mult[row]; its bins in
+// transposed smem, word k of thread t at [k*blockDim + t]) and walks each tree once through the pool's 16-byte nodes, down
+// to a leaf or to the deepest depth cut of this launch.  The node met at depth cut j (or the leaf the walk ended on above
+// it) adds its payload to votes[j] in tree order, from 0.0: the fp64 adds of predicting with the truncated forest.  After
+// tree T_i - 1 the first argmax of every votes[j] (the `v > best` rule of predict_forest_kernel) is counted into
+// cm[i][j][label][pred].  A launch covers depth cuts [j0, j0 + jn) of J.
+//
+// What bounds the walk is the L1: below the first few levels every lane of a warp is at a different node, so each level
+// costs 32 separate sector requests per warp.  The top `top_levels` levels of the CURRENT tree (2^K - 1 nodes,
+// heap-indexed by MLlib's node id; build_top_kernel) are therefore staged in shared memory, double-buffered with cp.async
+// one tree ahead: a scattered LDS.128 costs a handful of bank wavefronts instead of 32 tag lookups, and only the levels
+// below K go to the L1/L2.
+
+// top[tree][nid] = the tree's node with MLlib id nid, for nid < 2^K (entry 0 unused)
+__global__ void __launch_bounds__(256) build_top_kernel(const int4* __restrict__ nodes, const int32_t* __restrict__ node_tree,
+                                                        int64_t n_nodes, int K, int4* top) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_nodes) return;
+    const int4 nd = nodes[i];
+    if ((uint32_t)nd.w < (1u << K)) top[((int64_t)node_tree[i] << K) + nd.w] = nd;
+}
+
 constexpr int kGridMaxTreeCuts = 256;
 constexpr int kGridMaxDepthCuts = 31;                 // depths 0..30
 struct GridCuts { int32_t tree[kGridMaxTreeCuts]; int32_t depth[kGridMaxDepthCuts]; };
@@ -573,38 +477,6 @@ extern "C" int b200flow_build_top_nodes(const b200flow_node* nodes, const int32_
     if (n_nodes <= 0) return B200FLOW_OK;
     build_top_kernel<<<(unsigned)((n_nodes + 255) / 256), 256, 0, (cudaStream_t)stream>>>((const int4*)nodes, node_tree, n_nodes, top_levels, (int4*)top);
     return check_launch("build_top_nodes");
-}
-
-extern "C" int b200flow_predict(const uint8_t* tp, int32_t tp_stride, int64_t n_rows, const b200flow_node* nodes,
-                                const uint64_t* node_mask, const double* leaf_prob, const uint32_t* pool_counts, int32_t T,
-                                int32_t C, int32_t dt_mode, const void* top_nodes, int32_t top_levels,
-                                double* raw, double* prob, double* pred, void* stream) {
-    if (n_rows <= 0) return B200FLOW_OK;            // empty batch: nothing to do (pointers may be NULL)
-    B2F_REQUIRE(tp && nodes && pred && T > 0 && C > 0 && (tp_stride & 15) == 0, "predict: bad arguments");
-    B2F_REQUIRE(dt_mode ? pool_counts != nullptr : leaf_prob != nullptr, "predict: missing leaf payload");
-    B2F_REQUIRE(((uintptr_t)tp & 15) == 0, "predict: tp must be 16-byte aligned");
-    B2F_REQUIRE(!top_nodes || (top_levels >= 1 && top_levels <= 10 && ((uintptr_t)top_nodes & 15) == 0), "predict: bad top table");
-    static int rows_per_thread = -1;                      // tuning knob: independent tree walks per thread (memory-level parallelism)
-    if (rows_per_thread < 0) { const char* e = getenv("B200FLOW_PRED_ROWS"); rows_per_thread = (e && atoi(e) == 4) ? 4 : 2; }
-    const int kPredRows = rows_per_thread;
-    int bd = 128;
-    size_t per_thread = ((size_t)tp_stride + (size_t)C * 8) * kPredRows;
-    while (bd > 32 && per_thread * bd > 96 * 1024) bd >>= 1;
-    size_t smem = per_thread * bd + (top_nodes ? (size_t)2 * 16 * ((size_t)1 << top_levels) : 0);
-    B2F_REQUIRE(smem <= 200 * 1024, "predict: too many classes/features for shared memory");
-    int grid = grid_for(n_rows, bd * kPredRows, kNumSMs * 16);
-    cudaError_t e;
-    if (kPredRows == 4) {
-        e = cudaFuncSetAttribute(predict_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) predict_kernel<4><<<grid, bd, smem, (cudaStream_t)stream>>>(tp, tp_stride, n_rows, nodes, (const unsigned long long*)node_mask, leaf_prob,
-                                                                                          pool_counts, T, C, dt_mode, (const int4*)top_nodes, top_levels, raw, prob, pred);
-    } else {
-        e = cudaFuncSetAttribute(predict_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e == cudaSuccess) predict_kernel<2><<<grid, bd, smem, (cudaStream_t)stream>>>(tp, tp_stride, n_rows, nodes, (const unsigned long long*)node_mask, leaf_prob,
-                                                                                          pool_counts, T, C, dt_mode, (const int4*)top_nodes, top_levels, raw, prob, pred);
-    }
-    if (e != cudaSuccess) { set_error("predict: %s", cudaGetErrorString(e)); return B200FLOW_ERR_CUDA; }
-    return check_launch("predict");
 }
 
 extern "C" int b200flow_forest_layout_size(const b200flow_node* nodes, const int32_t* node_tree, int64_t n_nodes, int32_t T,

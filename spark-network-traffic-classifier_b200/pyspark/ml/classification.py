@@ -1145,7 +1145,7 @@ class OneVsRestModel(Model, _OneVsRestParams):
         return df._with(cols=cols)
 
     def _joint_predict(self, df, fcol):
-        """one tree walk over the K·T trees (b200flow_predict with C = K): the margins and the `>` argmax in one kernel"""
+        """one tree walk over the K·T trees (b200flow_predict_forest with C = K): the margins and the `>` argmax in one kernel"""
         j = self._joint
         if isinstance(j, (_OvRSVCJoint, _OvRFMJoint)):
             try:

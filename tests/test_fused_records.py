@@ -100,16 +100,31 @@ def test_every_launch_shape_builds_the_same_forest(shape, monkeypatch):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", ["merge", "generic"])
-@pytest.mark.parametrize("classes", [5, 23])
-def test_histogram_update_variants_build_the_same_forest(variant, classes, monkeypatch):
-    # B200FLOW_ROUTE_VARIANT: the default rotated-feature update vs the top-group merge vs the generic runtime loop
-    rec, plan, arity, C = _kdd_records(60000, classes, 29)
-    x, y, _ = plan.run(rec, torch.float64)
-    p = fr.ForestParams(num_trees=6, max_bins=70, max_depth=9, seed=3)
+@pytest.mark.parametrize("kind,classes", [("kdd", 5), ("kdd", 23), ("bytes78", 6), ("bytes78", 15)])
+def test_histogram_update_variants_build_the_same_forest(kind, classes, monkeypatch):
+    # featureSubsetStrategy="all": feature passes wider than 12, so the fused kernel runs its generic runtime loop instead of
+    # the rotated-feature update, on KDD's 32-byte packed records and on 78 features of 78 bins (7 bits: byte records)
+    if kind == "kdd":
+        rec, plan, arity, C = _kdd_records(60000, classes, 29)
+        x, y, _ = plan.run(rec, torch.float64)
+        p = fr.ForestParams(num_trees=6, max_bins=70, max_depth=9, seed=3, feature_subset_strategy="all")
+        fmt = ("packed", 32)
+    else:
+        g = torch.Generator(device=DEV); g.manual_seed(classes)
+        x = torch.rand((60000, 78), dtype=torch.float64, device=DEV, generator=g)
+        y = ((x[:, :6] > 0.5).sum(1) + (x[:, 6] + x[:, 7] > 1.0)) % classes
+        C, arity = classes, [0] * 78
+        y = y.to(torch.int32)
+        p = fr.ForestParams(num_trees=4, max_bins=78, max_depth=8, seed=3, feature_subset_strategy="all")
+        fmt = ("bytes", fr.tp_stride(78))
+    monkeypatch.setattr(fr, "FUSED", False)
     want = fr.fit_forest(x, y, C, arity, p).export()
-    monkeypatch.setenv("B200FLOW_ROUTE_VARIANT", variant)
-    got = fr.fit_forest(x, y, C, arity, p).export()
+    monkeypatch.setattr(fr, "FUSED", True)
+    m = fr.fit_forest(x, y, C, arity, p)
+    F = len(arity)
+    assert (m.train_stats["record_format"], m.train_stats["record_bytes"]) == fmt
+    assert -(-F // m.train_stats["route_passes"]) > 12                     # balanced passes: each wider than 12 features
+    got = m.export()
     assert forests_equal(got, want) == [] and np.array_equal(got["gain"], want["gain"])
 
 

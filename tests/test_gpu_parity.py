@@ -440,7 +440,7 @@ def test_dedup_does_not_change_the_forest(monkeypatch):
 
 def test_large_batch_size_independent_properties(monkeypatch):
     # Sizes the oracle cannot finish in seconds (1.2 M rows, 24 trees, depth 12) are checked through properties that do not
-    # depend on the size: (1) the product path (fused level kernel, unique records, top-level table, sharded-style padding)
+    # depend on the size: (1) the product path (fused level kernel, unique records, sharded-style padding)
     # builds byte for byte the forest of the plainest path (row-by-row, unfused hist + partition kernels); (2) the root
     # histogram of every tree sums to its bag weight total: sum of the roots' class counts == sum of the entries' weights;
     # (3) predictions do not depend on de-duplicating the test records, and raw votes sum to the number of trees.
@@ -457,7 +457,6 @@ def test_large_batch_size_independent_properties(monkeypatch):
     assert np.allclose(raw_a.sum(1).cpu().numpy(), 24.0, rtol=0, atol=1e-9)
     monkeypatch.setattr(fr, "DEDUP", False)
     monkeypatch.setattr(fr, "FUSED", False)
-    monkeypatch.setattr(fr, "TOP_LEVELS", 0)
     plain = fr.fit_forest(x, y, C, arity, p)
     ex_plain = plain.export()
     assert forests_equal(ex_fast, ex_plain) == [] and np.array_equal(ex_fast["gain"], ex_plain["gain"])

@@ -1,8 +1,9 @@
 """The three kernels of one forest level (csrc/forest.cu) called one by one through the C ABI, on synthetic records, entries
 and splits whose edges are placed on purpose, against the plain restatement in tests/level_oracle.py:
 
-  route_hist_level  every launch shape x histogram update, byte and 16/32/48/64-byte packed records, subset widths 1..13 and
-                    feature passes, 2..200 classes, segment lengths around the chunk size, one-sided and dropped children,
+  route_hist_level  every launch shape x histogram update (the subset width picks it: the rotated update up to 12 features a
+                    pass, the generic loop above), byte and 16/32/48/64-byte packed records, subset widths 1..41 and feature
+                    passes, 2..200 classes, segment lengths around the chunk size, one-sided and dropped children,
                     categorical masks in all four words, hot counters with large weights;
   partition_level + next_segments (the unfused routing);
   score_level       ragged and serial prefix scans, exact ties, ordered categoricals up to 255 categories, unordered ones with
@@ -26,8 +27,14 @@ from util import forests_equal
 
 DEV = "cuda"
 SHAPES = ["8x2", "8x1", "16x2", "16x1", "32x1"]
-VARIANTS = ["rotated", "merge", "generic"]
 SENTINEL = -7
+WIDTHS = ["narrow", "wide", "all"]
+
+
+def _width(name, narrow, F):
+    """subset width of each histogram update: `narrow` (rotated), `wide` = 13 (the generic loop: a pass wider than 12) or
+    every feature (featureSubsetStrategy="all"; feature passes where the child histograms do not fit at once)"""
+    return {"narrow": narrow, "wide": 13, "all": F}[name]
 
 
 def unordered_features(n, C, seed):
@@ -166,10 +173,8 @@ class RouteCase:
         self.subset_next = np.stack([np.sort(rng.choice(F, m, replace=False)) for _ in range(self.n_next)]).astype(np.int16)
 
 
-def _run_route(case, packed, route=True, extra_chunks=37, variant=None, shape=None, monkeypatch=None):
+def _run_route(case, packed, route=True, extra_chunks=37, shape=None, monkeypatch=None):
     """b200flow_route_hist_level on the case; returns (hist, ent_out, cursors, config)."""
-    if variant is not None and variant != "rotated":
-        monkeypatch.setenv("B200FLOW_ROUTE_VARIANT", variant)
     if shape is not None:
         monkeypatch.setenv("B200FLOW_ROUTE_SHAPE", shape)
     F, C, m, n_bins = case.F, case.C, case.m, case.n_bins
@@ -268,33 +273,35 @@ def _format(name):
 # ------------------------------------------------------------------------------------------------ route_hist_level
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape", SHAPES)
-@pytest.mark.parametrize("variant", VARIANTS)
+@pytest.mark.parametrize("width", WIDTHS)
 @pytest.mark.parametrize("fmt", ["bytes41", "packed32"])
-def test_route_variant_x_shape(fmt, variant, shape, monkeypatch):
+def test_route_variant_x_shape(fmt, width, shape, monkeypatch):
     F, fb, packed = _format(fmt)
+    m = _width(width, 7, F)
     nw, ks = map(int, shape.split("x"))
-    rng = np.random.default_rng(zlib.crc32((fmt + variant + shape).encode()))
-    case = RouteCase(rng, fb, 5, _lens(nw * ks * 32), 7)
-    got = _run_route(case, packed, variant=variant, shape=shape, monkeypatch=monkeypatch)
-    assert got[3][1] == 7
+    rng = np.random.default_rng(zlib.crc32((fmt + width + shape).encode()))
+    case = RouteCase(rng, fb, 5, _lens(nw * ks * 32), m)
+    got = _run_route(case, packed, shape=shape, monkeypatch=monkeypatch)
+    assert got[3][1] == m                                 # one pass of 7 (rotated), 13 or 41 (generic loop) features
     _check_route(case, got)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", VARIANTS)
+@pytest.mark.parametrize("width", WIDTHS)
 @pytest.mark.parametrize("fmt", list(FORMATS))
-def test_route_record_formats(fmt, variant, monkeypatch):
+def test_route_record_formats(fmt, width, monkeypatch):
     F, fb, packed = _format(fmt)
-    rng = np.random.default_rng(len(fmt) * 7 + F)
-    ch = _lib.route_hist_config(F, 9, max(fb), 5, FORMATS[fmt][2])[0]
-    case = RouteCase(rng, fb, 5, _lens(ch), 9)
-    _check_route(case, _run_route(case, packed, variant=variant, monkeypatch=monkeypatch))
+    mm = _width(width, 9, F)
+    rng = np.random.default_rng(len(fmt) * 7 + F + mm)
+    ch = _lib.route_hist_config(F, mm, max(fb), 5, FORMATS[fmt][2])[0]
+    case = RouteCase(rng, fb, 5, _lens(ch), mm)
+    _check_route(case, _run_route(case, packed, monkeypatch=monkeypatch))
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", VARIANTS)
-@pytest.mark.parametrize("m", list(range(1, 14)) + ["passes"])
-def test_route_subset_width(m, variant, monkeypatch):
+@pytest.mark.parametrize("m", list(range(1, 42)) + ["passes"])
+def test_route_subset_width(m, monkeypatch):
+    # every width of a 41-feature record in one pass: the rotated update compiled for 1..12, the generic loop from 13
     rng = np.random.default_rng(100 + (m if m != "passes" else 99))
     if m == "passes":                                     # child histograms too wide for one pass: only pass 0 routes
         F, fb, C, mm = 78, [64] * 78, 23, 36
@@ -305,43 +312,46 @@ def test_route_subset_width(m, variant, monkeypatch):
         ch, m_pass = _lib.route_hist_config(F, mm, 70, C, 0)
         assert m_pass == mm
     case = RouteCase(rng, fb, C, _lens(ch), mm)
-    got = _run_route(case, False, variant=variant, monkeypatch=monkeypatch)
+    got = _run_route(case, False, monkeypatch=monkeypatch)
     assert got[3][1] == m_pass
     _check_route(case, got)
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", VARIANTS)
+@pytest.mark.parametrize("width", WIDTHS)
 @pytest.mark.parametrize("C", [2, 23, 200])
-def test_route_classes(C, variant, monkeypatch):
-    # C > 128: the merge key has 8 label bits, so the merge update falls back to the rotated one
-    rng = np.random.default_rng(C)
+def test_route_classes(C, width, monkeypatch):
+    # C = 200: the wider subsets run in feature passes
+    m = _width(width, 5, 30)
+    rng = np.random.default_rng(C + m)
     fb = [16] * 30
-    case = RouteCase(rng, fb, C, _lens(_lib.route_hist_config(30, 5, 16, C, 0)[0]), 5)
-    _check_route(case, _run_route(case, False, variant=variant, monkeypatch=monkeypatch))
+    case = RouteCase(rng, fb, C, _lens(_lib.route_hist_config(30, m, 16, C, 0)[0]), m)
+    _check_route(case, _run_route(case, False, monkeypatch=monkeypatch))
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("fmt", ["bytes41", "packed48"])
-@pytest.mark.parametrize("variant", VARIANTS)
-def test_route_hot_counter_large_weights(variant, fmt, monkeypatch):
+@pytest.mark.parametrize("width", WIDTHS)
+def test_route_hot_counter_large_weights(width, fmt, monkeypatch):
     F, fb, packed = _format(fmt)
+    mm = _width(width, 6, F)
     rng = np.random.default_rng(7)
-    ch = _lib.route_hist_config(F, 6, max(fb), 5, FORMATS[fmt][2])[0]
-    case = RouteCase(rng, fb, 5, [0, 3 * ch + 17, ch, 11, 2 * ch, 40, 900], 6, hot=True)
-    _check_route(case, _run_route(case, packed, variant=variant, monkeypatch=monkeypatch))
+    ch = _lib.route_hist_config(F, mm, max(fb), 5, FORMATS[fmt][2])[0]
+    case = RouteCase(rng, fb, 5, [0, 3 * ch + 17, ch, 11, 2 * ch, 40, 900], mm, hot=True)
+    _check_route(case, _run_route(case, packed, monkeypatch=monkeypatch))
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("variant", VARIANTS)
-def test_route_masks_in_all_words(variant, monkeypatch):
+@pytest.mark.parametrize("width", WIDTHS)
+def test_route_masks_in_all_words(width, monkeypatch):
     # 256-bin categorical splits: mask words 1-3 decide for bins 64-255
+    m = _width(width, 4, 15)
     rng = np.random.default_rng(256)
     fb = [256] * 12 + [200, 130, 65]
-    ch = _lib.route_hist_config(15, 4, 256, 3, 0)[0]
-    case = RouteCase(rng, fb, 3, _lens(ch), 4, cat_every=1)
+    ch = _lib.route_hist_config(15, m, 256, 3, 0)[0]
+    case = RouteCase(rng, fb, 3, _lens(ch), m, cat_every=1)
     assert (case.split["kind"][2:] == 1).all()
-    _check_route(case, _run_route(case, False, variant=variant, monkeypatch=monkeypatch))
+    _check_route(case, _run_route(case, False, monkeypatch=monkeypatch))
 
 
 @pytest.mark.gpu

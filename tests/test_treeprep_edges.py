@@ -1,5 +1,4 @@
-"""Launch paths of the tree-preparation kernels (csrc/treeprep.cu) and the batch predictor (csrc/predict.cu) that the
-end-to-end forest tests never reach, each called through the C ABI and compared exactly with the CPU oracle or numpy.
+"""Launch paths of the tree-preparation kernels (csrc/treeprep.cu) that the end-to-end forest tests never reach, each called through the C ABI and compared exactly with the CPU oracle or numpy.
 
 exclusive scan: the single-CTA kernel (n <= 16 * 4096) and the three-launch path, including the totals kernel's loop over
 1024-block chunks (n > 1024 * 4096), with block sums near 2^31 and grand totals past 2^32.  group_rows: ids colliding in
@@ -10,25 +9,16 @@ bootstrap; bag_count / bag_fill with U not a multiple of 1024.  The Philox draw 
 threshold of the CDF head: pinned rows where it occurs.  dedup_rows: load exactly 0.5, strides 16 to 256, key_bytes = F
 and F + 1.  bin_rows: thresholds in global memory, the strided-feature path (F > 256), ld > F, NaN, +-inf, +-0 and values on
 a threshold.  find_splits: the 16384 / 16385 switch between the shared- and global-memory kernels, possible == numSplits,
-one and two samples, +-inf.  predict: top tables of 1 to 10 levels or none, stumps and trees deeper than the table, blocks
-shrunk below 128 threads by many classes, both vote modes, and the 4-rows-per-thread kernel."""
-import os
-import subprocess
-import sys
-
+one and two samples, +-inf.  (The batch predictor's cases are in test_predict_forest.py.)"""
 import numpy as np
 import pytest
 import torch
 
 import oracle
 from b200flow import _lib, forest as fr, gbt
-from b200flow._lib import NODE_DTYPE, B200FlowError, call, ptr
+from b200flow._lib import call, ptr
 
 DEV = "cuda"
-TESTS = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(TESTS)
-PKG = os.path.join(ROOT, "spark-network-traffic-classifier_b200")
-
 SAT = 0xFFFFFFFF
 
 
@@ -446,179 +436,3 @@ def test_find_splits(n_s, mb, count_on_device):
         assert np.array_equal(got_thr[f, : want.size].view(np.uint64), want.view(np.uint64)), f   # bit for bit
     if n_s >= mb:
         assert got_n[1] == mb - 1                                             # possible == numSplits: every midpoint
-
-
-# ------------------------------------------------------------------------------- predict
-PRED_F = 41
-PRED_T = 7
-PRED_DEPTHS = [0, 1, 3, 9, 12, 0, 14]          # stumps, trees within the top table, and deeper than 8 and 10 levels
-PRED_K = [None, 1, 3, 8, 10]
-PRED_C = [2, 23, 64, 180]
-
-
-def _make_pool(C, seed):
-    """a random forest pool in the layout of b200flow_node: roots 0..T-1, children appended in pairs (left, left + 1), node
-    ids heap-numbered; continuous splits on bins, and categorical ones (kind 1) on a left-set mask."""
-    rng = np.random.default_rng(seed)
-    feat, kb, left, nid, tree = [], [], [], [], []
-    for t in range(PRED_T):
-        feat.append(-1); kb.append(0); left.append(-1); nid.append(1); tree.append(t)
-    queue = [(t, 0, PRED_DEPTHS[t], True) for t in range(PRED_T)]           # (node, depth, tree depth, on the spine)
-    while queue:
-        nxt = []
-        for i, d, D, spine in queue:
-            if d >= D or not (spine or rng.random() < 0.7):
-                continue
-            li = len(feat)
-            feat[i] = int(rng.integers(0, PRED_F))
-            kb[i] = (65536 | int(rng.integers(0, 32))) if rng.random() < 0.3 else int(rng.integers(0, 32))
-            left[i] = li
-            for s in (0, 1):
-                feat.append(-1); kb.append(0); left.append(-1); nid.append(2 * nid[i] + s); tree.append(tree[i])
-            go = int(rng.integers(0, 2))
-            nxt += [(li, d + 1, D, spine and go == 0), (li + 1, d + 1, D, spine and go == 1)]
-        queue = nxt
-    P = len(feat)
-    nodes = np.zeros(P, NODE_DTYPE)
-    nodes["feat"], nodes["kind_bin"], nodes["left"], nodes["nid"] = feat, kb, left, nid
-    mask = rng.integers(0, 2 ** 63, (P, 4), dtype=np.int64).view(np.uint64)
-    leaf_prob = rng.random((P, C))
-    counts = rng.integers(0, 5000, (P, C)).astype(np.uint32)
-    return nodes, mask, leaf_prob, counts, np.asarray(tree, np.int32)
-
-
-def _pred_rows(n, seed):
-    rng = np.random.default_rng(seed)
-    tp = np.zeros((n, fr.tp_stride(PRED_F)), np.uint8)
-    tp[:, :PRED_F] = rng.integers(0, 40, (n, PRED_F))
-    tp[:, :8] = rng.integers(0, 256, (n, 8))                                  # bins in every word of a categorical mask
-    return tp
-
-
-def _walk(tp, nodes, mask, payload, T):
-    """votes of every row: payload of its leaf in each tree, added in tree order from 0.0 as the kernel does"""
-    n = tp.shape[0]
-    feat, kb, left = nodes["feat"].astype(np.int64), nodes["kind_bin"].astype(np.int64), nodes["left"].astype(np.int64)
-    votes = np.zeros((n, payload.shape[1]))
-    rows = np.arange(n)
-    for t in range(T):
-        idx = np.full(n, t, np.int64)
-        act = rows[feat[idx] >= 0]
-        while act.size:
-            nd = idx[act]
-            b = tp[act, feat[nd]].astype(np.int64)
-            cont = kb[nd] < 65536
-            bit = (mask[nd, b >> 6] >> (b & 63).astype(np.uint64)) & np.uint64(1)
-            right = np.where(cont, b > kb[nd], bit == 0).astype(np.int64)
-            idx[act] = left[nd] + right
-            act = act[feat[idx[act]] >= 0]
-        votes += payload[idx]
-    return votes
-
-
-def _want_predict(votes):
-    s = np.zeros(votes.shape[0])
-    for k in range(votes.shape[1]):                                           # sequential, class order
-        s = s + votes[:, k]
-    with np.errstate(invalid="ignore", divide="ignore"):
-        prob = np.where(s[:, None] != 0, votes / s[:, None], 0.0)
-    return votes, prob, np.argmax(votes, 1).astype(np.float64)              # first maximum
-
-
-def _pred_smem(C, K, rows):
-    """dynamic shared memory of predict_kernel, or None when b200flow_predict refuses it (restates csrc/predict.cu)"""
-    per_thread = (fr.tp_stride(PRED_F) + C * 8) * rows
-    bd = 128
-    while bd > 32 and per_thread * bd > 96 * 1024:
-        bd >>= 1
-    smem = per_thread * bd + (2 * 16 * (1 << K) if K else 0)
-    return smem if smem <= 200 * 1024 else None
-
-
-def _predict_cases():
-    """(name, C, K, dt_mode, n); n is never a multiple of a block's rows.  C = 2 with 600 001 rows loops the grid."""
-    out = []
-    for C in PRED_C + [250]:
-        for K in PRED_K if C != 250 else [None]:
-            for dt in (0, 1):
-                out.append(("C%d_K%s_dt%d" % (C, K, dt), C, K, dt, 1037 if C != 2 else 600_001))
-    return out
-
-
-def _run_predict(C, K, dt, n):
-    nodes, mask, leaf_prob, counts, tree = _make_pool(C, C)
-    tp = _dev(_pred_rows(n, C + n))
-    nodes_d = _dev(nodes.view(np.uint8).reshape(-1, 16))
-    top = None
-    if K:
-        top = torch.zeros((PRED_T << K, 4), dtype=torch.int32, device=DEV)
-        tree_d = _dev(tree)
-        call("b200flow_build_top_nodes", ptr(nodes_d), ptr(tree_d), nodes.shape[0], PRED_T, K, ptr(top))
-    raw = torch.empty((n, C), dtype=torch.float64, device=DEV); prob = torch.empty_like(raw)
-    pred = torch.empty(n, dtype=torch.float64, device=DEV)
-    mask_d, prob_d, counts_d = _dev(mask.view(np.int64)), _dev(leaf_prob), _dev(counts.view(np.int32))
-    call("b200flow_predict", ptr(tp), tp.shape[1], n, ptr(nodes_d), ptr(mask_d), ptr(prob_d), ptr(counts_d), PRED_T, C, dt,
-         ptr(top), K or 0, ptr(raw), ptr(prob), ptr(pred))
-    return raw.cpu().numpy(), prob.cpu().numpy(), pred.cpu().numpy()
-
-
-def _check_predict(got, C, K, dt, n):
-    nodes, mask, leaf_prob, counts, _ = _make_pool(C, C)
-    tp = _pred_rows(n, C + n)
-    votes = _walk(tp, nodes, mask, counts.astype(np.float64) if dt else leaf_prob, PRED_T)
-    for g, w, what in zip(got, _want_predict(votes), ("raw", "prob", "pred")):
-        assert np.array_equal(g.view(np.uint64), w.view(np.uint64)), (C, K, dt, what)
-
-
-def test_predict_pool_shapes():
-    # the fixture forests: every tree reaches its depth (a spine), so K = 8 and 10 tables hold only part of the deep trees
-    nodes, _, _, _, tree = _make_pool(23, 23)
-    depth = np.floor(np.log2(nodes["nid"].astype(np.float64))).astype(int)
-    assert [int(depth[tree == t].max()) for t in range(PRED_T)] == PRED_DEPTHS
-    assert _pred_smem(180, 8, 2) and _pred_smem(180, 10, 2) and _pred_smem(250, None, 2)
-    assert _pred_smem(180, 8, 4) and _pred_smem(180, 10, 4) is None and _pred_smem(250, None, 4) is None
-
-
-@pytest.mark.gpu
-@pytest.mark.parametrize("C", PRED_C + [250])
-def test_predict_against_walk(C):
-    for name, c, K, dt, n in _predict_cases():
-        if c == C:
-            _check_predict(_run_predict(c, K, dt, n), c, K, dt, n)
-
-
-_PRED4_CHILD = r"""
-import sys
-sys.path[:0] = [%r, %r, %r]
-import numpy as np, torch
-import test_treeprep_edges as t
-from b200flow._lib import B200FlowError
-res = {}
-for name, C, K, dt, n in t._predict_cases():
-    try:
-        raw, prob, pred = t._run_predict(C, K, dt, n)
-        res[name + "/raw"], res[name + "/prob"], res[name + "/pred"] = raw, prob, pred
-    except B200FlowError as e:
-        res[name + "/refused"] = np.array(str(e))
-torch.cuda.synchronize()
-np.savez(sys.argv[1], **res)
-"""
-
-
-@pytest.mark.gpu
-def test_predict_four_rows_per_thread(tmp_path):
-    # B200FLOW_PRED_ROWS is read once per process (a static in b200flow_predict), so the 4-row kernel runs in a child
-    env = dict(os.environ, B200FLOW_PRED_ROWS="4")
-    dst = str(tmp_path / "pred4.npz")
-    subprocess.run([sys.executable, "-c", _PRED4_CHILD % (ROOT, PKG, TESTS), dst], env=env, timeout=900, check=True)
-    got = np.load(dst)
-    for name, C, K, dt, n in _predict_cases():
-        if _pred_smem(C, K, 4) is None:               # too many classes for shared memory: a clean refusal, not a crash
-            assert "shared memory" in str(got[name + "/refused"]), name
-            continue
-        four = tuple(got[name + "/" + k] for k in ("raw", "prob", "pred"))
-        two = _run_predict(C, K, dt, n)
-        for a, b in zip(four, two):
-            assert np.array_equal(a.view(np.uint64), b.view(np.uint64)), name
-        if C != 2:
-            _check_predict(four, C, K, dt, n)
