@@ -16,7 +16,7 @@
 namespace b200flow {
 
 constexpr int kCsvWarps = 8;
-constexpr int kCsvRowCap = 4096;          // longest row (bytes) the tokenizer stages
+constexpr int kCsvRowCap = 4096;          // longest row (bytes before its '\n', a CRLF's '\r' included) the tokenizer stages
 constexpr int kCsvMaxCols = 1024;
 constexpr int kIdxThreads = 256;          // 256 threads x 16 bytes = one 4 KB block of text per CTA
 
@@ -143,10 +143,11 @@ __global__ void __launch_bounds__(kCsvWarps * 32) csv_rows_kernel(const CsvArgs 
         int nf = 0, len = 0;
         bool done = false;
         if (lane == 0) fs[0] = 0;
-        for (int base = 0; base < kCsvRowCap && !done; base += 32) {
+        for (int base = 0; base <= kCsvRowCap && !done; base += 32) {
             const int64_t p = s + base + lane;
             const uint8_t c = p < a.n_bytes ? __ldg(a.text + p) : (uint8_t)'\n';
             const uint32_t nl = __ballot_sync(0xffffffffu, c == '\n');
+            if (base == kCsvRowCap && !(nl & 1u)) break;         // a row of exactly kCsvRowCap bytes: only its '\n' is read here
             const int upto = nl ? __ffs(nl) - 1 : 32;
             const bool valid = lane < upto;
             if (valid) buf[base + lane] = c;
@@ -226,8 +227,9 @@ static size_t csv_rows_smem(int mode, int n_cols) {
 template <int MODE>
 static int csv_rows_launch(const CsvArgs& a, cudaStream_t stream, const char* what) {
     const size_t smem = csv_rows_smem(MODE, a.n_cols);
-    static bool attr_done = false;                              // per instantiation
-    if (!attr_done) { cudaFuncSetAttribute(csv_rows_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024); attr_done = true; }
+    // the limit belongs to the current device: set it on every launch, or a second GPU of the process could not run wide files
+    const cudaError_t e = cudaFuncSetAttribute(csv_rows_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) { cudaGetLastError(); set_error("%s: cudaFuncSetAttribute: %s", what, cudaGetErrorString(e)); return B200FLOW_ERR_CUDA; }
     const int64_t want = (a.n_rows + kCsvWarps - 1) / kCsvWarps;
     const int grid = (int)(want < (int64_t)kNumSMs * 4 ? want : (int64_t)kNumSMs * 4);
     csv_rows_kernel<MODE><<<grid, kCsvWarps * 32, smem, stream>>>(a);

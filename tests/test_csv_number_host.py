@@ -2,37 +2,17 @@
 against Python's own correctly rounded float() / int() — the same semantics as Java's Double.parseDouble / Integer.parseInt that
 Spark's CSV reader applies (kdd99.py:25, cicids17.py:19-20).  No GPU needed: the header is `__host__ __device__`."""
 import ctypes as C
-import os
-import struct
-import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-NULL, INT, LONG, DOUBLE, STRING = range(5)
-OK, NOT_A_NUMBER, UNSUPPORTED = range(3)
+from csv_corpus import (DOUBLE, INT, LONG, NOT_A_NUMBER, NULL, OK, STRING, UNSUPPORTED, build_host_lib, grammar_literals, long_literals,
+                        midpoint_literals, run, writer_literals)
 
 
 @pytest.fixture(scope="module")
 def lib(tmp_path_factory):
-    out = str(tmp_path_factory.mktemp("csvnum") / "libcsvnum.so")
-    subprocess.check_call(["g++", "-O2", "-shared", "-fPIC", "-std=c++17", "-I", os.path.join(ROOT, "spark-network-traffic-classifier_b200", "csrc"),
-                           os.path.join(ROOT, "tests", "native", "csv_number_host.cpp"), "-o", out])
-    return C.CDLL(out)
-
-
-def run(lib, fields):
-    raw = [f if isinstance(f, bytes) else f.encode() for f in fields]
-    offs = np.zeros(len(raw) + 1, np.int64)
-    np.cumsum([len(r) for r in raw], out=offs[1:])
-    blob = np.frombuffer(b"".join(raw) + b"\0", np.uint8)
-    n = len(raw)
-    cls, st, sti, iv = (np.zeros(n, np.int32) for _ in range(4))
-    val = np.zeros(n, np.float64)
-    lib.csvnum_batch(C.c_void_p(blob.ctypes.data), C.c_void_p(offs.ctypes.data), C.c_int64(n), C.c_void_p(cls.ctypes.data), C.c_void_p(st.ctypes.data),
-                     C.c_void_p(val.ctypes.data), C.c_void_p(sti.ctypes.data), C.c_void_p(iv.ctypes.data))
-    return cls, st, val, sti, iv
+    return build_host_lib(tmp_path_factory.mktemp("csvnum"))
 
 
 def bits(a):
@@ -52,32 +32,7 @@ def test_classification_follows_spark_inference(lib):
 
 
 def test_doubles_are_correctly_rounded_fast_path_and_128_bit_path(lib):
-    rng = np.random.default_rng(7)
-    fields = []
-    # the literals a CSV writer produces: repr (shortest round-trip, up to 17 digits), %.6f, %.17g, %e — over many magnitudes
-    mags = 10.0 ** rng.uniform(-9, 15, 150000)
-    vals = rng.standard_normal(150000) * mags
-    for v in vals[:50000]:
-        fields.append(repr(float(v)))
-    for v in vals[50000:90000]:
-        fields.append("%.6f" % v)
-    for v in vals[90000:120000]:
-        fields.append("%.17g" % v)
-    for v in vals[120000:150000]:
-        fields.append("%.10e" % v)
-    # hard cases: 16-19 digit mantissas (beyond 2^53) with small exponents, halfway patterns
-    for _ in range(60000):
-        nd = int(rng.integers(16, 20))
-        w = int(rng.integers(10 ** (nd - 1), 10 ** nd, dtype=np.uint64))
-        q = int(rng.integers(-27 + 0, 9))
-        s = str(w)
-        k = int(rng.integers(0, nd))
-        fields.append((s[:k] or "0") + "." + s[k:] + ("e%d" % (q + (nd - k))) if rng.random() < 0.5 else s + "e%d" % q)
-    for e in range(-300, 300, 7):                                        # exact binary halfway points written in decimal
-        x = float(2 ** 53 + 1)                                             # not representable: ties
-        fields.append(str(2 ** 53 + 1)); fields.append(str(2 ** 54 + 2)); fields.append(str(2 ** 53 + 3))
-    fields += ["0.1", "0.30000000000000004", "9007199254740993", "9007199254740992.5", "4.35", "0.000001", "123456789012345678",
-               "1.7976931348623157e27", "5e-27", "0.00", "1.00", "0.05", "-0.0", "0e999", "000.000"]
+    fields = writer_literals(np.random.default_rng(7))
     cls, st, val, _, _ = run(lib, fields)
     want = np.array([float(f) for f in fields])
     assert (cls[st == OK] != STRING).all()
@@ -87,13 +42,7 @@ def test_doubles_are_correctly_rounded_fast_path_and_128_bit_path(lib):
 
 
 def test_more_than_19_digits_exact_or_reported(lib):
-    rng = np.random.default_rng(9)
-    fields = []
-    for _ in range(40000):
-        nd = int(rng.integers(20, 40))
-        s = "".join(str(d) for d in rng.integers(0, 10, nd))
-        k = int(rng.integers(1, 12))
-        fields.append(s[:k] + "." + s[k:])
+    fields = long_literals(np.random.default_rng(9))
     fields += ["0.1000000000000000055511151231257827021181583404541015625",        # 0.1's exact binary expansion
                "9007199254740993.0000000000000000000001", "9007199254740993.00000000000000000000", "1" + "0" * 25, "0." + "0" * 30 + "1"]
     cls, st, val, _, _ = run(lib, fields)
@@ -140,8 +89,7 @@ def test_python_restatement_agrees_with_the_product_grammar(lib, tmp_path):
     the independent pin for the column types and values of a plain file."""
     from oracle import csv_ref
     rng = np.random.default_rng(11)
-    alphabet = list("0123456789") * 3 + list("+-.eE ") + list("aNIfnity\t")
-    fields = ["".join(rng.choice(alphabet, size=int(rng.integers(0, 9)))) for _ in range(200000)]
+    fields = grammar_literals(rng)
     fields += ["", "NaN", "Infinity", "-Infinity", "+Infinity", "Inf", "-Inf", "+Inf", " 12", "12 ", "1e5", "0x10", "1_000", "١٢", "1d", "1f", "٣.٥"]
     cls, st, val, sti, iv = run(lib, fields)
     raw = [f.encode() for f in fields]
@@ -167,22 +115,7 @@ def test_python_restatement_agrees_with_the_product_grammar(lib, tmp_path):
 def test_literals_next_to_rounding_boundaries(lib):
     """The hardest inputs for a decimal -> double converter are literals a hair above or below the midpoint of two adjacent
     doubles.  Built exactly with decimal arithmetic: midpoint, then cut or bumped at the 17th..19th significant digit."""
-    import decimal
-    import math
-    decimal.getcontext().prec = 60
-    rng = np.random.default_rng(21)
-    fields = []
-    for _ in range(30000):
-        d = float(rng.uniform(1, 10)) * 10.0 ** int(rng.integers(-8, 12))
-        mid = (decimal.Decimal(d) + decimal.Decimal(math.nextafter(d, math.inf))) / 2     # exact
-        digits = int(rng.integers(17, 20))
-        q = decimal.Decimal(1).scaleb(mid.adjusted() - digits + 1)
-        lo = mid.quantize(q, rounding=decimal.ROUND_FLOOR)
-        for v in (lo, lo + q):
-            s = format(v, "f") if rng.random() < 0.5 else format(v, "e")
-            fields.append(s)
-        if digits == 19 and rng.random() < 0.2:
-            fields.append(format(mid, "f"))                                              # the exact tie: > 19 digits, exact or refused
+    fields = midpoint_literals(np.random.default_rng(21))
     cls, st, val, _, _ = run(lib, fields)
     want = np.array([float(f) for f in fields])
     ok = st == OK
