@@ -447,6 +447,25 @@ int b200flow_kmeans_select(uint64_t seed, int64_t row_offset, int64_t n_rows, in
  * when the row's cluster has one member. */
 int b200flow_silhouette_rows(const double* x, int64_t n_rows, int32_t D, int64_t ld, const double* norms, const int32_t* cluster,
                              const double* Y, const double* psi, const int64_t* N, int32_t G, double* out, void* stream);
+/* BisectingKMeans, DESIGN.md §5t.  Distances as b200flow_kmeans_assign's; no cross-row reduction, so each row's outputs
+ * depend on that row and the centers alone.
+ * b200flow_bkm_assign: rows carry a dense node number node[i]; slot_of_node [num_nodes] gives the dividing slot s of a node
+ * (-1: not dividing).  centers [2m][D] are the children of the m slots (slot s: 2s left, 2s+1 right), present uint8 [2m].
+ * child[i] = 2s or 2s+1, the present child with the smaller squared distance (strict <: a tie goes left), or -1 when the
+ * row's node is not dividing or neither child is present.  prev (optional, int32 [n_rows], -1 or a child index of the row's
+ * slot): dist_prev[i] = the squared distance to centers[prev[i]] (0.0 where prev[i] or the row's slot is -1), the cost of
+ * the previous assignment against the centers recomputed from it. */
+int b200flow_bkm_assign(const double* x, int64_t n_rows, int32_t D, int64_t ld, const int32_t* node, int32_t num_nodes,
+                        const int32_t* slot_of_node, const double* centers, int32_t m, const uint8_t* present, const int32_t* prev,
+                        int32_t* child, double* dist_prev, void* stream);
+/* b200flow_bkm_predict: the cluster tree as node arrays left, right [num_nodes] (-1: absent), leaf [num_nodes] (the leaf
+ * ordinal, -1 for an internal node) and centers [num_nodes][D], num_nodes <= 4095, depth <= 63.  From root, each internal
+ * node sends the row to the existing child with the smaller squared distance (a tie goes to the first, left, child).
+ * out_leaf[i] = the leaf ordinal reached, out_dist[i] = the squared distance to that leaf's center (a root that is a leaf
+ * works). */
+int b200flow_bkm_predict(const double* x, int64_t n_rows, int32_t D, int64_t ld, const int32_t* left, const int32_t* right,
+                         const int32_t* leaf, const double* centers, int32_t num_nodes, int32_t root, int32_t* out_leaf,
+                         double* out_dist, void* stream);
 
 /* ---------------------------------------------------------- neural network ---
  * MultilayerPerceptronClassifier, DESIGN.md §5d.  layers (host int32 [n_layers]) = [D, h_1, ..., h_k, K]: affine +

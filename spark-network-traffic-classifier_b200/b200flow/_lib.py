@@ -80,6 +80,8 @@ _SIGNATURES = {
     "b200flow_kmeans_row_keys": [_U64, _I64, _I64, _P, _P],
     "b200flow_kmeans_select": [_U64, _I64, _I64, _I32, _P, _I32, _F64, _P, _P],
     "b200flow_silhouette_rows": [_P, _I64, _I32, _I64, _P, _P, _P, _P, _P, _I32, _P, _P],
+    "b200flow_bkm_assign": [_P, _I64, _I32, _I64, _P, _I32, _P, _P, _I32, _P, _P, _P, _P, _P],
+    "b200flow_bkm_predict": [_P, _I64, _I32, _I64, _P, _P, _P, _P, _I32, _I32, _P, _P, _P],
     "b200flow_mlp_loss_grad": [_P, _I32, _I64, _I64, _P, _P, _I32, _P, _I64, _P, _P],
     "b200flow_mlp_forward": [_P, _I32, _I64, _I64, _P, _I32, _P, _P, _P],
     "b200flow_svc_loss_grad": [_P, _I32, _I64, _I64, _I32, _P, _P, _I64, _P, _P, _I64, _P, _P],

@@ -1,12 +1,16 @@
-"""pyspark.ml.clustering shim: KMeans / KMeansModel on the b200flow k-means kernels (b200flow/kmeans.py, DESIGN.md §5c) and
-GaussianMixture / GaussianMixtureModel on the EM kernels (b200flow/gmm.py, DESIGN.md §5g).
+"""pyspark.ml.clustering shim: KMeans / KMeansModel on the b200flow k-means kernels (b200flow/kmeans.py, DESIGN.md §5c),
+BisectingKMeans / BisectingKMeansModel on the split-assign and tree-walk kernels (b200flow/bisecting_kmeans.py, DESIGN.md
+§5t) and GaussianMixture / GaussianMixtureModel on the EM kernels (b200flow/gmm.py, DESIGN.md §5g).
 
-The models are the same bits for any number of ranks.  Deviations from Spark: KMeans distances are exact (no
-fastSquaredDistance bound), the random draws are this project's Philox streams, distanceMeasure="cosine" and weightCol are
-refused; GaussianMixture's deviations are listed in b200flow/gmm.py."""
+The models are the same bits for any number of ranks.  Deviations from Spark: KMeans and BisectingKMeans distances are
+exact (no fastSquaredDistance bound), the random draws are this project's Philox streams, distanceMeasure="cosine" and
+weightCol are refused; BisectingKMeans' cluster costs are exact two-pass sums, children are compared on squared distances
+and equally large divisible clusters are chosen by heap index (b200flow/bisecting_kmeans.py); GaussianMixture's
+deviations are listed in b200flow/gmm.py."""
 import numpy as np
 import torch
 
+from b200flow import bisecting_kmeans as _bkm
 from b200flow import dist as bdist
 from b200flow import gmm as _gm
 from b200flow import kmeans as _km
@@ -118,6 +122,124 @@ class KMeansSummary:
         self.clusterSizes = [int(v) for v in np.asarray(res.cluster_sizes)]
         self.trainingCost = float(res.training_cost)
         self.numIter = int(res.num_iter)
+
+    @property
+    def cluster(self):
+        return self.predictions.select(self.predictionCol)
+
+
+class _BisectingKMeansParams:
+    _defaults = {"featuresCol": "features", "predictionCol": "prediction", "k": 4, "maxIter": 20, "seed": None,
+                 "minDivisibleClusterSize": 1.0, "distanceMeasure": "euclidean", "weightCol": None}
+
+
+class BisectingKMeans(Estimator, _BisectingKMeansParams):
+    """Spark 3's BisectingKMeans (DESIGN.md §5t).  maxIter = 0, which Spark's validator accepts but its fit cannot run, is
+    refused here; so are distanceMeasure="cosine", weightCol, more than 256 features and k > 2048."""
+
+    def __init__(self, featuresCol=None, predictionCol=None, maxIter=None, seed=None, k=None, minDivisibleClusterSize=None,
+                 distanceMeasure=None, weightCol=None):
+        kw = dict(locals()); kw.pop("self"); kw.pop("__class__", None)
+        super().__init__(**kw)
+
+    def _check(self):
+        """Spark's param validators, and the refusals of this implementation."""
+        g = self.getOrDefault
+        k, it, mdcs = g("k"), g("maxIter"), g("minDivisibleClusterSize")
+        if int(k) != k or int(k) <= 1:
+            raise IllegalArgumentException("BisectingKMeans parameter k given invalid value %r: it must be an integer > 1"
+                                           % (k,))
+        if int(it) != it or int(it) < 1:
+            raise IllegalArgumentException("maxIter must be an integer >= 1 for BisectingKMeans, got %r" % (it,))
+        if not float(mdcs) > 0.0:
+            raise IllegalArgumentException("minDivisibleClusterSize must be > 0, got %r" % (mdcs,))
+        dm = g("distanceMeasure")
+        if dm == "cosine":
+            raise IllegalArgumentException("distanceMeasure='cosine' is not supported by the b200flow BisectingKMeans (out of "
+                                           "scope); use 'euclidean'")
+        if dm != "euclidean":
+            raise IllegalArgumentException("distanceMeasure must be 'euclidean' or 'cosine', got %r" % (dm,))
+        if g("weightCol"):
+            raise IllegalArgumentException("weightCol is not supported by the b200flow BisectingKMeans (out of scope)")
+
+    def _fit(self, df):
+        self._check()
+        g = self.getOrDefault
+        x = _features(df, g("featuresCol"))
+        seed = _default_seed(self) if g("seed") is None else int(g("seed"))
+        try:
+            res = _bkm.bkm_fit(x, int(g("k")), max_iter=int(g("maxIter")), min_divisible=float(g("minDivisibleClusterSize")),
+                               seed=seed, group=bdist.group())
+        except ValueError as e:        # includes b200flow's UnsupportedParamError
+            raise IllegalArgumentException(str(e))
+        m = BisectingKMeansModel(res.tree, res.training_cost)
+        m._paramMap = {k: v for k, v in self._paramMap.items() if k in m._all_defaults()}
+        m._summary = BisectingKMeansSummary(m._with_prediction(df, res.leaf), res, int(g("k")), int(g("maxIter")),
+                                            g("featuresCol"), g("predictionCol"))
+        return m
+
+
+class BisectingKMeansModel(Model, _BisectingKMeansParams):
+    def __init__(self, tree, training_cost):
+        super().__init__()
+        self._tree = tree                  # b200flow.bisecting_kmeans.Tree
+        self._training_cost = float(training_cost)
+        self._summary = None
+
+    def clusterCenters(self):
+        return [r.copy() for r in self._tree.center[self._tree.leaf_nodes()]]
+
+    @property
+    def trainingCost(self):
+        return self._training_cost
+
+    @property
+    def hasSummary(self):
+        return self._summary is not None
+
+    @property
+    def summary(self):
+        if self._summary is None:
+            raise RuntimeError("No training summary available for this BisectingKMeansModel")
+        return self._summary
+
+    def _check_width(self, x):
+        if x.shape[1] != self._tree.center.shape[1]:
+            raise IllegalArgumentException("the model has %d features, the data %d" % (self._tree.center.shape[1], x.shape[1]))
+        return x
+
+    def predict(self, features):
+        """the leaf index of one feature vector, the walk transform takes"""
+        v = np.asarray(features.toArray() if hasattr(features, "toArray") else features, np.float64).reshape(1, -1)
+        leaf, _ = _bkm.bkm_predict(self._check_width(torch.from_numpy(v).cuda()), self._tree)
+        return int(leaf[0].item())
+
+    def computeCost(self, dataset):
+        """the sum of squared distances of the rows to the leaf centers they reach (deprecated in Spark 3, still there)"""
+        x = self._check_width(_features(dataset, self.getOrDefault("featuresCol")))
+        return _bkm.compute_cost(x, self._tree, group=bdist.group())
+
+    def _with_prediction(self, df, leaf):
+        name = self.getOrDefault("predictionCol")
+        if name in df._cols:
+            raise IllegalArgumentException("Output column %s already exists." % name)
+        cols = dict(df._cols)
+        cols[name] = ColumnData("numeric", leaf.to(torch.int32).contiguous(), "i32")
+        return df._with(cols=cols)
+
+    def _transform(self, df):
+        x = self._check_width(_features(df, self.getOrDefault("featuresCol")))
+        leaf, _ = _bkm.bkm_predict(x, self._tree)
+        return self._with_prediction(df, leaf)
+
+
+class BisectingKMeansSummary:
+    def __init__(self, predictions, res, k, max_iter, featuresCol, predictionCol):
+        self.predictions, self.featuresCol, self.predictionCol = predictions, featuresCol, predictionCol
+        self.k = k
+        self.clusterSizes = [int(v) for v in _bkm.cluster_sizes(res.leaf, k)]
+        self.trainingCost = float(res.training_cost)
+        self.numIter = max_iter
 
     @property
     def cluster(self):
