@@ -1,13 +1,4 @@
-"""Helpers shared by the preprocessing tests (tests/test_feature_scaling_gpu.py, tests/test_feature_scaling_two_ranks.py)."""
-import socket
-
-
-def free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
+"""Helpers for the preprocessing tests (tests/test_feature_scaling_gpu.py)."""
 
 
 def kdd_frame(n, C, seed):

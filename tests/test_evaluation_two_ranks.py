@@ -2,16 +2,11 @@
 shard to distinct (score, pos, neg) triples, the triples are all-gathered and reduced again, so the areas and the curve
 points equal the single-process result bit for bit — also when one rank holds no rows.  A CrossValidator scored by
 areaUnderROC gives the same avgMetrics as one process."""
-import json
-import os
-import time
-import traceback
-
 import numpy as np
 import pytest
 import torch
 
-from test_tuning_two_ranks import _free_port
+from ranks import block, run
 
 pytestmark = pytest.mark.gpu
 
@@ -61,58 +56,27 @@ def _cv(rec, dicts):
                                                  seed=2019).fit(df).avgMetrics]
 
 
-def _worker(rank, world, port, out_dir):
-    import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    torch.cuda.set_device(0)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
-    try:
-        sc, y = _data()
-        res = {}
-        for name, cut in SPLITS.items():
-            lo, hi = (0, cut) if rank == 0 else (cut, N)
-            res[name] = _areas(sc[:, lo:hi], y[lo:hi])
-        from b200flow import synth
-        rec, dicts = synth.make_kdd(N, 2, seed=17, device="cuda:0")
-        lo, hi = (0, 13000) if rank == 0 else (13000, N)
-        res["cv"] = _cv(rec[lo:hi].contiguous(), dicts)
-        open(os.path.join(out_dir, "res%d.json" % rank), "w").write(json.dumps(res))
-    except Exception:
-        open(os.path.join(out_dir, "error%d.txt" % rank), "w").write(traceback.format_exc())
-        raise
-    finally:
-        try:
-            dist.destroy_process_group()
-        except Exception:
-            pass
+def _ranks(rank, grp, dev):
+    sc, y = _data()
+    res = {}
+    for name, cut in SPLITS.items():
+        lo, hi = block(rank, cut, N)
+        res[name] = _areas(sc[:, lo:hi], y[lo:hi])
+    from b200flow import synth
+    rec, dicts = synth.make_kdd(N, 2, seed=17, device="cuda:0")
+    lo, hi = block(rank, 13000, N)
+    res["cv"] = _cv(rec[lo:hi].contiguous(), dicts)
+    return res
 
 
 def test_binary_evaluation_two_ranks_equals_single_process(tmp_path):
-    import torch.multiprocessing as mp
-    ctx = mp.start_processes(_worker, args=(2, _free_port(), str(tmp_path)), nprocs=2, join=False, start_method="spawn")
-    deadline = time.time() + 300
-    failed = None
-    try:
-        while not ctx.join(timeout=5):
-            if time.time() > deadline:
-                failed = "workers hung"
-                break
-    except Exception as e:
-        failed = "worker failed: %s" % e
-    if failed:
-        for pr in ctx.processes:
-            if pr.is_alive():
-                pr.kill()
-        errs = "\n".join("--- rank %d\n%s" % (r, open(tmp_path / ("error%d.txt" % r)).read()) for r in (0, 1)
-                         if (tmp_path / ("error%d.txt" % r)).exists())
-        pytest.fail("%s\n%s" % (failed, errs))
+    got = run(tmp_path, _ranks, timeout=300)
     sc, y = _data()
-    want = json.loads(json.dumps(_areas(sc, y)))
+    want = _areas(sc, y)
     from b200flow import synth
     rec, dicts = synth.make_kdd(N, 2, seed=17, device="cuda:0")
     cv = _cv(rec, dicts)
     for rank in (0, 1):
-        got = json.loads(open(tmp_path / ("res%d.json" % rank)).read())
         for name in SPLITS:
-            assert got[name] == want, (rank, name)
-        assert got["cv"] == cv, rank
+            assert got[rank][name] == want, (rank, name)
+        assert got[rank]["cv"] == cv, rank

@@ -2,16 +2,11 @@
 RobustScaler, MinMaxScaler, MaxAbsScaler, QuantileDiscretizer splits and approxQuantile equal the single-process run byte
 for byte for even and uneven shards and an empty first or last shard, and an all-missing column raises on both ranks.
 Two gloo ranks share one GPU; the NCCL case needs two GPUs and is skipped otherwise."""
-import json
-import os
-import time
-import traceback
-
 import numpy as np
 import pytest
 import torch
 
-from feature_helpers import free_port
+from ranks import block, run, two_gpus
 
 pytestmark = pytest.mark.gpu
 
@@ -62,61 +57,28 @@ def _run(m, dev):
     return out
 
 
-def _worker(rank, world, port, out_dir, backend):
-    import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    gpu = rank if backend == "nccl" else 0
-    torch.cuda.set_device(gpu)
-    kw = {"device_id": torch.device("cuda", gpu)} if backend == "nccl" else {}
-    dist.init_process_group(backend, rank=rank, world_size=world, **kw)
-    try:
-        m = _data()
-        res = {}
-        for name, cut in SPLITS.items():
-            lo, hi = (0, cut) if rank == 0 else (cut, N)
-            res[name] = _run(m[lo:hi], torch.device("cuda", gpu))
-        open(os.path.join(out_dir, "res%d.json" % rank), "w").write(json.dumps(res))
-    except Exception:
-        open(os.path.join(out_dir, "error%d.txt" % rank), "w").write(traceback.format_exc())
-        raise
-    finally:
-        try:
-            dist.destroy_process_group()
-        except Exception:
-            pass
+def _ranks(rank, grp, dev):
+    m = _data()
+    res = {}
+    for name, cut in SPLITS.items():
+        lo, hi = block(rank, cut, N)
+        res[name] = _run(m[lo:hi], dev)
+    return res
 
 
-def _two_ranks(tmp_path, backend):
-    import torch.multiprocessing as mp
-    ctx = mp.start_processes(_worker, args=(2, free_port(), str(tmp_path), backend), nprocs=2, join=False, start_method="spawn")
-    deadline = time.time() + 600
-    failed = None
-    try:
-        while not ctx.join(timeout=5):
-            if time.time() > deadline:
-                failed = "workers hung"
-                break
-    except Exception as e:
-        failed = "worker failed: %s" % e
-    if failed:
-        for pr in ctx.processes:
-            if pr.is_alive():
-                pr.kill()
-        errs = "\n".join("--- rank %d\n%s" % (r, open(tmp_path / ("error%d.txt" % r)).read()) for r in (0, 1)
-                         if (tmp_path / ("error%d.txt" % r)).exists())
-        pytest.fail("%s\n%s" % (failed, errs))
-    want = json.loads(json.dumps(_run(_data(), torch.device("cuda", 0))))
+def _two_ranks(tmp_path, mode):
+    got = run(tmp_path, _ranks, mode=mode)
+    want = _run(_data(), torch.device("cuda", 0))
     assert want["raised"] is True
     for rank in (0, 1):
-        got = json.loads(open(tmp_path / ("res%d.json" % rank)).read())
         for name in SPLITS:
-            assert got[name] == want, (rank, name)
+            assert got[rank][name] == want, (rank, name)
 
 
 def test_feature_scaling_two_gloo_ranks_equal_one_process(tmp_path):
     _two_ranks(tmp_path, "gloo")
 
 
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs two GPUs")
+@two_gpus
 def test_feature_scaling_two_nccl_ranks_equal_one_process(tmp_path):
     _two_ranks(tmp_path, "nccl")

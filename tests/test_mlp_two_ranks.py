@@ -3,22 +3,16 @@ straddling chunk by the rank holding its first row) and chained rank to rank, so
 and a whole fit's weights and objective history equal the single-process run byte for byte — for even and uneven
 shards, a shard shorter than one chunk and an empty shard.  Two gloo ranks share one GPU; the NCCL case needs two GPUs
 and is skipped otherwise."""
-import json
-import os
-import time
-import traceback
-
 import numpy as np
 import pytest
 import torch
 
-from test_tuning_two_ranks import _free_port
+from ranks import SPLITS, block, run, two_gpus
 
 pytestmark = pytest.mark.gpu
 
 N = 30000
 LAYERS = [41, 16, 5]
-SPLITS = {"even": 15000, "uneven": 11000, "short_first": 2500, "short_last": 28000, "empty_last": N, "empty_first": 0}
 
 
 def _data():
@@ -40,61 +34,28 @@ def _run(x, y, dev, grp):
             "hist": [v.hex() for v in fit.objective_history], "it": fit.iterations}
 
 
-def _worker(rank, world, port, out_dir, backend):
-    import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    gpu = rank if backend == "nccl" else 0
-    torch.cuda.set_device(gpu)
-    kw = {"device_id": torch.device("cuda", gpu)} if backend == "nccl" else {}
-    dist.init_process_group(backend, rank=rank, world_size=world, **kw)
-    try:
-        x, y = _data()
-        res = {}
-        for name, cut in SPLITS.items():
-            lo, hi = (0, cut) if rank == 0 else (cut, N)
-            res[name] = _run(x[lo:hi], y[lo:hi], torch.device("cuda", gpu), dist.group.WORLD)
-        open(os.path.join(out_dir, "res%d.json" % rank), "w").write(json.dumps(res))
-    except Exception:
-        open(os.path.join(out_dir, "error%d.txt" % rank), "w").write(traceback.format_exc())
-        raise
-    finally:
-        try:
-            dist.destroy_process_group()
-        except Exception:
-            pass
-
-
-def _two_ranks(tmp_path, backend):
-    import torch.multiprocessing as mp
-    ctx = mp.start_processes(_worker, args=(2, _free_port(), str(tmp_path), backend), nprocs=2, join=False, start_method="spawn")
-    deadline = time.time() + 600
-    failed = None
-    try:
-        while not ctx.join(timeout=5):
-            if time.time() > deadline:
-                failed = "workers hung"
-                break
-    except Exception as e:
-        failed = "worker failed: %s" % e
-    if failed:
-        for pr in ctx.processes:
-            if pr.is_alive():
-                pr.kill()
-        errs = "\n".join("--- rank %d\n%s" % (r, open(tmp_path / ("error%d.txt" % r)).read()) for r in (0, 1)
-                         if (tmp_path / ("error%d.txt" % r)).exists())
-        pytest.fail("%s\n%s" % (failed, errs))
+def _ranks(rank, grp, dev):
     x, y = _data()
-    want = json.loads(json.dumps(_run(x, y, torch.device("cuda", 0), None)))
+    res = {}
+    for name, cut in SPLITS(N).items():
+        lo, hi = block(rank, cut, N)
+        res[name] = _run(x[lo:hi], y[lo:hi], dev, grp)
+    return res
+
+
+def _two_ranks(tmp_path, mode):
+    got = run(tmp_path, _ranks, mode=mode)
+    x, y = _data()
+    want = _run(x, y, torch.device("cuda", 0), None)
     for rank in (0, 1):
-        got = json.loads(open(tmp_path / ("res%d.json" % rank)).read())
-        for name in SPLITS:
-            assert got[name] == want, (rank, name)
+        for name in SPLITS(N):
+            assert got[rank][name] == want, (rank, name)
 
 
 def test_mlp_two_gloo_ranks_equal_one_process(tmp_path):
     _two_ranks(tmp_path, "gloo")
 
 
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs two GPUs")
+@two_gpus
 def test_mlp_two_nccl_ranks_equal_one_process(tmp_path):
     _two_ranks(tmp_path, "nccl")

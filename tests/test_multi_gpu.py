@@ -1,107 +1,59 @@
 """Real multi-GPU check (needs >= 2 GPUs: `gpurun --gpus 2 -- python -m pytest tests/test_multi_gpu.py -m gpu`):
 rows sharded over 2 ranks + NCCL all-reduce of the level histograms must reproduce the 1-GPU forest byte for byte."""
-import os
-import socket
-
 import numpy as np
 import pytest
 import torch
 
+from ranks import block, run, two_gpus
+from util import kdd_luts_gpu, kdd_plan
+
 pytestmark = pytest.mark.gpu
 
 
-def _free_port():
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
-
-
-def _mark(out_dir, rank, what):
-    with open(os.path.join(out_dir, "progress%d.txt" % rank), "a") as f:
-        f.write(what + "\n")
-
-
-def _worker(rank, world, port, out_dir):
+def _ranks(rank, grp, dev):
     import torch.distributed as dist
-    from b200flow import dist as bdist, encode as enc, forest as fr, synth
-    import faulthandler
-    faulthandler.dump_traceback_later(150, exit=False, file=open(os.path.join(out_dir, "stack%d.txt" % rank), "w"))   # where a hang sits
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    torch.cuda.set_device(rank)
-    dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
-    try:
-        dev = torch.device("cuda", rank)
-        n = 60000
-        rec, dicts = synth.make_kdd(n, 5, seed=17, device=dev)              # identical global data in both ranks
-        schema = synth.kdd_schema()
-        lo, hi = bdist.shard_bounds(n, rank, world)
-        shard = rec[lo:hi].contiguous()
-        luts, ordered = {}, {}
-        for c in synth.KDD_CATEGORICAL + ["label"]:
-            cnt = bdist.all_reduce_sum_(enc.category_counts(shard, schema, c, len(dicts[c]))).cpu().numpy()
-            ordered[c], luts[c] = enc.string_index_order(cnt, dicts[c])
-        plan = enc.EncodePlan(schema)
-        for c in synth.KDD_COLUMNS:
-            if c not in synth.KDD_CATEGORICAL and c != "label":
-                plan.add_numeric(c)
-        for c in synth.KDD_CATEGORICAL:
-            plan.add_index(c, luts[c])
-        plan.set_label("label", luts["label"])
-        x, y, _ = plan.run(shard, torch.float64)
-        arity = [0] * 38 + [len(ordered[c]) for c in synth.KDD_CATEGORICAL]
-        C = len(ordered["label"])
-        p = fr.ForestParams(num_trees=8, max_bins=70, max_depth=10, seed=2019)
-        off, _ = bdist.global_offset(hi - lo, dev)
-        model = fr.fit_forest(x, y, C, arity, p, row_offset=off, group=bdist.group())
-        ex = model.export()
-        _mark(out_dir, rank, "all-reduce path done")
-        fr.RS_MIN_BYTES = 0            # every level through reduce-scatter -> sharded scoring -> all-gather of the split records
-        fr.RS_CHUNKS = 3               # ... in three pipelined slot ranges
-        ex_rs = fr.fit_forest(x, y, C, arity, p, row_offset=off, group=bdist.group()).export()
-        fr.RS_MIN_BYTES = 8 << 20
-        fr.RS_CHUNKS = 1
-        _mark(out_dir, rank, "reduce-scatter path done")
-        # uneven shards (21,000 / 39,000 rows: different findSplits sample capacities per rank) on the fused record path
-        cut = 21000
-        ulo, uhi = (0, cut) if rank == 0 else (cut, n)
-        ushard = rec[ulo:uhi].contiguous()
-        uoff, _ = bdist.global_offset(uhi - ulo, dev)
-        ex_uneven = fr.fit_forest_records(ushard, plan, C, arity, p, row_offset=uoff, group=bdist.group()).export()
-        _mark(out_dir, rank, "uneven shards done")
-        # one rank without any row: it still takes part in every collective
-        eshard = rec if rank == 0 else rec[:0].contiguous()
-        eoff, _ = bdist.global_offset(eshard.shape[0], dev)
-        ex_empty = fr.fit_forest_records(eshard, plan, C, arity, p, row_offset=eoff, group=bdist.group()).export()
-        _mark(out_dir, rank, "empty shard done")
-        if rank == 0:
-            np.savez(os.path.join(out_dir, "sharded.npz"), **ex)
-            np.savez(os.path.join(out_dir, "sharded_rs.npz"), **ex_rs)
-            np.savez(os.path.join(out_dir, "sharded_uneven.npz"), **ex_uneven)
-            np.savez(os.path.join(out_dir, "sharded_empty.npz"), **ex_empty)
-            xf, yf, _ = plan.run(rec, torch.float64)
-            single = fr.fit_forest(xf, yf, C, arity, p).export()
-            np.savez(os.path.join(out_dir, "single.npz"), **single)
-        dist.barrier()
-    finally:
-        dist.destroy_process_group()
+    from b200flow import dist as bdist, forest as fr, synth
+    n = 60000
+    rec, dicts = synth.make_kdd(n, 5, seed=17, device=dev)              # identical global data in both ranks
+    schema = synth.kdd_schema()
+    lo, hi = bdist.shard_bounds(n, rank, 2)
+    shard = rec[lo:hi].contiguous()
+    luts, ordered = kdd_luts_gpu(shard, schema, dicts, grp)
+    plan = kdd_plan(schema, luts, ordered)
+    x, y, _ = plan.run(shard, torch.float64)
+    arity = [0] * 38 + [len(ordered[c]) for c in synth.KDD_CATEGORICAL]
+    C = len(ordered["label"])
+    p = fr.ForestParams(num_trees=8, max_bins=70, max_depth=10, seed=2019)
+    off, _ = bdist.global_offset(hi - lo, dev)
+    model = fr.fit_forest(x, y, C, arity, p, row_offset=off, group=bdist.group())
+    ex = model.export()
+    fr.RS_MIN_BYTES = 0            # every level through reduce-scatter -> sharded scoring -> all-gather of the split records
+    fr.RS_CHUNKS = 3               # ... in three pipelined slot ranges
+    ex_rs = fr.fit_forest(x, y, C, arity, p, row_offset=off, group=bdist.group()).export()
+    fr.RS_MIN_BYTES = 8 << 20
+    fr.RS_CHUNKS = 1
+    # uneven shards (21,000 / 39,000 rows: different findSplits sample capacities per rank) on the fused record path
+    ulo, uhi = block(rank, 21000, n)
+    ushard = rec[ulo:uhi].contiguous()
+    uoff, _ = bdist.global_offset(uhi - ulo, dev)
+    ex_uneven = fr.fit_forest_records(ushard, plan, C, arity, p, row_offset=uoff, group=bdist.group()).export()
+    # one rank without any row: it still takes part in every collective
+    eshard = rec if rank == 0 else rec[:0].contiguous()
+    eoff, _ = bdist.global_offset(eshard.shape[0], dev)
+    ex_empty = fr.fit_forest_records(eshard, plan, C, arity, p, row_offset=eoff, group=bdist.group()).export()
+    single = None
+    if rank == 0:
+        xf, yf, _ = plan.run(rec, torch.float64)
+        single = fr.fit_forest(xf, yf, C, arity, p).export()
+    dist.barrier()
+    return ex, ex_rs, ex_uneven, ex_empty, single
 
 
-@pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs")
+@two_gpus
 def test_two_gpu_forest_is_byte_identical_to_one_gpu(tmp_path):
-    import time
-    import torch.multiprocessing as mp
-    ctx = mp.start_processes(_worker, args=(2, _free_port(), str(tmp_path)), nprocs=2, join=False, start_method="spawn")
-    deadline = time.time() + 200                      # a collective mismatch would hang for ever: bound it and say where
-    while not ctx.join(timeout=5):
-        if time.time() > deadline:
-            for pr in ctx.processes:
-                pr.kill()
-            prog = {r: (open(tmp_path / ("progress%d.txt" % r)).read().split("\n") if (tmp_path / ("progress%d.txt" % r)).exists() else []) for r in (0, 1)}
-            stacks = "\n".join("--- rank %d\n%s" % (r, open(tmp_path / ("stack%d.txt" % r)).read()[-3000:]) for r in (0, 1) if (tmp_path / ("stack%d.txt" % r)).exists())
-            pytest.fail("2-GPU workers hung; progress per rank: %r\n%s" % (prog, stacks))
-    a, b = np.load(tmp_path / "sharded.npz"), np.load(tmp_path / "single.npz")
-    assert sorted(a.files) == sorted(b.files)
-    c = np.load(tmp_path / "sharded_rs.npz")
-    d, e = np.load(tmp_path / "sharded_uneven.npz"), np.load(tmp_path / "sharded_empty.npz")
-    for k in a.files:
+    a, c, d, e, b = run(tmp_path, _ranks, mode="nccl", timeout=200)[0]
+    assert sorted(a) == sorted(b)
+    for k in a:
         assert np.array_equal(a[k], b[k]), k
         assert np.array_equal(c[k], b[k]), "reduce-scatter path: " + k
         assert np.array_equal(d[k], b[k]), "uneven shards, record path: " + k

@@ -3,20 +3,13 @@ both processes run the real kernels on cuda:0.  This exercises the global-row-ke
 weights, the all-reduced label scale and tree weights behind the label grid, the per-level int64 histogram all-reduce, the
 evaluator's all-reduced limb sums, the rank-wide label check and a rank whose shard is EMPTY walking every collective.  The
 models and metrics must be byte-identical to the single-process ones."""
-import os
-import socket
-import time
-import traceback
-
 import numpy as np
 import pytest
 import torch
 
+from ranks import block, run
+
 pytestmark = pytest.mark.gpu
-
-
-def _free_port():
-    s = socket.socket(); s.bind(("127.0.0.1", 0)); p = s.getsockname()[1]; s.close(); return p
 
 
 def _data(dev):
@@ -30,85 +23,48 @@ def _data(dev):
     return x, y, arity
 
 
-def _worker(rank, world, port, out_dir):
-    import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    torch.cuda.set_device(0)
-    dist.init_process_group("gloo", rank=rank, world_size=world)
+def _flat(rf, dt, m):
+    return dict(metrics=np.array([m[k] for k in sorted(m)]), **{"rf_" + k: v for k, v in rf.export().items()},
+                **{"dt_" + k: v for k, v in dt.export().items()})
+
+
+def _ranks(rank, grp, dev):
+    from b200flow import dist as bdist, metrics as bm, regression as br
+    x, y, arity = _data(dev)
+    n = x.shape[0]
+    lo, hi = bdist.shard_bounds(n, rank, 2)
+    p = br.RegressorParams(num_trees=4, max_depth=5, max_bins=16, subsampling_rate=0.8, seed=2019)
+    out = {}
+    for name, (a, b) in (("even", (lo, hi)), ("uneven", block(rank, 9000, n)), ("empty", block(rank, n, n))):
+        off, tot = bdist.global_offset(b - a, dev, grp)
+        assert tot == n and off == a
+        xs, ys = x[a:b].contiguous(), y[a:b].contiguous()
+        rf = br.fit_rf_regressor(xs, ys, arity, p, row_offset=off, group=grp)
+        dt = br.fit_dt_regressor(xs, ys, arity, p, row_offset=off, group=grp)
+        out[name] = _flat(rf, dt, bm.regression_metrics(ys, rf.predict(xs), group=grp))
+    # a NaN label on rank 1 only: both ranks refuse, none waits in a collective
+    yb = y[lo:hi].clone()
+    if rank == 1:
+        yb[5] = float("nan")
     try:
-        from b200flow import dist as bdist, metrics as bm, regression as br
-        dev = torch.device("cuda", 0)
-        x, y, arity = _data(dev)
-        n = x.shape[0]
-        grp = bdist.group()
-        lo, hi = bdist.shard_bounds(n, rank, world)
-        p = br.RegressorParams(num_trees=4, max_depth=5, max_bins=16, subsampling_rate=0.8, seed=2019)
-        out = {}
-        for name, (a, b) in (("even", (lo, hi)), ("uneven", (0, 9000) if rank == 0 else (9000, n)),
-                             ("empty", (0, n) if rank == 0 else (n, n))):
-            off, tot = bdist.global_offset(b - a, dev, grp)
-            assert tot == n and off == a
-            xs, ys = x[a:b].contiguous(), y[a:b].contiguous()
-            rf = br.fit_rf_regressor(xs, ys, arity, p, row_offset=off, group=grp)
-            dt = br.fit_dt_regressor(xs, ys, arity, p, row_offset=off, group=grp)
-            pred = rf.predict(xs)
-            m = bm.regression_metrics(ys, pred, group=grp)
-            out[name] = dict(rf=rf.export(), dt=dt.export(), metrics=np.array([m[k] for k in sorted(m)]))
-        # a NaN label on rank 1 only: both ranks refuse, none waits in a collective
-        yb = y[lo:hi].clone()
-        if rank == 1:
-            yb[5] = float("nan")
-        try:
-            br.fit_rf_regressor(x[lo:hi].contiguous(), yb, arity, p, row_offset=lo, group=grp)
-            refused = np.zeros(1)
-        except ValueError:
-            refused = np.ones(1)
-        np.save(os.path.join(out_dir, "refused%d.npy" % rank), refused)
-        if rank == 0:
-            for name, d in out.items():
-                np.savez(os.path.join(out_dir, name + ".npz"), metrics=d["metrics"],
-                         **{"rf_" + k: v for k, v in d["rf"].items()}, **{"dt_" + k: v for k, v in d["dt"].items()})
-        open(os.path.join(out_dir, "ok%d" % rank), "w").write("ok")
-    except Exception:
-        open(os.path.join(out_dir, "error%d.txt" % rank), "w").write(traceback.format_exc())
-        raise
-    finally:
-        try:
-            dist.destroy_process_group()
-        except Exception:
-            pass
+        br.fit_rf_regressor(x[lo:hi].contiguous(), yb, arity, p, row_offset=lo, group=grp)
+        refused = False
+    except ValueError:
+        refused = True
+    return out, refused
 
 
 def test_two_ranks_one_gpu_regression_equals_single_process(tmp_path):
-    import torch.multiprocessing as mp
-    ctx = mp.start_processes(_worker, args=(2, _free_port(), str(tmp_path)), nprocs=2, join=False, start_method="spawn")
-    deadline = time.time() + 300
-    failed = None
-    try:
-        while not ctx.join(timeout=5):
-            if time.time() > deadline:
-                failed = "workers hung"
-                break
-    except Exception as e:                                                    # a worker raised: its traceback is on file
-        failed = "worker failed: %s" % e
-    if failed:
-        for pr in ctx.processes:
-            if pr.is_alive():
-                pr.kill()
-        errs = "\n".join("--- rank %d\n%s" % (r, open(tmp_path / ("error%d.txt" % r)).read()) for r in (0, 1)
-                         if (tmp_path / ("error%d.txt" % r)).exists())
-        pytest.fail("%s\n%s" % (failed, errs))
+    (out, refused0), (_, refused1) = run(tmp_path, _ranks, timeout=300)
     from b200flow import metrics as bm, regression as br
     x, y, arity = _data(torch.device("cuda", 0))
     p = br.RegressorParams(num_trees=4, max_depth=5, max_bins=16, subsampling_rate=0.8, seed=2019)
     rf, dt = br.fit_rf_regressor(x, y, arity, p), br.fit_dt_regressor(x, y, arity, p)
-    m = bm.regression_metrics(y, rf.predict(x))
-    single = dict(metrics=np.array([m[k] for k in sorted(m)]), **{"rf_" + k: v for k, v in rf.export().items()},
-                  **{"dt_" + k: v for k, v in dt.export().items()})
+    single = _flat(rf, dt, bm.regression_metrics(y, rf.predict(x)))
     for name in ("even", "uneven", "empty"):
-        got = np.load(tmp_path / (name + ".npz"))
-        assert sorted(got.files) == sorted(single)
+        got = out[name]
+        assert sorted(got) == sorted(single)
         for k in single:
             assert np.array_equal(got[k].view(np.uint8), np.asarray(single[k]).view(np.uint8)), "%s shards: %s" % (name, k)
     assert (single["rf_is_leaf"] == 0).sum() > 20
-    assert [float(np.load(tmp_path / ("refused%d.npy" % r))[0]) for r in (0, 1)] == [1.0, 1.0]
+    assert [refused0, refused1] == [True, True]

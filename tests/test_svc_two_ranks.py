@@ -5,22 +5,16 @@ than one chunk and an empty shard.  An invalid label on one rank makes both rais
 shard is empty or holds only label 0 decides numClasses as the other does: the fit equals one process, and a label set
 that is not binary overall makes both ranks raise.  Two gloo ranks share one GPU; the NCCL
 case needs two GPUs and is skipped otherwise."""
-import json
-import os
-import time
-import traceback
-
 import numpy as np
 import pytest
 import torch
 
-from test_tuning_two_ranks import _free_port
+from ranks import SPLITS, block, run, two_gpus
 
 pytestmark = pytest.mark.gpu
 
 N = 30000
 D, K = 41, 5
-SPLITS = {"even": 15000, "uneven": 11000, "short_first": 2500, "short_last": 28000, "empty_last": N, "empty_first": 0}
 
 
 def _data():
@@ -101,72 +95,39 @@ def _shim_run(x, y, lo, hi, how, dev):
     return {"coef": _hex(f.coef), "b": float(f.intercept).hex(), "hist": _hex(f.objective_history), "it": f.iterations}
 
 
-def _worker(rank, world, port, out_dir, backend):
-    import torch.distributed as dist
-    os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port), RANK=str(rank), WORLD_SIZE=str(world))
-    gpu = rank if backend == "nccl" else 0
-    torch.cuda.set_device(gpu)
-    kw = {"device_id": torch.device("cuda", gpu)} if backend == "nccl" else {}
-    dist.init_process_group(backend, rank=rank, world_size=world, **kw)
-    try:
-        x, y = _data()
-        res = {}
-        for name, cut in SPLITS.items():
-            lo, hi = (0, cut) if rank == 0 else (cut, N)
-            res[name] = _run(x[lo:hi], y[lo:hi], torch.device("cuda", gpu), dist.group.WORLD)
-        xs, ys, n0 = _shim_data()
-        res["shim"] = {}
-        for name, (cut, how) in _shim_cases(n0).items():
-            lo, hi = (0, cut) if rank == 0 else (cut, N)
-            res["shim"][name] = _shim_run(xs, ys, lo, hi, how, torch.device("cuda", gpu))
-        open(os.path.join(out_dir, "res%d.json" % rank), "w").write(json.dumps(res))
-    except Exception:
-        open(os.path.join(out_dir, "error%d.txt" % rank), "w").write(traceback.format_exc())
-        raise
-    finally:
-        try:
-            dist.destroy_process_group()
-        except Exception:
-            pass
-
-
-def _two_ranks(tmp_path, backend):
-    import torch.multiprocessing as mp
-    ctx = mp.start_processes(_worker, args=(2, _free_port(), str(tmp_path), backend), nprocs=2, join=False, start_method="spawn")
-    deadline = time.time() + 600
-    failed = None
-    try:
-        while not ctx.join(timeout=5):
-            if time.time() > deadline:
-                failed = "workers hung"
-                break
-    except Exception as e:
-        failed = "worker failed: %s" % e
-    if failed:
-        for pr in ctx.processes:
-            if pr.is_alive():
-                pr.kill()
-        errs = "\n".join("--- rank %d\n%s" % (r, open(tmp_path / ("error%d.txt" % r)).read()) for r in (0, 1)
-                         if (tmp_path / ("error%d.txt" % r)).exists())
-        pytest.fail("%s\n%s" % (failed, errs))
+def _ranks(rank, grp, dev):
     x, y = _data()
-    want = json.loads(json.dumps(_run(x, y, torch.device("cuda", 0), None)))
+    res = {}
+    for name, cut in SPLITS(N).items():
+        lo, hi = block(rank, cut, N)
+        res[name] = _run(x[lo:hi], y[lo:hi], dev, grp)
+    xs, ys, n0 = _shim_data()
+    res["shim"] = {}
+    for name, (cut, how) in _shim_cases(n0).items():
+        lo, hi = block(rank, cut, N)
+        res["shim"][name] = _shim_run(xs, ys, lo, hi, how, dev)
+    return res
+
+
+def _two_ranks(tmp_path, mode):
+    got = run(tmp_path, _ranks, mode=mode)
+    x, y = _data()
+    want = _run(x, y, torch.device("cuda", 0), None)
     xs, ys, n0 = _shim_data()
     want_shim = {name: _shim_run(xs, ys, 0, N, how, torch.device("cuda", 0)) for name, (_, how) in _shim_cases(n0).items()}
     assert want_shim["one_class"] == {"raised": "LinearSVC only supports binary classification. 1 classes detected in label"}
     assert want_shim["three_classes"]["raised"].startswith("LinearSVC only supports binary classification. 3 classes")
     for rank in (0, 1):
-        got = json.loads(open(tmp_path / ("res%d.json" % rank)).read())
-        for name in SPLITS:
-            assert got[name] == want, (rank, name)
+        for name in SPLITS(N):
+            assert got[rank][name] == want, (rank, name)
         for name in want_shim:
-            assert got["shim"][name] == want_shim[name], (rank, name)
+            assert got[rank]["shim"][name] == want_shim[name], (rank, name)
 
 
 def test_svc_two_gloo_ranks_equal_one_process(tmp_path):
     _two_ranks(tmp_path, "gloo")
 
 
-@pytest.mark.skipif(not torch.cuda.is_available() or torch.cuda.device_count() < 2, reason="needs two GPUs")
+@two_gpus
 def test_svc_two_nccl_ranks_equal_one_process(tmp_path):
     _two_ranks(tmp_path, "nccl")

@@ -3,6 +3,7 @@ import numpy as np
 import torch
 
 import oracle
+from b200flow import dist as bdist
 from b200flow import encode as enc
 from b200flow import synth
 
@@ -15,11 +16,15 @@ def kdd_luts_oracle(rec_np, schema, dicts):
     return luts, ordered
 
 
-def kdd_luts_gpu(rec, schema, dicts):
+def kdd_luts_gpu(rec, schema, dicts, group=None):
+    """with a process group, every rank counts its own rows and the counts are summed over the group, so every rank
+    orders the categories as one process holding all the rows would"""
     luts, ordered = {}, {}
     for col in synth.KDD_CATEGORICAL + ["label"]:
-        counts = enc.category_counts(rec, schema, col, len(dicts[col])).cpu().numpy()
-        ordered[col], luts[col] = enc.string_index_order(counts, dicts[col])
+        counts = enc.category_counts(rec, schema, col, len(dicts[col]))
+        if group is not None:
+            bdist.all_reduce_sum_(counts, group)
+        ordered[col], luts[col] = enc.string_index_order(counts.cpu().numpy(), dicts[col])
     return luts, ordered
 
 
