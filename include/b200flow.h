@@ -753,6 +753,32 @@ int b200flow_group_centered_moments(const double* x, int64_t n_rows, int32_t W, 
                                     const double* centers, const double* y, double y_center, int64_t row_offset,
                                     double* partials, void* stream);
 
+/* ---------------------------------------------------------------- naive Bayes ---
+ * NaiveBayes (multinomial, complement, bernoulli, gaussian), DESIGN.md §5u.  Features x [n_rows][ld] are dense row-major,
+ * f32 (x_dtype 0) or f64 (x_dtype 1), widened exactly to f64; 1 <= D <= 256 and 1 <= C <= 256 classes.
+ * b200flow_nb_moments: rows [0, n_rows) are global rows row_offset + i with class labels[i] (rows whose label is outside
+ * [0, C) are left out) and weight weights[i] (NULL: 1.0).  For each 4096-row global chunk they touch (n_chunks =
+ * b200flow_group_sums_chunks(row_offset, n_rows)), partials (device):
+ *   centers NULL:      [n_chunks][C][D + 1], [c][j] = sum w x_j and [c][D] = sum w over the chunk's rows of class c;
+ *   centers [C + 1][D]: [n_chunks][C + 1][D], [c][j] = sum w (x_j - centers[c][j])^2 over the rows of class c and
+ *                      [C][j] = sum w (x_j - centers[C][j])^2 over every row with a label in [0, C).
+ * Each sum runs over the rows in row order from +0.0 without FMA, w (t t) for a centred term.  bad int64 [5] (optional,
+ * caller zeroes; counted by the pass without centers only) += the number of values x that are {non-finite, negative, not 0
+ * or 1}, of weights that are negative, NaN or infinite, and of labels outside [0, C). */
+int b200flow_nb_moments(const void* x, int32_t x_dtype, int64_t n_rows, int32_t D, int64_t ld, const int32_t* labels,
+                        const double* weights, int32_t C, const double* centers, int64_t row_offset, double* partials,
+                        int64_t* bad, void* stream);
+/* b200flow_nb_raw: raw [n_rows][C] (device f64); each value is one sum over j in feature order from 0.0, without FMA:
+ *   model 0 (gaussian): raw[i][c] = c0[c] - (s + c1[c]) / 2, s = sum (d d) / b[c][j], d = x_j - a[c][j];
+ *   model 1 (linear):   raw[i][c] = sum x_j a[c][j], then + c0[c];
+ *   model 2:            model 1, then raw[i][c] -= m + log(sum over the present classes in class order of exp(raw[i][c] - m)),
+ *                       m the row's largest present value.
+ * a, b [C][D], c0, c1 [C] (device f64; b and c1 gaussian only); classes with present[c] == 0 get -inf.  bad int64 [1]
+ * (optional, caller zeroes) += the number of values x that are not exactly 0 or 1. */
+int b200flow_nb_raw(const void* x, int32_t x_dtype, int64_t n_rows, int32_t D, int64_t ld, int32_t model, const double* a,
+                    const double* b, const double* c0, const double* c1, const uint8_t* present, int32_t C, double* raw,
+                    int64_t* bad, void* stream);
+
 /* ------------------------------------------------------- gradient-boosted trees ---
  * GBTClassifier (binary, LogLoss), DESIGN.md §5e.  The regression trees reuse the forest's level loop: feature_subsets,
  * partition_level, next_segments, grow_level (with C = 6: a node's int64 stats {Σw, Σw·q, Σw·q2} travel as six opaque

@@ -15,9 +15,12 @@ FMClassifier runs on the fused fp64 tensor-core factorization-machine kernel (b2
 OneVsRest(FMClassifier) trains its K models together, one kernel pass per gradient-descent iteration, each the same bits
 as its standalone fit, and its transform computes the K raw values in one launch.  Both are the same bits for any number
 of ranks.
-LogisticRegression and NaiveBayes (kdd99.py:57,67; cicids17.py:61,71) are OUT of the kernel scope (SURVEY.md
-§8f rank 4): torch fp64 implementations of MLlib's statistics / objective (b200flow/linear.py), checked against a numpy
-restatement and scikit-learn in tests/test_linear_models.py.
+NaiveBayes (kdd99.py:67; cicids17.py:71) fits complement, bernoulli and gaussian models, and any model with weightCol, on
+the class-moment and scoring kernels of csrc/naive_bayes.cu (b200flow/naive_bayes.py, DESIGN.md §5u), the same bits for any
+number of ranks; the unweighted multinomial fit and every multinomial transform stay torch fp64 (b200flow/linear.py).
+LogisticRegression (kdd99.py:57; cicids17.py:61) is OUT of the kernel scope (SURVEY.md §8f rank 4): a torch fp64
+implementation of MLlib's objective (b200flow/linear.py), checked against a numpy restatement and scikit-learn in
+tests/test_linear_models.py.
 """
 import zlib
 
@@ -29,6 +32,7 @@ from b200flow import forest as fr
 from b200flow import fm as _fm
 from b200flow import linear as _linear
 from b200flow import mlp as _mlp
+from b200flow import naive_bayes as _nb
 from b200flow import svc as _svc
 
 from . import Estimator, Model, Pipeline
@@ -359,21 +363,37 @@ class LogisticRegressionModel(_ProbModel):
 
 
 class NaiveBayes(Estimator):
-    """Multinomial naive Bayes with MLlib's smoothed prior and likelihood (b200flow/linear.py; kdd99.py:67, cicids17.py:71);
-    rejects negative features as MLlib does (the reason for the where-filters at cicids17.py:30-35)."""
-    _defaults = dict(_ProbModel._defaults, smoothing=1.0, modelType="multinomial")
+    """Naive Bayes with Spark 3's four model types (kdd99.py:67, cicids17.py:71).  The unweighted multinomial fit is
+    b200flow/linear.py's torch fit; complement, bernoulli, gaussian and any fit with weightCol run on the class-moment and
+    scoring kernels of csrc/naive_bayes.cu (b200flow/naive_bayes.py, DESIGN.md §5u).  multinomial and complement reject
+    negative features as Spark does (the reason for the where-filters at cicids17.py:30-35); gaussian takes them."""
+    _defaults = dict(_ProbModel._defaults, smoothing=1.0, modelType="multinomial", weightCol=None)
 
     def __init__(self, featuresCol=None, labelCol=None, predictionCol=None, probabilityCol=None, rawPredictionCol=None,
-                 smoothing=None, modelType=None):
+                 smoothing=None, modelType=None, weightCol=None):
         kw = dict(locals()); kw.pop("self"); kw.pop("__class__", None)
         super().__init__(**kw)
 
     def _fit(self, df):
-        if self.getOrDefault("modelType") != "multinomial":
-            raise IllegalArgumentException("only modelType='multinomial' is implemented")
+        g = self.getOrDefault
+        model_type, wcol = g("modelType"), g("weightCol")
+        if model_type not in _nb.MODEL_TYPES:
+            raise IllegalArgumentException("modelType must be one of %s, got %r" % (", ".join(_nb.MODEL_TYPES), model_type))
+        try:
+            smoothing = float(g("smoothing"))
+        except (TypeError, ValueError):
+            raise IllegalArgumentException("smoothing must be a number >= 0, got %r" % (g("smoothing"),))
+        if not smoothing >= 0.0:
+            raise IllegalArgumentException("smoothing must be >= 0, got %r" % (g("smoothing"),))
+        if wcol and wcol not in df._cols:
+            raise IllegalArgumentException("Field \"%s\" does not exist." % wcol)
         x, y, C, _ = _features_and_labels(df, self)
         try:
-            fit = _linear.nb_fit(x, y, C, float(self.getOrDefault("smoothing")), group=bdist.group())
+            if model_type == "multinomial" and not wcol:
+                fit = _linear.nb_fit(x, y, C, smoothing, group=bdist.group())
+            else:
+                w = df._column_tensor(wcol) if wcol else None
+                fit = _nb.nb_fit(x, y, C, model_type, smoothing, weights=w, group=bdist.group())
         except ValueError as e:
             raise IllegalArgumentException(str(e))
         m = NaiveBayesModel(fit, C)
@@ -382,6 +402,8 @@ class NaiveBayes(Estimator):
 
 
 class NaiveBayesModel(_ProbModel):
+    _defaults = dict(_ProbModel._defaults, smoothing=1.0, modelType="multinomial", weightCol=None)
+
     def __init__(self, fit, C):
         super().__init__()
         self._fit_result, self.numClasses = fit, C
@@ -394,8 +416,21 @@ class NaiveBayesModel(_ProbModel):
     def theta(self):
         return self._fit_result.theta.cpu().numpy()
 
+    @property
+    def sigma(self):
+        """the gaussian variances [C, D]; an empty [0, 0] matrix for the other model types, as in Spark."""
+        sigma = getattr(self._fit_result, "sigma", None)
+        return sigma.cpu().numpy() if sigma is not None else np.zeros((0, 0))
+
     def _transform(self, df):
-        raw = _linear.nb_raw(self._fit_result, df._cols[self.getOrDefault("featuresCol")].data)
+        x = df._cols[self.getOrDefault("featuresCol")].data
+        if self.getOrDefault("modelType") == "multinomial":
+            raw = _linear.nb_raw(self._fit_result, x)
+        else:
+            try:
+                raw = _nb.nb_raw(self._fit_result, x)
+            except ValueError as e:
+                raise IllegalArgumentException(str(e))
         return self._emit(df, raw, torch.softmax(raw, 1))
 
 
